@@ -22,8 +22,8 @@ sanitize:
 
 sass:
 	$(PYTHON) tools/dump_sass.py
-	$(PYTHON) tools/sass_census.py > profiles/sass_census.txt
-	$(PYTHON) tools/resource_usage.py > profiles/resource_usage.txt
+	$(PYTHON) tools/sass_census.py
+	$(PYTHON) tools/resource_usage.py
 
 bench:
 	$(PYTHON) bench.py --gpus 1 --steps 50 --warmup 10

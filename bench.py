@@ -39,8 +39,10 @@ def parse_args():
   p.add_argument("--warmup", type=int, default=10)
   p.add_argument("--impl", default="b200", choices=["b200", "reference"])
   p.add_argument("--global-batch", type=int, default=65536)
-  p.add_argument("--model", default="dlrm-mlperf",
-                 help="dlrm-mlperf | dlrm-small (26x100000) | dlrm-tiny (26x1000)")
+  p.add_argument("--model", default="dlrm-mlperf-20m",
+                 help="dlrm-mlperf-20m (MLPerf tables capped at 20M rows: 49.6 GiB fp32, fits one "
+                 "80 GB H100) | dlrm-mlperf (40M cap: 89.5 GiB, needs 2+ GPUs) | dlrm-small "
+                 "(26x100000) | dlrm-tiny (26x1000)")
   p.add_argument("--backend", default="fused", choices=["fused", "torch"])
   p.add_argument("--optimizer", default="sgd")
   p.add_argument("--dtype", default="bf16", choices=["bf16", "fp32"])
@@ -49,8 +51,7 @@ def parse_args():
   p.add_argument("--no-e2e", action="store_true")
   p.add_argument("--column-slice-threshold", default="auto",
                  help="elements, 'none', or 'auto' (default) = balance the looked-up columns per "
-                 "rank with slices >= 64 wide: 2^32 at 8 GPUs, no slicing at 1-4 (measured "
-                 "0.657 vs 0.662 ms at 8 GPUs)")
+                 "rank with slices >= 64 wide: 2^32 at 8 GPUs, no slicing at 1-4")
   p.add_argument("--data-parallel-threshold", default="auto",
                  help="replicate tables with at most this many elements (the reference's "
                  "data_parallel_threshold): 'none', a number, or 'auto' (default) = 2500 rows x "
@@ -71,6 +72,9 @@ def parse_args():
   p.add_argument("--alpha", type=float, default=0.0,
                  help="power-law exponent of the synthetic ids (0 = uniform; the reference's "
                       "synthetic benchmark uses 1.05)")
+  p.add_argument("--dump-outputs", default=None, metavar="DIR",
+                 help="after the timed steps, write what the last timed step computed (rank 0) "
+                      "as DIR/<name>.npy: see dump_outputs()")
   p.add_argument("--no-verify", action="store_true",
                  help="skip the pre-flight numerics check (2 steps of a 1/1000-rows plan on all "
                       "ranks vs a single-process fp32 PyTorch oracle on rank 0)")
@@ -167,6 +171,8 @@ def table_sizes_for(model: str):
   from distributed_embeddings_b200.models.dlrm import mlperf_table_sizes
   if model == "dlrm-mlperf":
     return mlperf_table_sizes()
+  if model == "dlrm-mlperf-20m":
+    return mlperf_table_sizes(max_rows=20_000_000)
   if model == "dlrm-full":
     return [s + 1 for s in CRITEO_1TB_FULL_SIZES]
   if model == "dlrm-small":
@@ -210,6 +216,48 @@ def gen_ids(rows: int, n: int, alpha: float, gen):
   g = 1.0 - alpha
   y = (r * ((rows + 1.0)**g - 1.0) + 1.0)**(1.0 / g)
   return (y.to(torch.int64) - 1).clamp_(0, rows - 1).to(torch.int32)
+
+
+def dump_outputs(out_dir, model, loss, max_bytes=64 << 20):
+  """What a caller of the timed training step receives, as float32 .npy files: the step's loss
+  (``loss``), the updated dense parameters (``bottom_mlp_<i>_weight`` / ``_bias``, ``top_mlp_...``)
+  and the updated embedding rows of this rank's part of every table ``t`` (``embedding_<t>``, with
+  ``_col<c>`` / ``_row<r>`` for column / row slices): all rows of a part with at most 1024 rows,
+  else 1024 rows drawn with a generator seeded by ``t``, so the same rows are sampled in every
+  run."""
+  import numpy as np
+  import torch
+  os.makedirs(out_dir, exist_ok=True)
+  arrays = {"loss": loss.detach().float().reshape(-1)}
+  for part in ("bottom_mlp", "top_mlp"):
+    lins = [m for m in getattr(model, part).net if isinstance(m, torch.nn.Linear)]
+    for i, lin in enumerate(lins):
+      arrays[f"{part}_{i}_weight"] = lin.weight.detach().float()
+      arrays[f"{part}_{i}_bias"] = lin.bias.detach().float()
+  # local tables of the same width are fused into one tensor: cut it back into the plan's tables
+  emb, st = model.embedding, model.embedding.strategy
+  weights = emb.weights
+  n_dp, n_col = len(emb.dp_layers), len(emb.local_embedding_layers)
+  parts = [(t, f"embedding_{t}", w) for t, w in zip(st.table_groups[0], weights[:n_dp])]
+  for s in st.shards[emb.rank]:
+    t = st.table_groups[1][s.table]
+    full = s.width == int(st.global_configs[t]["output_dim"])
+    name = f"embedding_{t}" if full else f"embedding_{t}_col{s.col_start}"
+    parts.append((t, name, weights[n_dp + s.local_table][s.row_offset:s.row_offset + s.rows]))
+  for gt, t in enumerate(st.table_groups[2]):
+    parts.append((t, f"embedding_{t}_row{emb.rank}", weights[n_dp + n_col + gt]))
+  for t, name, w in parts:
+    w = w.detach()
+    if w.shape[0] > 1024:
+      g = torch.Generator().manual_seed(t)
+      w = w[torch.randint(0, w.shape[0], (1024,), generator=g).to(w.device)]
+    arrays[name] = w.float()
+  total = sum(a.numel() * 4 for a in arrays.values())
+  if total > max_bytes:
+    raise ValueError(f"--dump-outputs: {total} bytes exceed the {max_bytes}-byte budget")
+  for name, a in arrays.items():
+    np.save(os.path.join(out_dir, name + ".npy"), a.cpu().numpy().astype(np.float32))
+  return total
 
 
 def verify(args, device, world, rank, compute_dtype, cst_for):
@@ -327,9 +375,10 @@ def verify(args, device, world, rank, compute_dtype, cst_for):
     # The trainer computes the dense side in bf16: against the fp32 oracle the two-step table
     # update agrees to ~10 % (aggregate L2; bf16 has 8 mantissa bits and the error compounds
     # through 9 layers and the second step), against the same plain-PyTorch code under bf16
-    # autocast to 4-9 % (measured; the hand-written kernels round at other places than
-    # autocast does).  A wrong routing / missing rank contribution / wrong gradient scale shows
-    # up as an error of the order of the update itself (~1.0) against both.
+    # autocast to a few % (the hand-written kernels round at other places than autocast does;
+    # the values of a run are in its JSON line's "verify" key).  A wrong routing / missing rank
+    # contribution / wrong gradient scale shows up as an error of the order of the update itself
+    # (~1.0) against both.
     tabs32, ol32 = oracle(None)
     tabs16, ol16 = oracle(compute_dtype if compute_dtype != torch.float32 else None)
     e32, u32, r32 = compare(tabs32)
@@ -526,12 +575,14 @@ def main():
       dist.barrier()
       torch.cuda.synchronize()
 
+  last_out = [None]
+
   def timed(fn, steps):
     sync_all()
     start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     start.record()
     for i in range(steps):
-      fn(i)
+      last_out[0] = fn(i)
     end.record()
     sync_all()
     ms = torch.tensor([start.elapsed_time(end)], device=device)
@@ -546,6 +597,8 @@ def main():
     sampler.start()
   _native.reset_launch_count()
   total_ms = timed(step_from_device, args.steps)
+  if args.dump_outputs and rank == 0:
+    dump_outputs(args.dump_outputs, model, last_out[0])
   launches = _native.launch_count()
   if use_fast and args.cuda_graph:
     # kernels replayed from the captured graph are not seen by the python-side counter:
@@ -641,7 +694,7 @@ def main():
             "optimizer": f"{args.optimizer} lr={args.lr}, warm-up 8000 / decay from 48000 steps "
                          "like the reference (embedding update fused in backward)",
             "l2_policy": "inputs larger than L2: random rows of "
-                         f"{table_gb / world:.1f} GiB tables per GPU vs 126 MB L2",
+                         f"{table_gb / world:.1f} GiB tables per GPU vs 50 MB L2",
         },
         "clocks": clocks,
         "e2e": e2e,

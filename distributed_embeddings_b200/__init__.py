@@ -1,4 +1,4 @@
-"""B200-native distributed embeddings.
+"""H100-native (sm_90a) distributed embeddings.
 
 Public API (capability parity with ``distributed_embeddings/__init__.py:17-27`` of the reference):
 ``Embedding``, ``IntegerLookup``, ``ConcatOneHotEmbedding``, ``embedding_lookup``,

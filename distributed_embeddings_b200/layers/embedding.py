@@ -41,7 +41,7 @@ class Embedding(nn.Module):
     output_dim: embedding width.
     embeddings_initializer: Keras-style identifier, :class:`Initializer` or callable.
     combiner: ``None`` | ``'sum'`` | ``'mean'``.
-    use_custom_kernel: run the sm_100a kernels (True) or the library path (False).
+    use_custom_kernel: run the sm_90a kernels (True) or the library path (False).
     sparse_grad: parameter gradient as a deduplicated sparse tensor (reference semantics).
 
   With a combiner the supported inputs / outputs are: N-D tensor ``(d1..dn)`` ->

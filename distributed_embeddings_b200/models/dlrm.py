@@ -25,8 +25,10 @@ CRITEO_1TB_MLPERF_SIZES = [
 ]
 
 
-def mlperf_table_sizes() -> List[int]:
-  return [s + 1 for s in CRITEO_1TB_MLPERF_SIZES]
+def mlperf_table_sizes(max_rows: int = 40_000_000) -> List[int]:
+  """Table sizes of the MLPerf configuration; ``max_rows`` below 40M caps the tables further, the
+  way a smaller ``max_ind_range`` does (20M: 104 M rows, 49.6 GiB fp32 at dim 128)."""
+  return [min(s, max_rows) + 1 for s in CRITEO_1TB_MLPERF_SIZES]
 
 
 class MLP(nn.Module):

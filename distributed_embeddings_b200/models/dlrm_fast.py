@@ -8,7 +8,7 @@ math as one static schedule over preallocated buffers:
   SGD + re-cast + gradient zeroing); gradients live in one flat buffer (symmetric memory when
   world > 1) that the one-shot NVLink all-reduce kernel reduces in place;
 * MLP layers: cuBLASLt bf16 GEMMs with fused bias+ReLU epilogues forward, plain GEMMs backward
-  (K padded 13->16 and 479->480 so the tcgen05 library kernels are eligible), fused
+  (K padded 13->16 and 479->480 so every layer meets the TMA alignment rules of the GEMM kernels), fused
   ReLU-backward+bias-gradient kernel;
 * dot interaction forward/backward: tensor-core kernels; the forward's head waits for the
   embedding owners' "output ready" signals, the backward pushes every piece of the embedding
@@ -62,9 +62,9 @@ class DLRMTrainStep:
     if gemm not in ("cublas", "fused_dgrad", "tcgen05", "tcgen05_pair"):
       raise ValueError("gemm must be cublas | fused_dgrad | tcgen05 | tcgen05_pair")
     # cublas: cuBLASLt everywhere.  fused_dgrad: forward/wgrad on cuBLASLt, dgrad on the
-    # first-party tcgen05 kernel with the ReLU-backward mask + bias gradient fused in its epilogue.
+    # first-party wgmma kernel with the ReLU-backward mask + bias gradient fused in its epilogue.
     # tcgen05: forward layers on the first-party kernel as well.  tcgen05_pair: same, with the
-    # CTA-pair (cta_group::2) kernel for layers at least 256 wide.
+    # 2-CTA cluster kernel for layers at least 256 wide.  (The option names are historical.)
     self.gemm = gemm
     self.model = model
     self.emb = model.embedding
@@ -85,9 +85,8 @@ class DLRMTrainStep:
     self.dim = model.embedding_dim
     # gradient all-to-all through local staging + a streaming copy kernel next to the interaction
     # backward (DE_B200_STREAM_PUSH=0: the interaction backward stores into peer memory itself)
-    # measured: 0.705 vs 0.738 ms per step at 8 GPUs with it, but 1.41 vs 1.33 ms at 2 GPUs (the
-    # copy kernel then competes with an interaction backward that keeps every SM busy), hence
-    # on from 4 GPUs; DE_B200_STREAM_PUSH=0/1 overrides
+    # on from 4 GPUs: at 2 GPUs the copy kernel competes with an interaction backward that keeps
+    # every SM busy (not measured on H100); DE_B200_STREAM_PUSH=0/1 overrides
     sp_env = os.environ.get("DE_B200_STREAM_PUSH", "auto")
     self._stream_push = self.world > 1 and (sp_env == "1" or (sp_env == "auto" and self.world >= 4))
     self._push_stream = torch.cuda.Stream(device=self.dev) if self._stream_push else None
@@ -104,7 +103,7 @@ class DLRMTrainStep:
     # replicated (data-parallel) embedding tables live in the flat dense buffers too: their
     # local-batch gradient is scattered into the gradient bucket, all-reduced with the MLP
     # gradients and applied by the same fused SGD kernel.  They come first so that they belong to
-    # the bucket that is reduced last (DE_B200_AR_OVERLAP).  Validated on 2 and 8 GPUs
+    # the bucket that is reduced last (DE_B200_AR_OVERLAP).  Covered by the 2- and 8-GPU tests
     # (tests/test_dist_gpu.py: replicated-table cases); bench.py replicates the < 2500-row tables.
     self._dp_slots = []
     pos = 0
@@ -171,9 +170,9 @@ class DLRMTrainStep:
     self._side = torch.cuda.Stream(device=dev) if overlap else None
     # weight-gradient GEMMs are off the critical path (head -> dgrads -> interaction -> embedding
     # backward): they run on a second side stream and join before the all-reduce
-    # (measured: +1.5 % at local batch 65536, but at small local batches the full-GPU cuBLAS
-    # kernels of the two streams interleave and stretch the critical chain: 0.66 -> 0.81 ms at 8
-    # GPUs, so it is only enabled for large local batches; DE_B200_WGRAD_STREAM=0/1 overrides)
+    # (at small local batches the full-GPU cuBLAS kernels of the two streams interleave and
+    # stretch the critical chain, so it is only enabled for large local batches; not measured on
+    # H100; DE_B200_WGRAD_STREAM=0/1 overrides)
     self._wgrad_overlap = os.environ.get("DE_B200_WGRAD_STREAM", "auto")
     self._wstream = torch.cuda.Stream(device=dev) if overlap else None
     # The top-MLP + head gradients (93 % of the dense parameters, complete as soon as the top MLP
@@ -183,8 +182,8 @@ class DLRMTrainStep:
     # cannot starve the kernels the peers wait for.  DE_B200_AR_OVERLAP=0/1 overrides the default
     # (on from 4 GPUs).
     ar_env = os.environ.get("DE_B200_AR_OVERLAP", "auto")
-    # measured: +1 % at 8 GPUs, -4 % at 2 GPUs (there the large local batch keeps every SM busy
-    # and the overlapped kernel only steals from the interaction backward)
+    # off at 2 GPUs: the large local batch keeps every SM busy and the overlapped kernel only
+    # steals from the interaction backward (not measured on H100)
     ar_on = ar_env == "1" or (ar_env == "auto" and self.world >= 4)
     self._ar_stream = torch.cuda.Stream(device=dev) if (overlap and self.world > 1 and ar_on) \
         else None

@@ -1,6 +1,6 @@
 """In-tree build of the native extension (``distributed_embeddings_b200/_C.so``).
 
-Kernels are compiled with nvcc for sm_100a only (``-gencode arch=compute_100a,code=sm_100a``);
+Kernels are compiled with nvcc for sm_90a only (``-gencode arch=compute_90a,code=sm_90a``);
 the torch bindings are compiled with the host compiler so the CUDA files never include torch
 headers (seconds per file).  The resulting shared object is loaded with
 ``torch.ops.load_library`` - there is no JIT step at import time, the .so travels with the tree.
@@ -24,10 +24,10 @@ BUILD_DIR = os.path.join(PKG_DIR, "ops", "_build")
 SO_PATH = os.path.join(PKG_DIR, "_C.so")
 
 CU_SOURCES = ["lookup_kernels.cu", "sparse_update_kernels.cu", "misc_kernels.cu", "comm_kernels.cu",
-              "dense_kernels.cu", "gemm_tcgen05.cu", "radix_sort.cu"]
+              "dense_kernels.cu", "gemm_wgmma.cu", "radix_sort.cu"]
 CPP_SOURCES = ["bindings.cpp"]
 
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def _nvcc() -> str:
@@ -66,7 +66,7 @@ def _run(cmd: List[str]):
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-  """Compile every CUDA/C++ source for sm_100a and link ``_C.so``.  Returns the .so path."""
+  """Compile every CUDA/C++ source for sm_90a and link ``_C.so``.  Returns the .so path."""
   os.makedirs(BUILD_DIR, exist_ok=True)
   cu = [os.path.join(CSRC, s) for s in CU_SOURCES if os.path.exists(os.path.join(CSRC, s))]
   cpp = [os.path.join(CSRC, s) for s in CPP_SOURCES]

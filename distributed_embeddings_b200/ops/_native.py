@@ -1,4 +1,4 @@
-"""Loader for the native sm_100a extension and numpy mirrors of its descriptor structs."""
+"""Loader for the native sm_90a extension and numpy mirrors of its descriptor structs."""
 from __future__ import annotations
 
 import os
@@ -72,7 +72,7 @@ def load(required: bool = False) -> bool:
       if not os.path.exists(SO_PATH):
         raise FileNotFoundError(
             f"{SO_PATH} is missing - run `python -m distributed_embeddings_b200.ops._build` "
-            "(or `make`) to compile the sm_100a kernels")
+            "(or `make`) to compile the sm_90a kernels")
       torch.ops.load_library(SO_PATH)
       sizes = list(torch.ops.de_b200.struct_sizes())
       mine = [INPUT_DESC.itemsize, TABLE_DESC.itemsize, MAX_PEERS, GRAD_ROUTE.itemsize,
@@ -144,7 +144,7 @@ def require():
   global _proxy
   if not load(required=False):
     raise RuntimeError(
-        "distributed_embeddings_b200: the native sm_100a extension is required for CUDA tensors "
+        "distributed_embeddings_b200: the native sm_90a extension is required for CUDA tensors "
         f"but could not be loaded ({_error!r}). There is no eager fallback on GPU.")
   if _proxy is None:
     _proxy = _OpsProxy(torch.ops.de_b200)

@@ -890,7 +890,7 @@ void cast_pad(const Tensor& src, Tensor dst) {
   check_launch();
 }
 
-// out[M,N] = act(a[M,K] @ b[N,K]^T + bias) on the hand-written tcgen05 kernel
+// out[M,N] = act(a[M,K] @ b[N,K]^T + bias) on the hand-written wgmma kernel
 void gemm_tn_bias_act(const Tensor& a, const Tensor& b, const c10::optional<Tensor>& bias,
                       Tensor out, bool relu, int64_t block_n) {
   check_bf16_2d(a, "a");

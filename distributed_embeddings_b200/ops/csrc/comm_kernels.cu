@@ -1,4 +1,4 @@
-// NVLink / NVSwitch communication kernels for sm_100a: flag barrier over peer-mapped signal pads
+// NVLink / NVSwitch communication kernels for sm_90a: flag barrier over peer-mapped signal pads
 // and the dense-gradient all-reduce (the data-parallel half of hybrid parallelism) as a single
 // kernel: reduce-scatter + all-gather over peer memory, fused with the 1/world scale and the
 // bf16/fp32 handling, either with plain P2P loads/stores or with NVSwitch multicast
@@ -637,7 +637,7 @@ void launch_copy_cast_2d(const void* src, int64_t src_stride, void* dst, int64_t
         ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0) {
       const int64_t n = rows * (cols / per16);
       int64_t blocks = (n + 255) / 256;
-      if (blocks > 148 * 16) blocks = 148 * 16;
+      if (blocks > kGridCapSms * 16) blocks = kGridCapSms * 16;
       copy_2d_vec16_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
           reinterpret_cast<const uint4*>(src), src_stride / per16, reinterpret_cast<uint4*>(dst),
           dst_stride / per16, rows, cols / per16);
@@ -646,7 +646,7 @@ void launch_copy_cast_2d(const void* src, int64_t src_stride, void* dst, int64_t
   }
   const int threads = 256;
   int64_t blocks = (rows * cols + threads - 1) / threads;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > kGridCapSms * 8) blocks = kGridCapSms * 8;
 #define DE_CC(S, D)                                                                              \
   copy_cast_2d_kernel<S, D><<<static_cast<unsigned>(blocks), threads, 0, stream>>>(              \
       reinterpret_cast<const S*>(src), src_stride, reinterpret_cast<D*>(dst), dst_stride, rows,  \
@@ -755,7 +755,7 @@ void launch_rowslice_reduce(const float* partial, int world, int64_t rows, int64
   const int total_width = static_cast<int>(part_stride);
   const int64_t n = rows * total_width;
   int64_t blocks = (n + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > kGridCapSms * 8) blocks = kGridCapSms * 8;
   if (out_dtype == 1)
     rowslice_reduce_kernel<__nv_bfloat16><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
         partial, world, rows, part_stride, reinterpret_cast<__nv_bfloat16*>(out), out_stride, cols,

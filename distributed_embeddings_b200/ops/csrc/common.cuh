@@ -1,4 +1,4 @@
-// Device helpers shared by the sm_100a kernels.
+// Device helpers shared by the sm_90a kernels.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -163,7 +163,7 @@ __device__ __forceinline__ void st_act(T* p, const FVec<VEC>& x) {
   }
 }
 
-// Fire-and-forget vector reduction into global memory (REDG.E.ADD.F32x4 on sm_100a).
+// Fire-and-forget vector reduction into global memory (REDG.E.ADD.F32x4 on sm_90a).
 template <int VEC>
 __device__ __forceinline__ void red_add_f32(float* p, const FVec<VEC>& x) {
   if constexpr (VEC == 8) {

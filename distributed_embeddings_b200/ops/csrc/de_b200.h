@@ -1,4 +1,4 @@
-// Host-callable launchers of the sm_100a kernels. Plain C++ (no torch headers) so that the .cu
+// Host-callable launchers of the sm_90a kernels. Plain C++ (no torch headers) so that the .cu
 // files compile in seconds; bindings.cpp adapts these to TORCH_LIBRARY ops.
 #pragma once
 #include <cuda_runtime.h>
@@ -7,6 +7,8 @@
 namespace de {
 
 constexpr int kMaxPeers = 16;
+// grid-stride elementwise kernels launch at most a few blocks per SM of an H100 SXM (132 SMs)
+constexpr int kGridCapSms = 132;
 
 // One entry per local input (feature) served by this rank. Resolved once from the sharding plan
 // so a single persistent kernel handles every table of the rank (hundreds in the large models).
@@ -266,7 +268,7 @@ void launch_sgd_update(float* p32, void* p16, float* g32, const float* lr_ptr, f
 void launch_cast_pad(const float* src, int src_cols, void* dst, int dst_cols, int64_t rows,
                      cudaStream_t stream);
 
-// ---- hand-written tcgen05 / TMA / TMEM GEMM with fused bias + activation epilogue ------------
+// ---- hand-written wgmma / TMA GEMM with fused bias + activation epilogue --------------------
 bool launch_gemm_tn_fused(const void* A, int64_t lda, const void* B, int64_t ldb, const void* bias,
                           void* C, int64_t ldc, int M, int N, int K, int epi, const void* act,
                           int64_t ldact, float* colsum, int block_n, int sm_count,

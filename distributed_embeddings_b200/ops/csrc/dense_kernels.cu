@@ -1,4 +1,4 @@
-// Dense-side kernels of the DLRM step for sm_100a (everything around the MLP GEMMs):
+// Dense-side kernels of the DLRM step for sm_90a (everything around the MLP GEMMs):
 //   * dot interaction forward / backward: per sample Gram matrix F F^T of the (n_emb + 1) x D
 //     feature matrix on tensor cores (mma.sync m16n8k16 bf16, one warp per sample).  The op is
 //     HBM bound (7 KB in, 1 KB out per sample), the MMA only has to keep up with the loads.  The
@@ -255,8 +255,7 @@ interact_bwd_kernel(const bf16* __restrict__ bottom, int64_t bottom_stride,
   }
 }
 
-// ---- v2 of the interaction backward (the default; measured 287 vs 370 us for v1 at one GPU,
-// profiles/r2_experiments/summary.txt).  ncu of v1: 60 % of the issue stalls are long_scoreboard, 25 %
+// ---- v2 of the interaction backward (the default).  v1 stalls mostly on long_scoreboard with few
 // warps active - a warp loads a sample, waits, computes, stores, and only then touches the next
 // sample.  v2 keeps the *next* sample's features and dz row in flight (cp.async into a second
 // buffer) while the current one is multiplied and stored, and reads dz from shared memory
@@ -668,7 +667,7 @@ void launch_avgpool_fwd(const void* x, int64_t x_stride, int n, void* out, int64
                         int out_len, int stride, int left, int64_t rows, cudaStream_t stream) {
   if (rows <= 0 || out_len <= 0) return;
   int64_t blocks = (rows * out_len + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > kGridCapSms * 16) blocks = kGridCapSms * 16;
   avgpool_fwd_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
       reinterpret_cast<const bf16*>(x), x_stride, n, reinterpret_cast<bf16*>(out), out_stride,
       out_len, stride, left, rows);
@@ -679,7 +678,7 @@ void launch_avgpool_bwd(const void* dout, int64_t dout_stride, int out_len, void
                         cudaStream_t stream) {
   if (rows <= 0 || n <= 0) return;
   int64_t blocks = (rows * n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > kGridCapSms * 16) blocks = kGridCapSms * 16;
   avgpool_bwd_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
       reinterpret_cast<const bf16*>(dout), dout_stride, out_len, reinterpret_cast<bf16*>(dx),
       dx_stride, n, stride, left, rows);
@@ -834,7 +833,7 @@ void launch_cast_pad(const float* src, int src_cols, void* dst, int dst_cols, in
                      cudaStream_t stream) {
   if (rows <= 0) return;
   int64_t blocks = (rows * dst_cols + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > kGridCapSms * 8) blocks = kGridCapSms * 8;
   cast_pad_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
       src, src_cols, reinterpret_cast<bf16*>(dst), dst_cols, rows);
 }

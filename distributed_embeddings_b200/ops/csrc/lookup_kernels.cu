@@ -1,9 +1,9 @@
-// Pooled embedding lookup forward and atomic scatter-add backward for sm_100a.
+// Pooled embedding lookup forward and atomic scatter-add backward for sm_90a.
 //
 // One persistent, descriptor-driven kernel serves every table of the rank.  A warp owns a tile
 // of 32 consecutive samples of one input; inside the warp, LPR lanes cooperate on one row
 // (LPR * VEC columns per pass) and 32/LPR rows are in flight side by side, with a further 4x
-// unroll so that >= 4 independent 16-byte row loads per lane are outstanding (HBM3e needs ~45 KB
+// unroll so that >= 4 independent 16-byte row loads per lane are outstanding (HBM3 needs ~16 KB
 // in flight per SM).  Sources of ids and destinations of pooled rows are *peer-mapped* pointers:
 // with world_size > 1 the kernel reads indices straight out of the requesters' staging buffers
 // and stores pooled rows straight into the requesters' output tensors over NVLink (the two
@@ -438,8 +438,8 @@ scatter_add_staged_kernel(const InputDesc* __restrict__ descs, int n_inputs, int
     // one-hot inputs: samples of the tile that hit the same row are summed in the warp (their
     // gradient rows are in shared memory anyway) and reduced into the table ONCE.  A table with
     // a handful of rows, or the head of a power-law id distribution, otherwise serialises
-    // thousands of reductions on a few L2 lines (measured at 8 GPUs: the rank that owns the
-    // tiny MLPerf tables took 179 us for this kernel, the others 56).
+    // thousands of reductions on a few L2 lines (the rank that owns the tiny MLPerf tables
+    // would take several times as long as the others).
     unsigned leaders = 0, my_peers = 0;
     if (onehot) {
       const bool valid = lane < tc.nsamp &&

@@ -1,4 +1,4 @@
-// COO -> CSR conversion and the IntegerLookup hash table for sm_100a.
+// COO -> CSR conversion and the IntegerLookup hash table for sm_90a.
 //
 // IntegerLookup maps raw int64 keys to contiguous indices [1, capacity) on the fly; index 0 is the
 // out-of-vocabulary bucket once the vocabulary is full.  The table is open addressed with linear

@@ -1,4 +1,4 @@
-// Deduplicated sparse backward for sm_100a: (row key, item) pairs -> radix sort -> unique
+// Deduplicated sparse backward for sm_90a: (row key, item) pairs -> radix sort -> unique
 // segments -> one lane group per unique row sums its gradient rows (pulled from peer-mapped
 // gradient buffers when world_size > 1) and applies the optimizer update in place
 // (SGD / Adagrad / row-wise Adagrad / lazy Adam), or emits (unique_ids, unique_grad) for an

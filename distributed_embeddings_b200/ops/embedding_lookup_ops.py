@@ -1,6 +1,6 @@
 """Python op wrappers + autograd glue for the embedding kernels.
 
-CUDA tensors run the hand-written sm_100a kernels (``_C.so``; there is no eager fallback on GPU),
+CUDA tensors run the hand-written sm_90a kernels (``_C.so``; there is no eager fallback on GPU),
 CPU tensors run a plain PyTorch implementation with identical semantics which doubles as the
 numerics oracle in the tests.
 

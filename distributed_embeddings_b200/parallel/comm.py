@@ -3,7 +3,7 @@ paths, peer-mapped *symmetric buffers* (cudaMalloc + CUDA IPC) for the hot paths
 
 Every rank allocates the same set of buffers; handles are exchanged once through the process
 group and opened with ``cudaIpcOpenMemHandle`` so each rank holds a device pointer to every
-peer's copy.  Kernels then load/store peer HBM directly over NVLink 5 / NVSwitch.  Cross-rank
+peer's copy.  Kernels then load/store peer HBM directly over NVLink 4 / NVSwitch.  Cross-rank
 ordering uses a signal pad of per-(channel, writer) epoch words written with ``st.release.sys``
 and polled with ``ld.acquire.sys`` under a bounded-spin watchdog (no infinite device spins).
 
@@ -262,8 +262,8 @@ class CommContext:
   def alloc_multicast(self, nbytes: int, name: str = "") -> Optional[MulticastBuffer]:
     """Symmetric buffer with an NVSwitch multicast mapping, or None when NVLS is unavailable
     (single GPU, no NVSwitch, or the handle exchange is not permitted in this container)."""
-    # opt-in (DE_B200_NVLS=1): validated numerically, but no end-to-end gain was measured over the
-    # P2P kernel at 2 and 8 GPUs, and the P2P path needs nothing beyond CUDA IPC
+    # opt-in (DE_B200_NVLS=1): it needs an NVSwitch system, and the P2P path needs nothing beyond
+    # CUDA IPC
     if not self.p2p or self.world_size == 1 or os.environ.get("DE_B200_NVLS", "0") != "1":
       return None
     ok = 1

@@ -5,7 +5,7 @@
 runs the index / pooled-vector exchanges.  Two execution back ends share the plan, the weights and
 the checkpoint surface:
 
-* ``fused`` (CUDA): descriptor-driven sm_100a kernels that read indices from and write pooled
+* ``fused`` (CUDA): descriptor-driven sm_90a kernels that read indices from and write pooled
   vectors / pull gradients to peer HBM over NVLink (see ``fused.py``); no NCCL on the hot path.
 * ``torch``: the same data flow expressed with ``torch.distributed`` collectives and autograd
   (works on CPU/gloo and GPU/NCCL, with user-defined embedding layers and host-resident tables).

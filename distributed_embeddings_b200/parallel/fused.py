@@ -1,4 +1,4 @@
-"""Fused execution engine of :class:`DistributedEmbedding` (CUDA, sm_100a).
+"""Fused execution engine of :class:`DistributedEmbedding` (CUDA, sm_90a).
 
 Data flow of one training step on every rank (``W`` ranks, local batch ``b``, global ``B = W*b``).
 Every exchange is a *push* over NVLink from inside a data kernel, and the cross-GPU ordering is
@@ -170,7 +170,7 @@ class FusedEngine:
 
     A fused producer (the DLRM interaction backward) that stores its gradient pieces straight
     into peer memory is throttled by NVLink back-pressure on its own load/store pipe: compute
-    and transfer serialise (measured: 407 GB/s against the 700 GB/s a pure copy kernel reaches).
+    and transfer serialise, well below the rate a pure copy kernel reaches.
     With this on, the producer writes the pieces of remote owners into ``gstage`` (owner-major,
     local memory, ``routes_stage``) and counts finished rows per chunk of ``chunk_rows``
     samples; :meth:`launch_streamed_push` runs a small copy kernel next to it that forwards

@@ -269,8 +269,7 @@ class DistEmbeddingStrategy:
     widths = [self.slice_widths(c, threshold, self.world_size) for c in configs]
     # per-sample work of every table of the group, in "rows of one column": every id is a row
     # gathered (and read-modify-written in the backward), every input one pooled vector out and
-    # one gradient vector in over NVLink, worth about two row accesses each at the measured
-    # HBM / NVLink rates (profiles/README.md)
+    # one gradient vector in over NVLink, worth about two row accesses each at HBM / NVLink rates
     lookups = [0] * len(configs)
     for k, t in enumerate(col_map):
       lookups[t] += self.input_hotness[self.input_groups[1][k]] + 2

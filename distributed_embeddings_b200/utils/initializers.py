@@ -2,7 +2,7 @@
 
 Tables can be hundreds of GB, so initializers fill an already-allocated device tensor in row
 chunks instead of materialising a host copy (the reference forces initialisation onto the CPU
-to dodge the 2x temporary, embedding.py:28-38; on a 180 GB B200 in-place chunked device init is
+to dodge the 2x temporary, embedding.py:28-38; on an 80 GB H100 in-place chunked device init is
 both simpler and faster).
 """
 from __future__ import annotations

@@ -1,4 +1,4 @@
-"""Packaging: builds the sm_100a extension in-tree, then installs the python package."""
+"""Packaging: builds the sm_90a extension in-tree, then installs the python package."""
 import os
 import subprocess
 import sys
@@ -19,7 +19,7 @@ class BuildWithKernels(build_py):
 setup(
     name="distributed-embeddings-b200",
     version="0.1.0",
-    description="B200-native hybrid-parallel embeddings (PyTorch + sm_100a CUDA + NVLink P2P)",
+    description="H100-native hybrid-parallel embeddings (PyTorch + sm_90a CUDA + NVLink P2P)",
     packages=find_packages(include=["distributed_embeddings_b200", "distributed_embeddings_b200.*"]),
     package_data={"distributed_embeddings_b200": ["_C.so", "ops/csrc/*"]},
     cmdclass={"build_py": BuildWithKernels},

@@ -1,4 +1,4 @@
-"""GPU runs of the distributed cases: fused back end (sm_100a kernels + P2P) and the torch/NCCL
+"""GPU runs of the distributed cases: fused back end (sm_90a kernels + P2P) and the torch/NCCL
 back end.  world=1 exercises the kernels on one GPU; world>=2 needs several GPUs (NVLink P2P)."""
 import pytest
 import torch

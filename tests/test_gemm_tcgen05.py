@@ -1,4 +1,4 @@
-"""Hand-written tcgen05/TMA/TMEM GEMM with fused bias+ReLU epilogue vs a PyTorch fp32 reference."""
+"""Hand-written wgmma/TMA GEMM with fused bias+ReLU epilogue vs a PyTorch fp32 reference."""
 import pytest
 import torch
 
@@ -46,7 +46,7 @@ def test_gemm_strided_views_and_no_bias():
 @pytest.mark.parametrize("m,n,k", [(4096, 512, 256), (777, 256, 1024), (8192, 1024, 1024),
                                    (1000, 128, 256)])
 def test_fused_dgrad_relu_bias(m, n, k):
-  """dx = (dy @ W) * (x > 0) and db = colsum(dx) in one tcgen05 kernel (W^T given K-major)."""
+  """dx = (dy @ W) * (x > 0) and db = colsum(dx) in one wgmma kernel (W^T given K-major)."""
   ops = _native.require()
   torch.manual_seed(m + n)
   dy = (torch.randn(m, k, device="cuda") * 0.5).bfloat16()
@@ -64,7 +64,7 @@ def test_fused_dgrad_relu_bias(m, n, k):
                                    (8192, 1024, 1024), (777, 512, 512), (300, 256, 256)])
 @pytest.mark.parametrize("relu", [True, False])
 def test_gemm_cta_pair_matches_reference(m, n, k, relu):
-  """block_n=512 selects the 2-CTA kernel (UMMA 256x256x16, cta_group::2)."""
+  """block_n=512 selects the 2-CTA cluster kernel (256x256 tile, B tile multicast to both CTAs)."""
   ops = _native.require()
   torch.manual_seed(m + n + k)
   a = (torch.randn(m, k, device="cuda") * 0.5).bfloat16()

@@ -1,4 +1,4 @@
-"""The offline analysis tools keep working on the artifacts committed under profiles/ (no GPU)."""
+"""The offline analysis tools: timelines, step budgets, SASS and plan reports (no GPU)."""
 import os
 import shutil
 import subprocess
@@ -14,8 +14,41 @@ def _run(*args):
                         timeout=300, check=False)
 
 
-def test_step_budget_on_the_committed_timeline():
-  out = _run("tools/step_budget.py", "profiles/r2/critical_path_n8.txt")
+def _trace(rank_delay, steps=3):
+  """A chrome trace of ``bench.py --profile-all-ranks`` shape: ``steps`` steps of six kernels (id
+  push, lookup, dense GEMM, interaction, all-reduce, embedding update), 400 us apart."""
+  ev, t = [], 1000.0
+  for _ in range(steps):
+    t0 = t + rank_delay
+    for name, dur in (("void de::(anonymous namespace)::push_segments_kernel<int>(...)", 10),
+                      ("void de::(anonymous namespace)::lookup_fwd_kernel<int, bf16, 4>(...)", 40),
+                      ("nvjet_tst_128x256_64x6_2x2_2cta_v_bz_relubias", 30),
+                      ("void de::(anonymous namespace)::interact_fwd_kernel<128>(...)", 25),
+                      ("void de::(anonymous namespace)::allreduce_p2p_kernel<false>(...)", 20),
+                      ("void de::(anonymous namespace)::scatter_add_staged_kernel<int, bf16>(...)",
+                       35)):
+      ev.append({"ph": "X", "cat": "kernel", "name": name, "ts": t0, "dur": dur})
+      t0 += dur + 1
+    t += 400
+  return {"traceEvents": ev}
+
+
+def _write_traces(prof, delays):
+  import json
+  for rank, delay in enumerate(delays):
+    suffix = ".trace.json" if rank == 0 else f".rank{rank}.trace.json"
+    with open(prof + suffix, "w", encoding="utf-8") as f:
+      json.dump(_trace(delay), f)
+
+
+def test_step_budget_on_an_eight_rank_timeline(tmp_path):
+  prof = str(tmp_path / "prof.txt")
+  _write_traces(prof, [1.5 * r for r in range(8)])
+  timeline = _run("tools/critical_path.py", prof, "--step", "1")
+  assert timeline.returncode == 0, timeline.stderr[-1000:]
+  path = tmp_path / "timeline.txt"
+  path.write_text(timeline.stdout, encoding="utf-8")
+  out = _run("tools/step_budget.py", str(path))
   assert out.returncode == 0, out.stderr[-1000:]
   text = out.stdout
   assert text.count("== rank ") == 8
@@ -51,14 +84,14 @@ def test_resource_usage_lists_the_hot_kernels():
 
 
 @pytest.mark.skipif(shutil.which("cuobjdump") is None, reason="CUDA toolkit not on PATH")
-def test_sass_census_shows_the_blackwell_opcodes():
+def test_sass_census_shows_the_hopper_opcodes():
   so = os.path.join(ROOT, "distributed_embeddings_b200", "_C.so")
   if not os.path.exists(so):
     pytest.skip("extension not built")
   out = _run("tools/sass_census.py")
   assert out.returncode == 0, out.stderr[-1000:]
   text = out.stdout
-  for op in ("UTCHMMA", "UTMALDG", "REDG", "LDGSTS", "HMMA", "STRONG.SYS", "MATCH.ANY"):
+  for op in ("HGMMA", "UTMALDG", "REDG", "LDGSTS", "HMMA", "STRONG.SYS", "MATCH.ANY"):
     assert op in text, op
 
 
@@ -84,29 +117,8 @@ def test_plan_report_cli():
 def test_critical_path_and_step_budget_on_a_synthetic_trace(tmp_path):
   """tools/critical_path.py merges the per-rank chrome traces of `bench.py --profile-all-ranks`
   into one timeline; tools/step_budget.py reads that text.  Two ranks, three steps each."""
-  import json
-
-  def trace(rank_delay):
-    ev, t = [], 1000.0
-    for _ in range(3):
-      t0 = t + rank_delay
-      for name, dur in (("void de::(anonymous namespace)::push_segments_kernel<int>(...)", 10),
-                        ("void de::(anonymous namespace)::lookup_fwd_kernel<int, bf16, 4>(...)", 40),
-                        ("nvjet_tst_128x256_64x6_2x2_2cta_v_bz_relubias", 30),
-                        ("void de::(anonymous namespace)::interact_fwd_kernel<128>(...)", 25),
-                        ("void de::(anonymous namespace)::allreduce_p2p_kernel<false>(...)", 20),
-                        ("void de::(anonymous namespace)::scatter_add_staged_kernel<int, bf16>(...)",
-                         35)):
-        ev.append({"ph": "X", "cat": "kernel", "name": name, "ts": t0, "dur": dur})
-        t0 += dur + 1
-      t += 400
-    return {"traceEvents": ev}
-
   prof = str(tmp_path / "prof.txt")
-  with open(prof + ".trace.json", "w", encoding="utf-8") as f:
-    json.dump(trace(0.0), f)
-  with open(prof + ".rank1.trace.json", "w", encoding="utf-8") as f:
-    json.dump(trace(7.0), f)
+  _write_traces(prof, [0.0, 7.0])
   out = _run("tools/critical_path.py", prof, "--step", "1")
   assert out.returncode == 0, out.stderr[-1000:]
   text = out.stdout

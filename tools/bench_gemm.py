@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""tcgen05 GEMM (+bias+ReLU epilogue) vs cuBLASLt (_addmm_activation) on the DLRM layer shapes."""
+"""First-party wgmma GEMM (+bias+ReLU epilogue) vs cuBLASLt (_addmm_activation) on the DLRM layer shapes."""
 import json
 import os
 import sys
@@ -41,13 +41,13 @@ for (n, k) in [(512, 16), (256, 512), (128, 256), (1024, 480), (1024, 1024), (51
     if n < bn:
       continue
     t = timeit(lambda: ops.gemm_tn_bias_act(x, w, bias, out, True, bn))
-    res[f"tcgen05_bn{bn}_us"] = round(t, 1)
-    res[f"tcgen05_bn{bn}_tflops"] = round(flops / t / 1e6, 1)
+    res[f"wgmma_bn{bn}_us"] = round(t, 1)
+    res[f"wgmma_bn{bn}_tflops"] = round(flops / t / 1e6, 1)
   if n >= 256:
-    # CTA-pair kernel (cta_group::2), see gemm_tn_pair_kernel
+    # 2-CTA cluster kernel (B tile multicast), see gemm_tn_pair_kernel
     t = timeit(lambda: ops.gemm_tn_bias_act(x, w, bias, out, True, 512))
-    res["tcgen05_pair_us"] = round(t, 1)
-    res["tcgen05_pair_tflops"] = round(flops / t / 1e6, 1)
+    res["wgmma_pair_us"] = round(t, 1)
+    res["wgmma_pair_tflops"] = round(flops / t / 1e6, 1)
   rows.append(res)
   print(json.dumps(res))
 os.makedirs("gpurun_out", exist_ok=True)

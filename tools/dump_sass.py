@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Full SASS listings of the hot kernels of ``_C.so`` (one file per kernel under
-``profiles/sass/``; cuobjdump runs without a GPU):
+``sass/`` of the output directory, default the current one; cuobjdump runs without a GPU):
 
     python tools/dump_sass.py            # the curated list below
     python tools/dump_sass.py --all      # every kernel (large)
@@ -8,7 +8,7 @@
 The listings are the evidence for what the kernels are built from: peer-memory ``STG`` /
 ``LDG`` and the system-scope flag protocol (``ST.E.STRONG.SYS`` / ``LD.E.STRONG.SYS``) inside the
 data kernels, ``REDG.E.ADD.F32x4`` table updates, ``LDGSTS`` + ``LDSM`` + ``HMMA`` interaction,
-``UTMALDG`` / ``UTCHMMA`` / ``LDTM`` / ``UTCBAR`` GEMMs, ``LDGMC`` multimem all-reduce."""
+``UTMALDG`` / ``HGMMA`` GEMMs, ``LDGMC`` multimem all-reduce."""
 import argparse
 import os
 import re
@@ -17,7 +17,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SO = os.path.join(ROOT, "distributed_embeddings_b200", "_C.so")
-OUT = os.path.join(ROOT, "profiles", "sass")
+OUT = os.path.join(os.getcwd(), "sass")
 
 # (file stem, regex on the demangled name): the instantiations the DLRM / synthetic steps run
 HOT = [

@@ -5,7 +5,7 @@ gathers and sends per step, and how unbalanced the plan is.
   python tools/plan_report.py --model dlrm-mlperf --world 8 --data-parallel-threshold 320000
   python tools/plan_report.py --model small --world 8 --strategy traffic_balanced
   python tools/plan_report.py --tables 1000000x128,5000x64,250000000x128 --world 4 \\
-      --column-slice-threshold auto --hbm-gib 180
+      --column-slice-threshold auto --hbm-gib 79
 
 Uses the same planner the run would use (``DistEmbeddingStrategy``, ``traffic_report``,
 ``memory_report``); nothing is allocated.
@@ -57,7 +57,7 @@ def main(argv=None):
   ap.add_argument("--row-slice-threshold", default=None)
   ap.add_argument("--data-parallel-threshold", default=None)
   ap.add_argument("--global-batch", type=int, default=65536)
-  ap.add_argument("--hbm-gib", type=float, default=180.0, help="per-GPU memory to check against")
+  ap.add_argument("--hbm-gib", type=float, default=79.0, help="per-GPU memory to check against")
   ap.add_argument("--optimizer-slots", type=int, default=0,
                   help="fp32 state copies per table element (adagrad 1, adam 2)")
   ap.add_argument("--json", action="store_true")

@@ -3,7 +3,7 @@
 bank) from ``cuobjdump -res-usage`` - the ``-Xptxas -v`` numbers of the binary that actually ships,
 no GPU needed:
 
-    python tools/resource_usage.py > profiles/resource_usage.txt
+    python tools/resource_usage.py > resource_usage.txt
 """
 import os
 import re
@@ -28,7 +28,7 @@ def main():
       rows.append((src, m.group(1), res))
   names = subprocess.run(["cu++filt"] + [r[1] for r in rows], capture_output=True, text=True,
                          check=False).stdout.splitlines()
-  print("# cuobjdump -res-usage of distributed_embeddings_b200/_C.so (sm_100a); static shared "
+  print("# cuobjdump -res-usage of distributed_embeddings_b200/_C.so (sm_90a); static shared "
         "memory only - dynamic shared memory is set at launch")
   print(f"{'source':<26} {'regs':>5} {'stack':>6} {'local':>6} {'smem':>7} {'const0':>7}  kernel")
   for (src, _, res), name in sorted(zip(rows, names), key=lambda x: (x[0][0], x[1])):

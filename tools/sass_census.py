@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Per-kernel SASS mnemonic census of the built extension (cuobjdump runs without a GPU):
-   python tools/sass_census.py > profiles/sass_census.txt"""
+   python tools/sass_census.py"""
 import collections
 import os
 import re
@@ -9,7 +9,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SO = os.path.join(ROOT, "distributed_embeddings_b200", "_C.so")
-NOTABLE = re.compile(r"^(UTCHMMA|UTMALDG|UTMASTG|UTCBAR|UTCATOMSWS|UBLKCP|SYNCS|HMMA|LDGSTS|LDSM|REDG|"
+NOTABLE = re.compile(r"^(HGMMA|WARPGROUP|UTMALDG|UTMASTG|UTCBAR|UTCATOMSWS|UBLKCP|SYNCS|HMMA|LDGSTS|LDSM|REDG|"
                      r"ATOMG|ATOMS|MATCH|LDGMC|STGMC|REDGMC|LDG\.E\.128|STG\.E\.128|LDTM|STTM|MULTIMEM|MEMBAR|"
                      r"LDG\.E\.STRONG\.SYS|STG\.E\.STRONG\.SYS|LD\.E\.STRONG\.SYS|ST\.E\.STRONG\.SYS|"
                      r"CCTL|UCGABAR|ELECT|REDUX|SHFL)")
@@ -23,7 +23,7 @@ def main():
     out = subprocess.run(["cu++filt"] + names, capture_output=True, text=True, check=False).stdout
     for n, d in zip(names, out.splitlines()):
       demangle[n] = d
-  print(f"# SASS mnemonic census of distributed_embeddings_b200/_C.so (sm_100a), per kernel")
+  print(f"# SASS mnemonic census of distributed_embeddings_b200/_C.so (sm_90a), per kernel")
   print("# columns: kernel | instructions | notable opcodes (count)\n")
   cur, counts, total = None, None, 0
   rows = []
@@ -47,7 +47,7 @@ def main():
       k = NOTABLE.match(op)
       if k:
         # keep the qualifiers that carry meaning (2CTA, MULTICAST, F32x4, sizes)
-        key = op if op.startswith(("UTC", "UTMA", "REDG", "HMMA", "MATCH", "MULTIMEM", "LDTM", "LDGMC", "STGMC", "REDGMC",
+        key = op if op.startswith(("HGMMA", "UTMA", "REDG", "HMMA", "MATCH", "MULTIMEM", "LDTM", "LDGMC", "STGMC", "REDGMC",
                                    "UBLKCP")) else k.group(1)
         counts[key] += 1
   flush()

@@ -7,7 +7,7 @@ which exactly one / several / no kernels were running, and the *exposed* time of
 the wall-clock during which only kernels of that category were running (what would have to shrink
 for the step to get shorter).  No GPU needed.
 
-  python tools/step_budget.py profiles/r2/critical_path_n8.txt > profiles/r2/step_budget_n8.txt
+  python tools/step_budget.py critical_path_n8.txt > step_budget_n8.txt
 """
 import re
 import sys
