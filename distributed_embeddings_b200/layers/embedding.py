@@ -17,7 +17,25 @@ from ..utils import initializers
 
 
 def _embedding_lookup_native(param, ids, combiner=None):
-  """Library (non-custom-kernel) path, used for host-resident tables."""
+  """Library (non-custom-kernel) path, used for host-resident tables.  bf16 / fp16 tables pool
+  the gathered rows in fp32 (no fp32 copy of the table) and return the table dtype, like the
+  kernels."""
+  if param.dtype in (torch.bfloat16, torch.float16) and combiner is not None:
+    if isinstance(ids, RaggedIds):
+      splits = ids.row_splits.to(torch.int64)
+      counts = splits[1:] - splits[:-1]
+      values = ids.values.to(torch.int64)
+    else:
+      values = ids.to(torch.int64).reshape(-1)
+      counts = torch.full((ids.shape[0],), ids.shape[1], dtype=torch.int64, device=ids.device)
+    rows = nn.functional.embedding(values, param).float()
+    sample = torch.repeat_interleave(torch.arange(counts.numel(), device=rows.device),
+                                     counts.to(rows.device))
+    out = torch.zeros(counts.numel(), param.shape[1], dtype=torch.float32, device=rows.device)
+    out = out.index_add(0, sample, rows)
+    if combiner == "mean":
+      out = out / counts.clamp(min=1).to(out).unsqueeze(1)
+    return out.to(param.dtype)
   if isinstance(ids, RaggedIds):
     mode = "sum" if combiner == "sum" else "mean"
     return nn.functional.embedding_bag(ids.values.to(torch.int64),
@@ -87,7 +105,8 @@ class Embedding(nn.Module):
     self.sparse_grad = sparse_grad
     self.layer_name = name
     self.cpu_offloaded = False
-    # no autocast: tables stay fp32 (reference embedding.py:92,111)
+    # no autocast: tables stay in their storage dtype, fp32 by default (reference
+    # embedding.py:92,111); bf16 / fp16 tables are pooled in fp32
     self.embeddings = nn.Parameter(torch.empty(self.input_dim, self.output_dim, dtype=dtype,
                                                device=device),
                                    requires_grad=True)
@@ -166,14 +185,18 @@ class Embedding(nn.Module):
     }
 
   @classmethod
-  def from_config(cls, config: Dict[str, Any], device=None):
+  def from_config(cls, config: Dict[str, Any], device=None, dtype=None):
     """Create a layer from a config; stock-embedding configs are accepted
-    (``mask_zero`` / ``input_length`` are dropped, reference embedding.py:163-170)."""
+    (``mask_zero`` / ``input_length`` are dropped, reference embedding.py:163-170).  A ``dtype``
+    inside the config is dropped as well; the ``dtype`` argument sets the table's storage
+    (default fp32)."""
     config = dict(config)
     for k in ("mask_zero", "input_length", "layer_type", "cpu_offload", "input_dims", "offsets",
               "batch_input_shape", "dtype", "trainable", "sparse", "padding_idx", "max_norm",
               "norm_type", "scale_grad_by_freq"):
       config.pop(k, None)
+    if dtype is not None:
+      config["dtype"] = dtype
     return cls(device=device, **config)
 
   def extra_repr(self):

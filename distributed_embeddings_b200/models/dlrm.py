@@ -80,7 +80,10 @@ class DLRM(nn.Module):
                compute_dtype: torch.dtype = torch.bfloat16,
                backend: str = "auto",
                world_size: Optional[int] = None,
-               rank: Optional[int] = None):
+               rank: Optional[int] = None,
+               table_dtype: torch.dtype = torch.float32):
+    """``table_dtype``: storage of the model-parallel embedding tables (fp32, bf16 or fp16, see
+    :class:`DistributedEmbedding`); bf16 fits the 40M-row MLPerf tables on one 80 GB GPU."""
     super().__init__()
     if bottom_mlp_dims[-1] != embedding_dim:
       raise ValueError("bottom MLP must end at the embedding width for the dot interaction")
@@ -105,7 +108,8 @@ class DLRM(nn.Module):
                                           compute_dtype=compute_dtype,
                                           backend=backend,
                                           world_size=world_size,
-                                          rank=rank)
+                                          rank=rank,
+                                          table_dtype=table_dtype)
     # the activation is consumed inside this module's step: no defensive copy of the engine buffer
     self.embedding.zero_copy_output = True
     ii, jj = torch.tril_indices(n, n, offset=-1)

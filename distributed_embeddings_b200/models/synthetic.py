@@ -129,11 +129,13 @@ class _SyntheticBase(nn.Module):
 
 class SyntheticModel(_SyntheticBase):
   """Synthetic model on :class:`DistributedEmbedding` (``memory_balanced``, sum combiner, shared
-  multi-hot inputs through ``input_table_map``)."""
+  multi-hot inputs through ``input_table_map``).  ``table_dtype``: storage of the model-parallel
+  tables (fp32, bf16 or fp16, see :class:`DistributedEmbedding`)."""
 
   def __init__(self, model_config: ModelConfig, column_slice_threshold=None, dp_input=False,
                device=None, compute_dtype=torch.float32, backend="auto",
-               row_slice_threshold=None, data_parallel_threshold=None, strategy="memory_balanced"):
+               row_slice_threshold=None, data_parallel_threshold=None, strategy="memory_balanced",
+               table_dtype=torch.float32):
     super().__init__()
     tables, imap, hots = expand(model_config)[:3]
     self.input_table_map = imap
@@ -147,7 +149,8 @@ class SyntheticModel(_SyntheticBase):
                                           row_slice_threshold=row_slice_threshold,
                                           data_parallel_threshold=data_parallel_threshold,
                                           device=device, compute_dtype=compute_dtype,
-                                          backend=backend, input_hotness=list(hots))
+                                          backend=backend, input_hotness=list(hots),
+                                          table_dtype=table_dtype)
     self.embedding.zero_copy_output = True  # consumed inside this module's step
     total = sum(tables[t][1] for t in imap)
     if self.interact_stride is not None:

@@ -137,14 +137,16 @@ std::vector<int64_t> struct_sizes() {
 void lookup_fwd(const Tensor& descs, int64_t n_inputs, int64_t batch, int64_t src_batch,
                 int64_t dst_batch, int64_t dst_stride, at::IntArrayRef src_ptrs,
                 at::IntArrayRef dst_ptrs, int64_t rot, bool ids64, int64_t act_dtype, bool vec4,
-                at::IntArrayRef sync, int64_t tile_samples) {
+                at::IntArrayRef sync, int64_t tile_samples, int64_t table_dtype, bool vec8) {
   TORCH_CHECK(descs.is_cuda(), "descs must live on the GPU");
+  TORCH_CHECK(table_dtype >= 0 && table_dtype <= 2, "table_dtype: 0 fp32, 1 bf16, 2 fp16");
   c10::cuda::CUDAGuard guard(descs.device());
   de::launch_lookup_fwd(reinterpret_cast<const de::InputDesc*>(descs.data_ptr()),
                         static_cast<int>(n_inputs), batch, src_batch, dst_batch, dst_stride,
                         to_peers(src_ptrs), to_peers(dst_ptrs), static_cast<int>(rot), ids64,
                         static_cast<int>(act_dtype), vec4, sm_count(), cur_stream(),
-                        to_sync(sync), static_cast<int>(tile_samples));
+                        to_sync(sync), static_cast<int>(tile_samples),
+                        static_cast<int>(table_dtype), vec8);
   check_launch();
 }
 
@@ -352,8 +354,10 @@ void segment_update(const Tensor& descs, const Tensor& tables, int64_t n_tables,
                     double beta2, double bias1, double bias2, double grad_scale,
                     double weight_decay, int64_t lr_ptr, const c10::optional<Tensor>& emit_keys,
                     const c10::optional<Tensor>& emit_rows, int64_t max_width, int64_t act_dtype,
-                    bool vec4, const c10::optional<Tensor>& scratch, int64_t step_ptr) {
+                    bool vec4, const c10::optional<Tensor>& scratch, int64_t step_ptr,
+                    int64_t table_dtype) {
   c10::cuda::CUDAGuard guard(descs.device());
+  TORCH_CHECK(table_dtype >= 0 && table_dtype <= 2, "table_dtype: 0 fp32, 1 bf16, 2 fp16");
   de::OptimizerArgs opt;
   opt.kind = static_cast<int32_t>(opt_kind);
   opt.lr = static_cast<float>(lr);
@@ -381,7 +385,7 @@ void segment_update(const Tensor& descs, const Tensor& tables, int64_t n_tables,
         reinterpret_cast<const uint32_t*>(sorted_items.data_ptr<int>()), n_items,
         seg_start.data_ptr<int64_t>(), n_unique.data_ptr<int64_t>(), opt,
         scratch->data_ptr<float>(), static_cast<int>(sw), static_cast<int>(max_width),
-        static_cast<int>(act_dtype), sm_count(), cur_stream());
+        static_cast<int>(act_dtype), sm_count(), cur_stream(), static_cast<int>(table_dtype));
     TORCH_CHECK(ok, "balanced update launch failed");
     check_launch();
     return;
@@ -394,7 +398,7 @@ void segment_update(const Tensor& descs, const Tensor& tables, int64_t n_tables,
       seg_start.data_ptr<int64_t>(), n_unique.data_ptr<int64_t>(), sorted_keys.numel(), opt,
       emit_keys.has_value() ? emit_keys->data_ptr<int64_t>() : nullptr,
       emit_rows.has_value() ? emit_rows->data_ptr<float>() : nullptr, static_cast<int>(max_width),
-      static_cast<int>(act_dtype), vec4, sm_count(), cur_stream());
+      static_cast<int>(act_dtype), vec4, sm_count(), cur_stream(), static_cast<int>(table_dtype));
   check_launch();
 }
 
@@ -432,18 +436,21 @@ void check_ids(const Tensor& values, const c10::optional<Tensor>& offsets) {
                 "row_splits must be a contiguous int64 CUDA tensor");
 }
 
-// out[b, :] = combine_{k in sample b} param[ids[k], :]
+// out[b, :] = combine_{k in sample b} param[ids[k], :]   (pooled in fp32, stored in the table's
+// dtype like nn.EmbeddingBag, or in bf16 with out_bf16)
 Tensor embedding_lookup_fwd(const Tensor& param, const Tensor& values,
                             const c10::optional<Tensor>& offsets, int64_t hotness, int64_t batch,
                             int64_t combiner, bool out_bf16) {
-  TORCH_CHECK(param.is_cuda() && param.dim() == 2 && param.scalar_type() == at::kFloat &&
+  const auto pt = param.scalar_type();
+  TORCH_CHECK(param.is_cuda() && param.dim() == 2 &&
+                  (pt == at::kFloat || pt == at::kBFloat16 || pt == at::kHalf) &&
                   param.is_contiguous(),
-              "param must be a contiguous fp32 [rows, width] CUDA tensor");
+              "param must be a contiguous fp32, bf16 or fp16 [rows, width] CUDA tensor");
   check_ids(values, offsets);
   c10::cuda::CUDAGuard guard(param.device());
   const int64_t width = param.size(1);
-  Tensor out = at::empty({batch, width},
-                         param.options().dtype(out_bf16 ? at::kBFloat16 : at::kFloat));
+  const int tdt = dtype_code(pt);
+  Tensor out = at::empty({batch, width}, param.options().dtype(out_bf16 ? at::kBFloat16 : pt));
   if (batch == 0) return out;
   de::InputDesc d = single_desc(param.data_ptr(), values, offsets, hotness, param.size(0), width,
                                 combiner);
@@ -460,8 +467,9 @@ Tensor embedding_lookup_fwd(const Tensor& param, const Tensor& values,
   const int64_t ts = std::max<int64_t>(32 / lanes_per_row, std::min<int64_t>(32, 64 / avg_hot));
   de::launch_lookup_fwd(reinterpret_cast<const de::InputDesc*>(dd.data_ptr()), 1, batch, batch,
                         batch, width, src, dst, 0, values.scalar_type() == at::kLong,
-                        out_bf16 ? 1 : 0, width % 4 == 0, sm_count(), cur_stream(), de::no_sync(),
-                        static_cast<int>(std::max<int64_t>(1, ts)));
+                        out_bf16 ? 1 : tdt, width % 4 == 0, sm_count(), cur_stream(),
+                        de::no_sync(), static_cast<int>(std::max<int64_t>(1, ts)), tdt,
+                        width % 8 == 0 && reinterpret_cast<uintptr_t>(param.data_ptr()) % 16 == 0);
   check_launch();
   return out;
 }
@@ -526,7 +534,7 @@ std::tuple<Tensor, Tensor> embedding_lookup_grad(const Tensor& values,
   std::vector<int64_t> gp = {reinterpret_cast<int64_t>(grad.data_ptr())};
   segment_update(dd, td, 1, batch, batch, gstride, gp, std::get<0>(sorted), std::get<1>(sorted),
                  std::get<2>(sorted), std::get<3>(sorted), de::kOptEmit, 0, 0, 0, 0, 1, 1, 1.0, 0, 0,
-                 emit_keys, emit_rows, width, gdt, vec4, c10::nullopt, 0);
+                 emit_keys, emit_rows, width, gdt, vec4, c10::nullopt, 0, 0);
   // sizing the IndexedSlices-style result needs the unique count on the host (compat path only)
   int64_t n_unique = std::get<3>(sorted).item<int64_t>();
   if (n_unique > 0) {
@@ -994,7 +1002,7 @@ TORCH_LIBRARY(de_b200, m) {
   m.def(
       "lookup_fwd(Tensor descs, int n_inputs, int batch, int src_batch, int dst_batch, "
       "int dst_stride, int[] src_ptrs, int[] dst_ptrs, int rot, bool ids64, int act_dtype, "
-      "bool vec4, int[] sync, int tile_samples) -> ()",
+      "bool vec4, int[] sync, int tile_samples, int table_dtype=0, bool vec8=False) -> ()",
       &lookup_fwd);
   m.def(
       "scatter_add_bwd(Tensor descs, int n_inputs, int batch, int src_batch, int grad_batch, "
@@ -1018,7 +1026,7 @@ TORCH_LIBRARY(de_b200, m) {
       "Tensor seg_start, Tensor n_unique, int opt_kind, float lr, float eps, float beta1, "
       "float beta2, float bias1, float bias2, float grad_scale, float weight_decay, int lr_ptr, "
       "Tensor? emit_keys, Tensor? emit_rows, int max_width, int act_dtype, bool vec4, "
-      "Tensor? scratch, int step_ptr) -> ()",
+      "Tensor? scratch, int step_ptr, int table_dtype=0) -> ()",
       &segment_update);
   m.def(
       "embedding_lookup_fwd(Tensor param, Tensor values, Tensor? offsets, int hotness, int batch, "

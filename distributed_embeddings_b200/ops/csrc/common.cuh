@@ -76,7 +76,10 @@ __device__ __forceinline__ FVec<VEC> ld_f32_rw(const float* p) {
 
 template <int VEC>
 __device__ __forceinline__ void st_f32(float* p, const FVec<VEC>& x) {
-  if constexpr (VEC == 4) {
+  if constexpr (VEC == 8) {
+    *reinterpret_cast<float4*>(p) = make_float4(x.v[0], x.v[1], x.v[2], x.v[3]);
+    *reinterpret_cast<float4*>(p + 4) = make_float4(x.v[4], x.v[5], x.v[6], x.v[7]);
+  } else if constexpr (VEC == 4) {
     *reinterpret_cast<float4*>(p) = make_float4(x.v[0], x.v[1], x.v[2], x.v[3]);
   } else {
 #pragma unroll
@@ -152,6 +155,13 @@ template <typename T, int VEC>
 __device__ __forceinline__ void st_act(T* p, const FVec<VEC>& x) {
   if constexpr (sizeof(T) == 4) {
     st_f32<VEC>(reinterpret_cast<float*>(p), x);
+  } else if constexpr (VEC == 8) {
+    uint4 t;
+    t.x = pack2<T>(x.v[0], x.v[1]);
+    t.y = pack2<T>(x.v[2], x.v[3]);
+    t.z = pack2<T>(x.v[4], x.v[5]);
+    t.w = pack2<T>(x.v[6], x.v[7]);
+    *reinterpret_cast<uint4*>(p) = t;
   } else if constexpr (VEC == 4) {
     uint2 t;
     t.x = pack2<T>(x.v[0], x.v[1]);
@@ -160,6 +170,130 @@ __device__ __forceinline__ void st_act(T* p, const FVec<VEC>& x) {
   } else {
 #pragma unroll
     for (int i = 0; i < VEC; ++i) p[i] = from_f32<T>(x.v[i]);
+  }
+}
+
+// ---- embedding tables: fp32, bf16 or fp16 storage, fp32 arithmetic -------------------------
+// Read-only row fragment of a table in the forward (tables are immutable during the lookup):
+// fp32 rows as float4 / scalars, 16-bit rows as one 16-byte (VEC 8), 8-byte (VEC 4) or 2-byte
+// load per lane, converted to fp32 in registers.
+template <typename TabT, int VEC>
+__device__ __forceinline__ FVec<VEC> ld_tab(const TabT* p) {
+  if constexpr (sizeof(TabT) == 4) {
+    return ld_f32<VEC>(reinterpret_cast<const float*>(p));
+  } else {
+    FVec<VEC> r;
+    if constexpr (VEC == 8) {
+      const uint4 t = __ldg(reinterpret_cast<const uint4*>(p));
+      const uint32_t w[4] = {t.x, t.y, t.z, t.w};
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const float2 f = unpack2<TabT>(w[i]);
+        r.v[2 * i] = f.x;
+        r.v[2 * i + 1] = f.y;
+      }
+    } else if constexpr (VEC == 4) {
+      const uint2 t = __ldg(reinterpret_cast<const uint2*>(p));
+      const float2 fa = unpack2<TabT>(t.x), fb = unpack2<TabT>(t.y);
+      r.v[0] = fa.x; r.v[1] = fa.y; r.v[2] = fb.x; r.v[3] = fb.y;
+    } else {
+      const unsigned short* q = reinterpret_cast<const unsigned short*>(p);
+#pragma unroll
+      for (int i = 0; i < VEC; ++i) {
+        const unsigned short b = __ldg(q + i);
+        r.v[i] = to_f32<TabT>(*reinterpret_cast<const TabT*>(&b));
+      }
+    }
+    return r;
+  }
+}
+
+// Stochastic rounding of fp32 to bf16 / fp16 (the write-back of half-precision tables).
+// The rule, mirrored bit for bit by ops/stochastic_rounding.py:
+//   lo, hi = the neighbouring representable values of x in the target type; lo == hi -> x.
+//   u = (r >> 8) * 2^-24;  result = u * (hi - lo) < x - lo ? hi : lo
+// with every fp32 operation exact, so E[result] = x.  NaN / inf and values beyond the finite
+// range convert as round-to-nearest does.  r is a 32-bit hash of (optimizer step, row key,
+// column): the result does not depend on which thread stores the element, and the step counter
+// is device resident, so CUDA-graph replays draw fresh bits.
+__device__ __forceinline__ uint32_t sr_mix(uint32_t h) {
+  h ^= h >> 16;
+  h *= 0x7feb352du;
+  h ^= h >> 15;
+  h *= 0x846ca68bu;
+  h ^= h >> 16;
+  return h;
+}
+__device__ __forceinline__ uint32_t sr_row_seed(uint32_t step, int64_t key) {
+  uint32_t h = sr_mix(step + 0x9e3779b9u);
+  h = sr_mix(h ^ static_cast<uint32_t>(key));
+  return sr_mix(h ^ static_cast<uint32_t>(static_cast<uint64_t>(key) >> 32));
+}
+__device__ __forceinline__ uint32_t sr_bits(uint32_t row_seed, int col) {
+  return sr_mix(row_seed ^ static_cast<uint32_t>(col));
+}
+
+template <typename T>
+__device__ __forceinline__ unsigned short round_stochastic(float x, uint32_t r) {
+  static_assert(sizeof(T) == 2, "16-bit target");
+  unsigned short rn;
+  float max_finite;
+  if constexpr (std::is_same<T, __half>::value) {
+    rn = __half_as_ushort(__float2half_rn(x));
+    max_finite = 65504.f;
+  } else {
+    rn = __bfloat16_as_ushort(__float2bfloat16_rn(x));
+    max_finite = 0x1.fep+127f;  // 3.3895e38
+  }
+  auto value = [](unsigned short b) {
+    if constexpr (std::is_same<T, __half>::value) return __half2float(__ushort_as_half(b));
+    else return __bfloat162float(__ushort_as_bfloat16(b));
+  };
+  const float rn_f = value(rn);
+  // representable, NaN, +-inf or beyond the finite range: round to nearest
+  if (rn_f == x || !(fabsf(x) <= max_finite)) return rn;
+  // the other neighbour: one step away from rn towards x in the ordered 16-bit encoding
+  const int ord = (rn & 0x8000) ? -static_cast<int>(rn & 0x7fff) : static_cast<int>(rn);
+  const bool up = rn_f < x;
+  const int o2 = up ? ord + 1 : ord - 1;
+  const unsigned short nb = o2 >= 0 ? static_cast<unsigned short>(o2)
+                                    : static_cast<unsigned short>(0x8000 | (-o2));
+  const float nb_f = value(nb);
+  const float lo = up ? rn_f : nb_f, hi = up ? nb_f : rn_f;
+  const float u = __fmul_rn(static_cast<float>(r >> 8), 5.9604644775390625e-8f);  // 2^-24
+  const bool take_hi = __fmul_rn(u, __fsub_rn(hi, lo)) < __fsub_rn(x, lo);
+  const unsigned short lo_b = up ? rn : nb, hi_b = up ? nb : rn;
+  return take_hi ? hi_b : lo_b;
+}
+
+// Plain (coherent) row fragment of a table for read-modify-write in the update kernels.
+template <typename TabT, int VEC>
+__device__ __forceinline__ FVec<VEC> ld_tab_rw(const TabT* p) {
+  return ld_act<TabT, VEC>(p);
+}
+
+// Write-back of an updated row fragment: fp32 as is, 16-bit with stochastic rounding keyed by
+// (step, row key, column).
+template <typename TabT, int VEC>
+__device__ __forceinline__ void st_tab(TabT* p, const FVec<VEC>& x, uint32_t step, int64_t key,
+                                       int col) {
+  if constexpr (sizeof(TabT) == 4) {
+    st_f32<VEC>(reinterpret_cast<float*>(p), x);
+  } else {
+    const uint32_t seed = sr_row_seed(step, key);
+    unsigned short b[VEC];
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) b[i] = round_stochastic<TabT>(x.v[i], sr_bits(seed, col + i));
+    if constexpr (VEC == 4) {
+      uint2 t;
+      t.x = static_cast<uint32_t>(b[0]) | (static_cast<uint32_t>(b[1]) << 16);
+      t.y = static_cast<uint32_t>(b[2]) | (static_cast<uint32_t>(b[3]) << 16);
+      *reinterpret_cast<uint2*>(p) = t;
+    } else {
+      unsigned short* q = reinterpret_cast<unsigned short*>(p);
+#pragma unroll
+      for (int i = 0; i < VEC; ++i) q[i] = b[i];
+    }
   }
 }
 

@@ -13,7 +13,8 @@ constexpr int kGridCapSms = 132;
 // One entry per local input (feature) served by this rank. Resolved once from the sharding plan
 // so a single persistent kernel handles every table of the rank (hundreds in the large models).
 struct alignas(16) InputDesc {
-  const void* table;       // base of the (fused) local table, row major [rows, width] fp32
+  const void* table;       // base of the (fused) local table, row major [rows, width]; fp32,
+                           // bf16 or fp16 (one storage type per launch: `table_dtype`)
   const void* ids;         // direct ids pointer, or nullptr -> src_ptrs[s] + ids_off
   const int64_t* offsets;  // CSR row_splits for ragged inputs, nullptr for fixed hotness
   int64_t ids_off;         // element offset of this input inside a source staging buffer
@@ -79,7 +80,7 @@ enum OptimizerKind : int32_t { kOptSGD = 0, kOptAdagrad = 1, kOptRowwiseAdagrad 
 
 // One entry per (fused) local table, used by the sorted/deduplicated update path.
 struct alignas(16) TableDesc {
-  void* weight;       // [rows, width] fp32
+  void* weight;       // [rows, width]; fp32, bf16 or fp16 (`table_dtype` of the launch)
   void* state0;       // Adagrad accumulator [rows,width] / row-wise [rows] / Adam m
   void* state1;       // Adam v
   int64_t rows;
@@ -98,21 +99,25 @@ struct OptimizerArgs {
   float weight_decay;
   const float* lr_ptr;  // optional device-resident learning rate (overrides lr; graph replay safe)
   const float* step_ptr;  // optional device-resident Adam step count t (bias1/bias2 are then
-                          // recomputed as 1 - beta^t on the device; graph replay safe)
+                          // recomputed as 1 - beta^t on the device; graph replay safe); it
+                          // also keys the stochastic rounding of 16-bit tables
 };
 
 // ---- pooled lookup forward (+ optional fused push to peer output buffers) ------------------
 // ids come from src.p[g / src_batch] (peer mapped) or desc.ids; pooled rows are stored to
 // dst.p[g / dst_batch] + (g % dst_batch) * dst_stride + dst_col.
 // act_dtype: 0 = fp32, 1 = bf16, 2 = fp16 (dtype of the activations / gradients on the wire)
+// table_dtype: storage of every table of the launch, same codes; rows are pooled in fp32.
+// vec8 (16-bit tables with vec4 only): every width, destination column and row stride is a
+// multiple of 8, so a lane loads 8 columns (16 bytes) at a time.
 void launch_lookup_fwd(const InputDesc* descs, int n_inputs, int64_t batch, int64_t src_batch,
                        int64_t dst_batch, int64_t dst_stride, const PeerPtrs& src,
                        const PeerPtrs& dst, int rot, bool ids64, int act_dtype, bool vec4,
                        int sm_count, cudaStream_t stream, const SyncArgs& sync,
-                       int tile_samples = 32);
+                       int tile_samples = 32, int table_dtype = 0, bool vec8 = false);
 
 // ---- backward: atomic scatter-add of (scaled) gradient rows into the table (SGD fast path,
-// also used to build dense gradients of replicated tables). Gradient rows are pulled from
+// also used to build dense gradients of replicated tables).  fp32 tables only. Gradient rows are pulled from
 // grad.p[g / grad_batch] + (g % grad_batch) * grad_stride + dst_col (peer mapped).
 void launch_scatter_add_bwd(const InputDesc* descs, int n_inputs, int64_t batch, int64_t src_batch,
                             int64_t grad_batch, int64_t grad_stride, const PeerPtrs& src,
@@ -150,7 +155,7 @@ void launch_segment_update(const InputDesc* descs, const TableDesc* tables, int 
                            const uint32_t* sorted_items, const int64_t* seg_start,
                            const int64_t* n_unique, int64_t n_items, const OptimizerArgs& opt,
                            int64_t* emit_keys, float* emit_rows, int max_width, int act_dtype,
-                           bool vec4, int sm_count, cudaStream_t stream);
+                           bool vec4, int sm_count, cudaStream_t stream, int table_dtype = 0);
 
 bool launch_balanced_update(const InputDesc* descs, const TableDesc* tables, int n_tables,
                             int64_t batch, int64_t grad_batch, int64_t grad_stride,
@@ -158,7 +163,8 @@ bool launch_balanced_update(const InputDesc* descs, const TableDesc* tables, int
                             const uint32_t* sorted_items, int64_t n_items,
                             const int64_t* seg_start, const int64_t* n_unique,
                             const OptimizerArgs& opt, float* scratch, int scratch_width,
-                            int max_width, int act_dtype, int sm_count, cudaStream_t stream);
+                            int max_width, int act_dtype, int sm_count, cudaStream_t stream,
+                            int table_dtype = 0);
 
 // ---- misc ---------------------------------------------------------------------------------
 void launch_row_to_split(const int64_t* coo_indices, int64_t nnz, int64_t num_rows,

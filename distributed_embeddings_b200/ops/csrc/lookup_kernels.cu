@@ -26,6 +26,9 @@ constexpr int kWarpsPerBlock = kThreads / 32;
 constexpr int kTile = 32;  // samples per warp tile
 constexpr int kUnroll = 4;
 constexpr int kBlocksPerSM = 4;  // 64 registers / thread -> 32 resident warps per SM
+// 16-bit rows read 8 columns per lane: the 4 row fragments of 8 fp32 each in flight need ~80
+// registers (at 64 they spill), so these instantiations keep 3 blocks per SM
+constexpr int fwd_blocks_per_sm(int vec) { return vec == 8 ? 3 : kBlocksPerSM; }
 
 __device__ __forceinline__ void prefetch_l2(const void* p) {
   asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
@@ -93,12 +96,12 @@ __device__ __forceinline__ IdReader<IdT> make_reader(const InputDesc& D, const P
 }
 
 // =============================================================================== forward
-template <typename IdT, typename OutT, int VEC>
-__global__ void __launch_bounds__(kThreads, kBlocksPerSM)
-lookup_fwd_kernel(const InputDesc* __restrict__ descs, int n_inputs, int64_t batch,
-                  int64_t src_batch, int64_t dst_batch, int64_t dst_stride,
-                  const __grid_constant__ PeerPtrs src, const __grid_constant__ PeerPtrs dst,
-                  int rot, const __grid_constant__ SyncArgs sync, int ts) {
+template <typename IdT, typename OutT, int VEC, typename TabT>
+__device__ __forceinline__ void lookup_fwd_body(const InputDesc* __restrict__ descs, int n_inputs,
+                                                int64_t batch, int64_t src_batch,
+                                                int64_t dst_batch, int64_t dst_stride,
+                                                const PeerPtrs& src, const PeerPtrs& dst, int rot,
+                                                const SyncArgs& sync, int ts) {
   // ts = samples per warp tile (power of two <= 32): 32 for one-hot inputs; multi-hot inputs
   // get smaller tiles so that a launch still has enough warps when every sample pools tens or
   // hundreds of rows (the reference splits long reductions over blockDim.y, CU:195-226)
@@ -115,11 +118,12 @@ lookup_fwd_kernel(const InputDesc* __restrict__ descs, int n_inputs, int64_t bat
     if (tc.nsamp <= 0) continue;
     const InputDesc D = descs[tc.f];
     const int W = D.width;
-    const int nvec = (W + VEC - 1) / VEC;           // VEC==4 requires W % 4 == 0
+    const int nvec = (W + VEC - 1) / VEC;           // VEC==4 / 8 requires W % VEC == 0
     const int lpr = min(32, pow2_ceil(nvec));       // lanes per row
     const int rpw = 32 / lpr;                       // rows in flight per warp
     const int sub = lane / lpr, li = lane - sub * lpr;
-    const float* table = reinterpret_cast<const float*>(D.table);
+    // fp32, bf16 or fp16 rows (one type per launch); pooling is always fp32
+    const TabT* table = reinterpret_cast<const TabT*>(D.table);
     OutT* out_base = reinterpret_cast<OutT*>(dst.p[tc.d]);
     const int64_t i0 = tc.g0 - static_cast<int64_t>(tc.d) * dst_batch;
     const IdReader<IdT> rd = make_reader<IdT>(D, src, src_batch);
@@ -152,7 +156,7 @@ lookup_fwd_kernel(const InputDesc* __restrict__ descs, int n_inputs, int64_t bat
             const int64_t id = __shfl_sync(0xffffffffu, tile_id, r & 31);
             if (ok[u]) {
               if (static_cast<uint64_t>(id) < static_cast<uint64_t>(D.sub_rows)) {
-                acc[u] = ld_f32<VEC>(table + (D.row_base + id) * W + col);
+                acc[u] = ld_tab<TabT, VEC>(table + (D.row_base + id) * W + col);
               } else if (skip_empty) {
                 // row slices: another rank owns this id - unless it lies outside the whole
                 // table, then the first / last shard stores the zero row (flags 2 / 4)
@@ -178,7 +182,8 @@ lookup_fwd_kernel(const InputDesc* __restrict__ descs, int n_inputs, int64_t bat
           FVec<VEC> acc;
           acc.zero();
           int h = 0, hits = 0;
-          constexpr int kHotUnroll = 8;  // rows of one sample in flight
+          // rows of one sample in flight (16-byte rows of 8 columns: 4, or the fragments spill)
+          constexpr int kHotUnroll = VEC == 8 ? 4 : 8;
           for (; h + kHotUnroll <= n; h += kHotUnroll) {
             int64_t id[kHotUnroll];
             FVec<VEC> x[kHotUnroll];
@@ -189,7 +194,7 @@ lookup_fwd_kernel(const InputDesc* __restrict__ descs, int n_inputs, int64_t bat
             for (int u = 0; u < kHotUnroll; ++u) {
               x[u].zero();
               if (static_cast<uint64_t>(id[u]) < static_cast<uint64_t>(D.sub_rows)) {
-                x[u] = ld_f32<VEC>(table + (D.row_base + id[u]) * W + col);
+                x[u] = ld_tab<TabT, VEC>(table + (D.row_base + id[u]) * W + col);
                 ++hits;
               }
             }
@@ -199,7 +204,7 @@ lookup_fwd_kernel(const InputDesc* __restrict__ descs, int n_inputs, int64_t bat
           for (; h < n; ++h) {
             const int64_t id = static_cast<int64_t>(p[h]) + D.id_shift;
             if (static_cast<uint64_t>(id) < static_cast<uint64_t>(D.sub_rows)) {
-              acc.add(ld_f32<VEC>(table + (D.row_base + id) * W + col));
+              acc.add(ld_tab<TabT, VEC>(table + (D.row_base + id) * W + col));
               ++hits;
             }
           }
@@ -211,6 +216,28 @@ lookup_fwd_kernel(const InputDesc* __restrict__ descs, int n_inputs, int64_t bat
     }
   }
   sync_tail(sync);  // every pooled row of this rank is on its way: tell the requesters
+}
+
+// fp32 tables
+template <typename IdT, typename OutT, int VEC>
+__global__ void __launch_bounds__(kThreads, kBlocksPerSM)
+lookup_fwd_kernel(const InputDesc* __restrict__ descs, int n_inputs, int64_t batch,
+                  int64_t src_batch, int64_t dst_batch, int64_t dst_stride,
+                  const __grid_constant__ PeerPtrs src, const __grid_constant__ PeerPtrs dst,
+                  int rot, const __grid_constant__ SyncArgs sync, int ts) {
+  lookup_fwd_body<IdT, OutT, VEC, float>(descs, n_inputs, batch, src_batch, dst_batch,
+                                         dst_stride, src, dst, rot, sync, ts);
+}
+
+// bf16 / fp16 tables (TabT)
+template <typename IdT, typename OutT, int VEC, typename TabT>
+__global__ void __launch_bounds__(kThreads, fwd_blocks_per_sm(VEC))
+lookup_fwd_tab16_kernel(const InputDesc* __restrict__ descs, int n_inputs, int64_t batch,
+                        int64_t src_batch, int64_t dst_batch, int64_t dst_stride,
+                        const __grid_constant__ PeerPtrs src, const __grid_constant__ PeerPtrs dst,
+                        int rot, const __grid_constant__ SyncArgs sync, int ts) {
+  lookup_fwd_body<IdT, OutT, VEC, TabT>(descs, n_inputs, batch, src_batch, dst_batch, dst_stride,
+                                        src, dst, rot, sync, ts);
 }
 
 // =============================================================================== backward
@@ -519,35 +546,73 @@ int64_t count_tiles(int n_inputs, int64_t batch, int64_t dst_batch, int ts = kTi
 
 }  // namespace
 
-#define DE_DISPATCH_FWD(IdT, OutT, VEC)                                                        \
-  lookup_fwd_kernel<IdT, OutT, VEC><<<grid, kThreads, 0, stream>>>(                            \
-      descs, n_inputs, batch, src_batch, dst_batch, dst_stride, src, dst, rot, sync, ts)
-#define DE_DISPATCH_FWD_T(IdT, VEC)                                                            \
+// fp32 tables keep their own kernel; 16-bit tables take lookup_fwd_tab16_kernel
+template <typename IdT, typename OutT, int VEC, typename TabT>
+static void launch_fwd(int grid, cudaStream_t stream, const InputDesc* descs, int n_inputs,
+                       int64_t batch, int64_t src_batch, int64_t dst_batch, int64_t dst_stride,
+                       const PeerPtrs& src, const PeerPtrs& dst, int rot, const SyncArgs& sync,
+                       int ts) {
+  if constexpr (std::is_same<TabT, float>::value)
+    lookup_fwd_kernel<IdT, OutT, VEC><<<grid, kThreads, 0, stream>>>(
+        descs, n_inputs, batch, src_batch, dst_batch, dst_stride, src, dst, rot, sync, ts);
+  else
+    lookup_fwd_tab16_kernel<IdT, OutT, VEC, TabT><<<grid, kThreads, 0, stream>>>(
+        descs, n_inputs, batch, src_batch, dst_batch, dst_stride, src, dst, rot, sync, ts);
+}
+#define DE_DISPATCH_FWD(IdT, OutT, VEC, TabT)                                                  \
+  launch_fwd<IdT, OutT, VEC, TabT>(grid, stream, descs, n_inputs, batch, src_batch, dst_batch, \
+                                   dst_stride, src, dst, rot, sync, ts)
+#define DE_DISPATCH_FWD_T(IdT, VEC, TabT)                                                      \
   do {                                                                                         \
-    if (act_dtype == 1) DE_DISPATCH_FWD(IdT, __nv_bfloat16, VEC);                              \
-    else if (act_dtype == 2) DE_DISPATCH_FWD(IdT, __half, VEC);                                \
-    else DE_DISPATCH_FWD(IdT, float, VEC);                                                     \
+    if (act_dtype == 1) DE_DISPATCH_FWD(IdT, __nv_bfloat16, VEC, TabT);                        \
+    else if (act_dtype == 2) DE_DISPATCH_FWD(IdT, __half, VEC, TabT);                          \
+    else DE_DISPATCH_FWD(IdT, float, VEC, TabT);                                               \
   } while (0)
+#define DE_DISPATCH_FWD_ID(VEC, TabT)                                                          \
+  do {                                                                                         \
+    if (ids64) DE_DISPATCH_FWD_T(int64_t, VEC, TabT);                                          \
+    else DE_DISPATCH_FWD_T(int32_t, VEC, TabT);                                                \
+  } while (0)
+
+template <typename TabT>
+static void dispatch_fwd_half(int vec, const InputDesc* descs, int n_inputs, int64_t batch,
+                              int64_t src_batch, int64_t dst_batch, int64_t dst_stride,
+                              const PeerPtrs& src, const PeerPtrs& dst, int rot, bool ids64,
+                              int act_dtype, int grid, cudaStream_t stream, const SyncArgs& sync,
+                              int ts) {
+  // 16-bit rows: 8 columns (one 16-byte load) per lane where the widths allow it
+  if (vec == 8) DE_DISPATCH_FWD_ID(8, TabT);
+  else if (vec == 4) DE_DISPATCH_FWD_ID(4, TabT);
+  else DE_DISPATCH_FWD_ID(1, TabT);
+}
 
 void launch_lookup_fwd(const InputDesc* descs, int n_inputs, int64_t batch, int64_t src_batch,
                        int64_t dst_batch, int64_t dst_stride, const PeerPtrs& src,
                        const PeerPtrs& dst, int rot, bool ids64, int act_dtype, bool vec4,
                        int sm_count, cudaStream_t stream, const SyncArgs& sync,
-                       int tile_samples) {
+                       int tile_samples, int table_dtype, bool vec8) {
   if (n_inputs <= 0 || batch <= 0) {
     launch_sync_only(sync, stream);  // keep the signalling protocol in step
     return;
   }
   int ts = 1;
   while (ts * 2 <= tile_samples && ts < kTile) ts *= 2;  // power of two in [1, 32]
-  const int grid = grid_for(count_tiles(n_inputs, batch, dst_batch, ts), sm_count, kBlocksPerSM);
-  if (vec4) {
-    if (ids64) DE_DISPATCH_FWD_T(int64_t, 4);
-    else DE_DISPATCH_FWD_T(int32_t, 4);
-  } else {
-    if (ids64) DE_DISPATCH_FWD_T(int64_t, 1);
-    else DE_DISPATCH_FWD_T(int32_t, 1);
+  if (table_dtype != 0) {
+    const int vec = vec4 ? (vec8 ? 8 : 4) : 1;
+    const int grid = grid_for(count_tiles(n_inputs, batch, dst_batch, ts), sm_count,
+                              fwd_blocks_per_sm(vec));
+    if (table_dtype == 1)
+      dispatch_fwd_half<__nv_bfloat16>(vec, descs, n_inputs, batch, src_batch, dst_batch,
+                                       dst_stride, src, dst, rot, ids64, act_dtype, grid, stream,
+                                       sync, ts);
+    else
+      dispatch_fwd_half<__half>(vec, descs, n_inputs, batch, src_batch, dst_batch, dst_stride,
+                                src, dst, rot, ids64, act_dtype, grid, stream, sync, ts);
+    return;
   }
+  const int grid = grid_for(count_tiles(n_inputs, batch, dst_batch, ts), sm_count, kBlocksPerSM);
+  if (vec4) DE_DISPATCH_FWD_ID(4, float);
+  else DE_DISPATCH_FWD_ID(1, float);
 }
 
 #define DE_DISPATCH_BWD(IdT, GradT, VEC)                                                       \

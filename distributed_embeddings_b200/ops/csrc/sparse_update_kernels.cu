@@ -92,13 +92,30 @@ __device__ __forceinline__ void resolve_step(OptimizerArgs& opt) {
   }
 }
 
+// The step that keys the stochastic rounding of 16-bit tables: the same device-resident count
+// (fp32 tables do not use it, and their kernels never read it).  The count is an fp32 word that
+// advances by 1.0 per step, exact up to 2^24 = 16.7 M steps; beyond that it stops changing and
+// every later step would draw the same bits for a given (row, column), which biases the rounding.
+// Runs that long need an integer counter here.
+template <typename TabT>
+__device__ __forceinline__ uint32_t rounding_step(const OptimizerArgs& opt) {
+  if constexpr (sizeof(TabT) == 2) {
+    return opt.step_ptr != nullptr ? static_cast<uint32_t>(*opt.step_ptr) : 0u;
+  } else {
+    return 0u;
+  }
+}
+
 // ------------------------------------------------------------------ per-row optimizer apply
-template <int VEC>
+// The weight is read in its storage type (TabT: fp32, bf16 or fp16), the optimizer runs in fp32
+// on fp32 state, and a 16-bit weight is written back with stochastic rounding (st_tab).  Every
+// row has exactly one writer per step, so each element is rounded once.
+template <typename TabT, int VEC>
 __device__ __forceinline__ void apply_update(const TableDesc& T, const OptimizerArgs& opt,
                                              int64_t row, int col, const FVec<VEC>& g,
-                                             float row_sumsq_mean) {
-  float* w = reinterpret_cast<float*>(T.weight) + row * T.width + col;
-  FVec<VEC> wv = ld_f32_rw<VEC>(w);
+                                             float row_sumsq_mean, uint32_t step) {
+  TabT* w = reinterpret_cast<TabT*>(T.weight) + row * T.width + col;
+  FVec<VEC> wv = ld_tab_rw<TabT, VEC>(w);
   FVec<VEC> gv = g;
   if (opt.weight_decay != 0.f) gv.fma(opt.weight_decay, wv);
   if (opt.kind == kOptSGD) {
@@ -132,7 +149,7 @@ __device__ __forceinline__ void apply_update(const TableDesc& T, const Optimizer
     st_f32<VEC>(m, mv);
     st_f32<VEC>(v, vv);
   }
-  st_f32<VEC>(w, wv);
+  st_tab<TabT, VEC>(w, wv, step, T.key_base + row, col);
 }
 
 // Sum of the gradient rows of one unique key restricted to this lane's columns.
@@ -185,19 +202,18 @@ __device__ __forceinline__ FVec<VEC> reduce_segment(const InputDesc* __restrict_
   return acc;
 }
 
-template <typename GradT, int VEC>
-__global__ void __launch_bounds__(kThreads)
-segment_update_kernel(const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables,
-                      int n_tables, int lpr, int64_t batch, int64_t grad_batch,
-                      int64_t grad_stride, const __grid_constant__ PeerPtrs grad,
-                      const int64_t* __restrict__ sorted_keys,
-                      const uint32_t* __restrict__ sorted_items,
-                      const int64_t* __restrict__ seg_start, const int64_t* __restrict__ n_unique_p,
-                      const __grid_constant__ OptimizerArgs opt_in, int64_t* __restrict__ emit_keys,
-                      float* __restrict__ emit_rows, int emit_width) {
+template <typename GradT, int VEC, typename TabT>
+__device__ __forceinline__ void segment_update_body(
+    const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables, int n_tables,
+    int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride, const PeerPtrs& grad,
+    const int64_t* __restrict__ sorted_keys, const uint32_t* __restrict__ sorted_items,
+    const int64_t* __restrict__ seg_start, const int64_t* __restrict__ n_unique_p,
+    const OptimizerArgs& opt_in, int64_t* __restrict__ emit_keys, float* __restrict__ emit_rows,
+    int emit_width) {
   OptimizerArgs opt = opt_in;
   if (opt.lr_ptr != nullptr) opt.lr = *opt.lr_ptr;
   resolve_step(opt);
+  const uint32_t sr_step = rounding_step<TabT>(opt);
   const int64_t n_unique = *n_unique_p;
   const int64_t sentinel = tables[n_tables - 1].key_base + tables[n_tables - 1].rows;
   const int lane = threadIdx.x & 31;
@@ -267,10 +283,36 @@ segment_update_kernel(const InputDesc* __restrict__ descs, const TableDesc* __re
       if (opt.kind == kOptEmit) {
         st_f32<VEC>(emit_rows + u * emit_width + col, g);
       } else {
-        apply_update<VEC>(T, opt, row, col, g, row_state);
+        apply_update<TabT, VEC>(T, opt, row, col, g, row_state, sr_step);
       }
     }
   }
+}
+
+// fp32 tables
+template <typename GradT, int VEC>
+__global__ void __launch_bounds__(kThreads) segment_update_kernel(const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables,
+    int n_tables, int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
+    const __grid_constant__ PeerPtrs grad, const int64_t* __restrict__ sorted_keys,
+    const uint32_t* __restrict__ sorted_items, const int64_t* __restrict__ seg_start,
+    const int64_t* __restrict__ n_unique_p, const __grid_constant__ OptimizerArgs opt_in,
+    int64_t* __restrict__ emit_keys, float* __restrict__ emit_rows, int emit_width) {
+  segment_update_body<GradT, VEC, float>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
+                                     sorted_keys, sorted_items, seg_start, n_unique_p, opt_in,
+                                     emit_keys, emit_rows, emit_width);
+}
+
+// bf16 / fp16 tables (TabT)
+template <typename GradT, int VEC, typename TabT>
+__global__ void __launch_bounds__(kThreads) segment_update_tab16_kernel(const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables,
+    int n_tables, int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
+    const __grid_constant__ PeerPtrs grad, const int64_t* __restrict__ sorted_keys,
+    const uint32_t* __restrict__ sorted_items, const int64_t* __restrict__ seg_start,
+    const int64_t* __restrict__ n_unique_p, const __grid_constant__ OptimizerArgs opt_in,
+    int64_t* __restrict__ emit_keys, float* __restrict__ emit_rows, int emit_width) {
+  segment_update_body<GradT, VEC, TabT>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
+                                     sorted_keys, sorted_items, seg_start, n_unique_p, opt_in,
+                                     emit_keys, emit_rows, emit_width);
 }
 
 // ------------------------------------------------------------------ occurrence-balanced update
@@ -328,9 +370,10 @@ __device__ __forceinline__ int find_table(const TableDesc* __restrict__ tables, 
 }
 
 // Apply the optimizer to one row given the complete (scaled) gradient fragment of this lane.
+template <typename TabT>
 __device__ __forceinline__ void apply_row(const TableDesc& T, const OptimizerArgs& opt,
                                           int64_t row, int col, FVec<4> g, int lpr,
-                                          unsigned group_mask) {
+                                          unsigned group_mask, uint32_t step) {
   const bool col_ok = col < T.width;
   float row_state = 0.f;
   if (opt.kind == kOptRowwiseAdagrad) {
@@ -345,23 +388,20 @@ __device__ __forceinline__ void apply_row(const TableDesc& T, const OptimizerArg
     __syncwarp(group_mask);
     if (col == 0) *st = row_state;
   }
-  if (col_ok) apply_update<4>(T, opt, row, col, g, row_state);
+  if (col_ok) apply_update<TabT, 4>(T, opt, row, col, g, row_state, step);
 }
 
-template <typename GradT>
-__global__ void __launch_bounds__(kThreads)
-balanced_update_kernel(const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables,
-                       int n_tables, int lpr, int64_t batch, int64_t grad_batch,
-                       int64_t grad_stride, const __grid_constant__ PeerPtrs grad,
-                       const int64_t* __restrict__ sorted_keys,
-                       const uint32_t* __restrict__ sorted_items, int64_t n_items,
-                       const int64_t* __restrict__ seg_start,
-                       const int64_t* __restrict__ n_unique_p,
-                       const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch,
-                       int scratch_width) {
+template <typename GradT, typename TabT>
+__device__ __forceinline__ void balanced_update_body(
+    const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables, int n_tables,
+    int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride, const PeerPtrs& grad,
+    const int64_t* __restrict__ sorted_keys, const uint32_t* __restrict__ sorted_items,
+    int64_t n_items, const int64_t* __restrict__ seg_start, const int64_t* __restrict__ n_unique_p,
+    const OptimizerArgs& opt_in, float* __restrict__ scratch, int scratch_width) {
   OptimizerArgs opt = opt_in;
   if (opt.lr_ptr != nullptr) opt.lr = *opt.lr_ptr;
   resolve_step(opt);
+  const uint32_t sr_step = rounding_step<TabT>(opt);
   const int64_t n_unique = *n_unique_p;
   const int64_t sentinel = tables[n_tables - 1].key_base + tables[n_tables - 1].rows;
   const int lane = threadIdx.x & 31;
@@ -413,7 +453,7 @@ balanced_update_kernel(const InputDesc* __restrict__ descs, const TableDesc* __r
             FVec<4> g = acc;
             g.scale(opt.grad_scale);
             if (start_done) {
-              apply_row(T, opt, run_key - T.key_base, col, g, lpr, group_mask);
+              apply_row<TabT>(T, opt, run_key - T.key_base, col, g, lpr, group_mask, sr_step);
             } else if (col < T.width) {
               // continues a segment that started in an earlier chunk: that chunk owns the slot
               const int64_t s = segment_start_of(seg_start, n_unique, k0);
@@ -436,7 +476,7 @@ balanced_update_kernel(const InputDesc* __restrict__ descs, const TableDesc* __r
       FVec<4> g = acc;
       g.scale(opt.grad_scale);
       if (start_done && end_done) {
-        apply_row(T, opt, run_key - T.key_base, col, g, lpr, group_mask);
+        apply_row<TabT>(T, opt, run_key - T.key_base, col, g, lpr, group_mask, sr_step);
       } else if (col < T.width) {
         const int64_t s = start_done ? run_start : segment_start_of(seg_start, n_unique, k0);
         red_add_f32<4>(scratch + (s / kChunk) * scratch_width + col, g);
@@ -447,14 +487,39 @@ balanced_update_kernel(const InputDesc* __restrict__ descs, const TableDesc* __r
 
 // One lane group per chunk: if a segment that crosses the chunk's end border starts in this chunk,
 // its complete gradient sits in the chunk's scratch row: apply it, then clear the row.
-__global__ void __launch_bounds__(kThreads)
-finalize_crossing_kernel(const TableDesc* __restrict__ tables, int n_tables, int lpr,
-                         const int64_t* __restrict__ sorted_keys, int64_t n_items,
-                         const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch,
-                         int scratch_width) {
+template <typename GradT>
+__global__ void __launch_bounds__(kThreads) balanced_update_kernel(const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables,
+    int n_tables, int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
+    const __grid_constant__ PeerPtrs grad, const int64_t* __restrict__ sorted_keys,
+    const uint32_t* __restrict__ sorted_items, int64_t n_items,
+    const int64_t* __restrict__ seg_start, const int64_t* __restrict__ n_unique_p,
+    const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch, int scratch_width) {
+  balanced_update_body<GradT, float>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
+                                    sorted_keys, sorted_items, n_items, seg_start, n_unique_p,
+                                    opt_in, scratch, scratch_width);
+}
+
+template <typename GradT, typename TabT>
+__global__ void __launch_bounds__(kThreads) balanced_update_tab16_kernel(const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables,
+    int n_tables, int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
+    const __grid_constant__ PeerPtrs grad, const int64_t* __restrict__ sorted_keys,
+    const uint32_t* __restrict__ sorted_items, int64_t n_items,
+    const int64_t* __restrict__ seg_start, const int64_t* __restrict__ n_unique_p,
+    const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch, int scratch_width) {
+  balanced_update_body<GradT, TabT>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
+                                    sorted_keys, sorted_items, n_items, seg_start, n_unique_p,
+                                    opt_in, scratch, scratch_width);
+}
+
+template <typename TabT>
+__device__ __forceinline__ void finalize_crossing_body(
+    const TableDesc* __restrict__ tables, int n_tables, int lpr,
+    const int64_t* __restrict__ sorted_keys, int64_t n_items, const OptimizerArgs& opt_in,
+    float* __restrict__ scratch, int scratch_width) {
   OptimizerArgs opt = opt_in;
   if (opt.lr_ptr != nullptr) opt.lr = *opt.lr_ptr;
   resolve_step(opt);
+  const uint32_t sr_step = rounding_step<TabT>(opt);
   const int64_t sentinel = tables[n_tables - 1].key_base + tables[n_tables - 1].rows;
   const int lane = threadIdx.x & 31;
   const int rpw = 32 / lpr;
@@ -484,8 +549,25 @@ finalize_crossing_kernel(const TableDesc* __restrict__ tables, int n_tables, int
       z.zero();
       st_f32<4>(sp, z);
     }
-    apply_row(T, opt, key - T.key_base, col, g, lpr, group_mask);
+    apply_row<TabT>(T, opt, key - T.key_base, col, g, lpr, group_mask, sr_step);
   }
+}
+
+__global__ void __launch_bounds__(kThreads)
+finalize_crossing_kernel(const TableDesc* __restrict__ tables, int n_tables, int lpr,
+                         const int64_t* __restrict__ sorted_keys, int64_t n_items,
+                         const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch,
+                         int scratch_width) {
+  finalize_crossing_body<float>(tables, n_tables, lpr, sorted_keys, n_items, opt_in, scratch, scratch_width);
+}
+
+template <typename TabT>
+__global__ void __launch_bounds__(kThreads)
+finalize_crossing_tab16_kernel(const TableDesc* __restrict__ tables, int n_tables, int lpr,
+                         const int64_t* __restrict__ sorted_keys, int64_t n_items,
+                         const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch,
+                         int scratch_width) {
+  finalize_crossing_body<TabT>(tables, n_tables, lpr, sorted_keys, n_items, opt_in, scratch, scratch_width);
 }
 
 int grid_cap(int64_t work_warps, int sm_count, int per_sm) {
@@ -557,10 +639,38 @@ void unique_segments(void* temp, size_t temp_bytes, const int64_t* sorted_keys, 
   finish_segments_kernel<<<1, 32, 0, stream>>>(seg_start, n_unique, n);
 }
 
-#define DE_DISPATCH_SEG(GradT, VEC)                                                            \
-  segment_update_kernel<GradT, VEC><<<grid, kThreads, 0, stream>>>(                            \
-      descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,         \
-      sorted_items, seg_start, n_unique, opt, emit_keys, emit_rows, emit_width)
+template <typename GradT, int VEC, typename TabT>
+static void launch_seg(int grid, cudaStream_t stream, const InputDesc* descs,
+                       const TableDesc* tables, int n_tables, int lpr, int64_t batch,
+                       int64_t grad_batch, int64_t grad_stride, const PeerPtrs& grad,
+                       const int64_t* sorted_keys, const uint32_t* sorted_items,
+                       const int64_t* seg_start, const int64_t* n_unique,
+                       const OptimizerArgs& opt, int64_t* emit_keys, float* emit_rows,
+                       int emit_width) {
+  if constexpr (std::is_same<TabT, float>::value)
+    segment_update_kernel<GradT, VEC><<<grid, kThreads, 0, stream>>>(
+        descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
+        sorted_items, seg_start, n_unique, opt, emit_keys, emit_rows, emit_width);
+  else
+    segment_update_tab16_kernel<GradT, VEC, TabT><<<grid, kThreads, 0, stream>>>(
+        descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
+        sorted_items, seg_start, n_unique, opt, emit_keys, emit_rows, emit_width);
+}
+#define DE_DISPATCH_SEG(GradT, VEC, TabT)                                                      \
+  launch_seg<GradT, VEC, TabT>(grid, stream, descs, tables, n_tables, lpr, batch, grad_batch,  \
+                               grad_stride, grad, sorted_keys, sorted_items, seg_start,        \
+                               n_unique, opt, emit_keys, emit_rows, emit_width)
+#define DE_DISPATCH_SEG_G(VEC, TabT)                                                           \
+  do {                                                                                         \
+    if (act_dtype == 1) DE_DISPATCH_SEG(__nv_bfloat16, VEC, TabT);                             \
+    else if (act_dtype == 2) DE_DISPATCH_SEG(__half, VEC, TabT);                               \
+    else DE_DISPATCH_SEG(float, VEC, TabT);                                                    \
+  } while (0)
+#define DE_DISPATCH_SEG_V(TabT)                                                                \
+  do {                                                                                         \
+    if (vec4) DE_DISPATCH_SEG_G(4, TabT);                                                      \
+    else DE_DISPATCH_SEG_G(1, TabT);                                                           \
+  } while (0)
 
 void launch_segment_update(const InputDesc* descs, const TableDesc* tables, int n_tables,
                            int64_t batch, int64_t grad_batch, int64_t grad_stride,
@@ -568,7 +678,7 @@ void launch_segment_update(const InputDesc* descs, const TableDesc* tables, int 
                            const uint32_t* sorted_items, const int64_t* seg_start,
                            const int64_t* n_unique, int64_t n_items, const OptimizerArgs& opt,
                            int64_t* emit_keys, float* emit_rows, int max_width, int act_dtype,
-                           bool vec4, int sm_count, cudaStream_t stream) {
+                           bool vec4, int sm_count, cudaStream_t stream, int table_dtype) {
   const int emit_width = max_width;
   if (n_items <= 0 || n_tables <= 0) return;
   // lanes per row from the widest table of this launch (narrower tables leave lanes idle)
@@ -582,15 +692,57 @@ void launch_segment_update(const InputDesc* descs, const TableDesc* tables, int 
   const int rpw = 32 / lpr;
   const int64_t warps = (n_items + rpw - 1) / rpw;
   const int grid = grid_cap(warps, sm_count, 8);
-  if (vec4) {
-    if (act_dtype == 1) DE_DISPATCH_SEG(__nv_bfloat16, 4);
-    else if (act_dtype == 2) DE_DISPATCH_SEG(__half, 4);
-    else DE_DISPATCH_SEG(float, 4);
-  } else {
-    if (act_dtype == 1) DE_DISPATCH_SEG(__nv_bfloat16, 1);
-    else if (act_dtype == 2) DE_DISPATCH_SEG(__half, 1);
-    else DE_DISPATCH_SEG(float, 1);
-  }
+  // the emit path never touches the table: one instantiation serves every storage type
+  if (table_dtype == 1 && opt.kind != kOptEmit) DE_DISPATCH_SEG_V(__nv_bfloat16);
+  else if (table_dtype == 2 && opt.kind != kOptEmit) DE_DISPATCH_SEG_V(__half);
+  else DE_DISPATCH_SEG_V(float);
+}
+
+template <typename GradT, typename TabT>
+static void launch_balanced_g(const InputDesc* descs, const TableDesc* tables, int n_tables,
+                              int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
+                              const PeerPtrs& grad, const int64_t* sorted_keys,
+                              const uint32_t* sorted_items, int64_t n_items,
+                              const int64_t* seg_start, const int64_t* n_unique,
+                              const OptimizerArgs& opt, float* scratch, int scratch_width,
+                              int grid, cudaStream_t stream) {
+  if constexpr (std::is_same<TabT, float>::value)
+    balanced_update_kernel<GradT><<<grid, kThreads, 0, stream>>>(
+        descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
+        sorted_items, n_items, seg_start, n_unique, opt, scratch, scratch_width);
+  else
+    balanced_update_tab16_kernel<GradT, TabT><<<grid, kThreads, 0, stream>>>(
+        descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
+        sorted_items, n_items, seg_start, n_unique, opt, scratch, scratch_width);
+}
+
+template <typename TabT>
+static void launch_balanced(const InputDesc* descs, const TableDesc* tables, int n_tables, int lpr,
+                            int64_t batch, int64_t grad_batch, int64_t grad_stride,
+                            const PeerPtrs& grad, const int64_t* sorted_keys,
+                            const uint32_t* sorted_items, int64_t n_items,
+                            const int64_t* seg_start, const int64_t* n_unique,
+                            const OptimizerArgs& opt, float* scratch, int scratch_width,
+                            int act_dtype, int grid, cudaStream_t stream) {
+  if (act_dtype == 1)
+    launch_balanced_g<__nv_bfloat16, TabT>(descs, tables, n_tables, lpr, batch, grad_batch,
+                                           grad_stride, grad, sorted_keys, sorted_items, n_items,
+                                           seg_start, n_unique, opt, scratch, scratch_width, grid,
+                                           stream);
+  else if (act_dtype == 2)
+    launch_balanced_g<__half, TabT>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride,
+                                    grad, sorted_keys, sorted_items, n_items, seg_start, n_unique,
+                                    opt, scratch, scratch_width, grid, stream);
+  else
+    launch_balanced_g<float, TabT>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride,
+                                   grad, sorted_keys, sorted_items, n_items, seg_start, n_unique,
+                                   opt, scratch, scratch_width, grid, stream);
+  if constexpr (std::is_same<TabT, float>::value)
+    finalize_crossing_kernel<<<grid, kThreads, 0, stream>>>(tables, n_tables, lpr, sorted_keys,
+                                                            n_items, opt, scratch, scratch_width);
+  else
+    finalize_crossing_tab16_kernel<TabT><<<grid, kThreads, 0, stream>>>(
+        tables, n_tables, lpr, sorted_keys, n_items, opt, scratch, scratch_width);
 }
 
 // Occurrence-balanced variant (vec4, tables up to 128 columns wide, fused optimizers only).
@@ -602,7 +754,8 @@ bool launch_balanced_update(const InputDesc* descs, const TableDesc* tables, int
                             const uint32_t* sorted_items, int64_t n_items,
                             const int64_t* seg_start, const int64_t* n_unique,
                             const OptimizerArgs& opt, float* scratch, int scratch_width,
-                            int max_width, int act_dtype, int sm_count, cudaStream_t stream) {
+                            int max_width, int act_dtype, int sm_count, cudaStream_t stream,
+                            int table_dtype) {
   if (n_items <= 0 || n_tables <= 0) return true;
   if (max_width > 128 || max_width % 4 || scratch_width % 4 || opt.kind == kOptEmit) return false;
   int lpr = 1;
@@ -610,20 +763,18 @@ bool launch_balanced_update(const InputDesc* descs, const TableDesc* tables, int
   const int rpw = 32 / lpr;
   const int64_t n_chunks = (n_items + kChunk - 1) / kChunk;
   const int grid = grid_cap((n_chunks + rpw - 1) / rpw, sm_count, 8);
-  if (act_dtype == 1)
-    balanced_update_kernel<__nv_bfloat16><<<grid, kThreads, 0, stream>>>(
-        descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
-        sorted_items, n_items, seg_start, n_unique, opt, scratch, scratch_width);
-  else if (act_dtype == 2)
-    balanced_update_kernel<__half><<<grid, kThreads, 0, stream>>>(
-        descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
-        sorted_items, n_items, seg_start, n_unique, opt, scratch, scratch_width);
+  if (table_dtype == 1)
+    launch_balanced<__nv_bfloat16>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride,
+                                   grad, sorted_keys, sorted_items, n_items, seg_start, n_unique,
+                                   opt, scratch, scratch_width, act_dtype, grid, stream);
+  else if (table_dtype == 2)
+    launch_balanced<__half>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
+                            sorted_keys, sorted_items, n_items, seg_start, n_unique, opt, scratch,
+                            scratch_width, act_dtype, grid, stream);
   else
-    balanced_update_kernel<float><<<grid, kThreads, 0, stream>>>(
-        descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
-        sorted_items, n_items, seg_start, n_unique, opt, scratch, scratch_width);
-  finalize_crossing_kernel<<<grid, kThreads, 0, stream>>>(tables, n_tables, lpr, sorted_keys,
-                                                          n_items, opt, scratch, scratch_width);
+    launch_balanced<float>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
+                           sorted_keys, sorted_items, n_items, seg_start, n_unique, opt, scratch,
+                           scratch_width, act_dtype, grid, stream);
   return cudaGetLastError() == cudaSuccess;
 }
 

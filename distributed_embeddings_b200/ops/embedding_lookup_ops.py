@@ -41,16 +41,18 @@ def _sample_ids_cpu(values, offsets, hotness, batch):
 
 
 def _lookup_fwd_cpu(param, values, offsets, hotness, batch, combiner):
+  """Pooled in fp32 whatever the table dtype; the result has the table's dtype."""
   rows, width = param.shape
   flat = values.reshape(-1).to(torch.int64)
   sample, counts = _sample_ids_cpu(flat, offsets, hotness, batch)
   ok = (flat >= 0) & (flat < rows)
-  gathered = param[flat.clamp(0, rows - 1)] * ok.unsqueeze(1).to(param.dtype)
-  out = torch.zeros(batch, width, dtype=param.dtype, device=param.device)
+  acc = torch.float32 if param.dtype in (torch.bfloat16, torch.float16) else param.dtype
+  gathered = param[flat.clamp(0, rows - 1)].to(acc) * ok.unsqueeze(1).to(acc)
+  out = torch.zeros(batch, width, dtype=acc, device=param.device)
   out.index_add_(0, sample, gathered)
   if combiner == 1:
-    out = out / counts.clamp(min=1).unsqueeze(1).to(param.dtype)
-  return out
+    out = out / counts.clamp(min=1).unsqueeze(1).to(acc)
+  return out.to(param.dtype)
 
 
 def _lookup_grad_cpu(values, offsets, hotness, batch, combiner, grad, num_rows):

@@ -225,6 +225,13 @@ class DistributedEmbedding(nn.Module):
     device / process_group / backend / compute_dtype: execution placement (keyword only).
       ``compute_dtype`` is the dtype of the returned activations (bf16 halves the bytes on the
       wire like the reference's mixed precision mode, dist_model_parallel.py:866).
+    table_dtype: storage dtype of the model-parallel tables (table-parallel, column slices, row
+      slices, CPU-offloaded tables): ``torch.float32`` (default), ``torch.bfloat16`` or
+      ``torch.float16`` (keyword only).  Half-precision tables take half the memory; rows are
+      pooled in fp32, the optimizer and its state stay fp32 and the new weights are written back
+      with stochastic rounding (``ops/stochastic_rounding.py``).  Replicated tables stay fp32.
+      The ``dtype`` of a passed ``Embedding`` layer or config is ignored here, as it always was.
+      Checkpoints (``get_weights`` / ``save_weights``) are fp32 whatever the table dtype.
   """
 
   def __init__(self,
@@ -243,10 +250,15 @@ class DistributedEmbedding(nn.Module):
                compute_dtype: Optional[torch.dtype] = None,
                rank: Optional[int] = None,
                world_size: Optional[int] = None,
-               input_hotness: Optional[Sequence[int]] = None):
+               input_hotness: Optional[Sequence[int]] = None,
+               table_dtype: torch.dtype = torch.float32):
     super().__init__()
     if strategy not in STRATEGIES:
       raise ValueError(f"Unsupported shard strategy {strategy}")
+    if table_dtype not in (torch.float32, torch.bfloat16, torch.float16):
+      raise ValueError(f"table_dtype must be torch.float32, torch.bfloat16 or torch.float16, "
+                       f"got {table_dtype}")
+    self.table_dtype = table_dtype
     self.group = process_group
     if world_size is None:
       world_size = dist.get_world_size(process_group) if dist_ready() else 1
@@ -360,7 +372,11 @@ class DistributedEmbedding(nn.Module):
         config["use_custom_kernel"] = False
       if not local:
         config["sparse_grad"] = False  # replicated tables are all-reduced as dense gradients
-      layer = layer_type.from_config(config, device=dev)
+      if local and self.table_dtype != torch.float32:
+        # created in the table dtype directly: no transient fp32 copy of a large table
+        layer = layer_type.from_config(config, device=dev, dtype=self.table_dtype)
+      else:
+        layer = layer_type.from_config(config, device=dev)
       if offloaded and torch.cuda.is_available():
         layer.embeddings.data = layer.embeddings.data.pin_memory()
     else:
@@ -615,20 +631,21 @@ class DistributedEmbedding(nn.Module):
       return group_rank
     return dist.get_global_rank(self.group, group_rank)
 
-  def get_weights(self, all_ranks: bool = False) -> List[np.ndarray]:
+  def get_weights(self, all_ranks: bool = False, chunk: int = 1 << 26) -> List[np.ndarray]:
     """Return the *global, unsharded* tables as numpy arrays in original table order.
 
     The layout is independent of the sharding: a checkpoint written with 8 column-sliced ranks
     loads on one GPU.  Only rank 0 receives the arrays unless ``all_ranks`` (other ranks get an
-    empty list for the model-parallel tables they do not own).
+    empty list for the model-parallel tables they do not own).  Shards are read (and cast to
+    fp32) in pieces of at most ``chunk`` elements.
     """
     weights = self.weights
     n_dp, n_col = len(self.dp_layers), len(self.local_embedding_layers)
     return self._gather_global(weights[:n_dp], weights[n_dp:n_dp + n_col],
-                               weights[n_dp + n_col:], all_ranks)
+                               weights[n_dp + n_col:], all_ranks, chunk=chunk)
 
   def _gather_global(self, dp_tensors, col_tensors, row_tensors, all_ranks: bool,
-                     per_row: bool = False) -> List[Optional[np.ndarray]]:
+                     per_row: bool = False, chunk: int = 1 << 26) -> List[Optional[np.ndarray]]:
     """Assemble global per-table arrays from this rank's local tensors (one per replicated
     layer / fused local table / row shard; ``None`` entries of ``dp_tensors`` are skipped).
     ``per_row``: the local tensors hold one value per row (row-wise optimizer state); the column
@@ -657,11 +674,11 @@ class DistributedEmbedding(nn.Module):
             if src is not None:
               src = src.reshape(-1, 1)
             part = np.empty((s.rows, 1), dtype=np.float32) if collect else None
-            self._bcast_rows(src, s.rows, 1, r, part, 0)
+            self._bcast_rows(src, s.rows, 1, r, part, 0, chunk)
             if out is not None:
               out += part * (s.width / width)
           else:
-            self._bcast_rows(src, s.rows, s.width, r, out, s.col_start)
+            self._bcast_rows(src, s.rows, s.width, r, out, s.col_start, chunk)
       result[t] = out
     for gt, t in enumerate(st.table_groups[2]):
       cfg = st.global_configs[t]
@@ -673,7 +690,7 @@ class DistributedEmbedding(nn.Module):
         if src is not None and per_row:
           src = src.reshape(-1, 1)
         sub = out[lo:hi] if out is not None else None
-        self._bcast_rows(src, hi - lo, w_out, r, sub, 0)
+        self._bcast_rows(src, hi - lo, w_out, r, sub, 0, chunk)
       result[t] = out
     if not collect:
       return []

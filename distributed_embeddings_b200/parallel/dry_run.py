@@ -32,6 +32,7 @@ import numpy as np
 import torch
 
 from ..ops._native import GRAD_ROUTE, INPUT_DESC, MAX_PEERS, TABLE_DESC
+from ..ops.stochastic_rounding import stochastic_round
 from . import fused as _fused
 
 
@@ -242,10 +243,13 @@ class DryOps:
                                      hot, "peer ids"))
     return torch.cat(parts).to(torch.int64), torch.full((g1 - g0,), hot, dtype=torch.int64)
 
-  def _table(self, d) -> torch.Tensor:
+  def _table(self, d, table_dtype: int = 0) -> torch.Tensor:
+    """The rows a descriptor may address, in the launch's table dtype (bounds-checked at its
+    element size)."""
     w = int(d["width"])
     rows = int(d["row_base"]) + int(d["sub_rows"])
-    return self.world.tensor(int(d["table"]), torch.float32, rows * w, "table").view(rows, w)
+    return self.world.tensor(int(d["table"]), self._ADT[int(table_dtype)], rows * w,
+                             "table").view(rows, w)
 
   @staticmethod
   def _pool_index(lens: torch.Tensor) -> torch.Tensor:
@@ -253,9 +257,11 @@ class DryOps:
 
   # -- forward -------------------------------------------------------------------------------
   def lookup_fwd(self, descs, n_inputs, batch, src_batch, dst_batch, dst_stride, src_ptrs,
-                 dst_ptrs, rot, ids64, act_dtype, vec4, sync, tile_samples=32):
+                 dst_ptrs, rot, ids64, act_dtype, vec4, sync, tile_samples=32, table_dtype=0,
+                 vec8=False):
     self._count("lookup_fwd")
     assert 1 <= tile_samples <= 32
+    assert not vec8 or (vec4 and int(table_dtype) != 0), "vec8 is for 16-bit tables with vec4"
     self._wait(sync)
     odt = self._ADT[int(act_dtype)]
     osz = 4 if int(act_dtype) == 0 else 2
@@ -263,7 +269,10 @@ class DryOps:
       width, col = int(d["width"]), int(d["dst_col"])
       if vec4:
         assert width % 4 == 0 and col % 4 == 0 and dst_stride % 4 == 0, "vec4 alignment"
-      table = self._table(d)
+      if vec8:
+        assert width % 8 == 0 and col % 8 == 0 and dst_stride % 8 == 0, "vec8 alignment"
+        assert int(d["table"]) % 16 == 0, "vec8: 16-byte aligned table"
+      table = self._table(d, table_dtype).float()  # rows are pooled in fp32
       for dd in range(-(-batch // dst_batch)):
         g0, g1 = dd * dst_batch, min(batch, (dd + 1) * dst_batch)
         ns = g1 - g0
@@ -462,11 +471,16 @@ class DryOps:
   def segment_update(self, descs, tables, n_tables, batch, grad_batch, grad_stride, grad_ptrs,
                      keys, items, seg, n_unique, kind, lr, eps, beta1, beta2, bias1, bias2,
                      grad_scale, weight_decay, lr_ptr, emit_keys, emit_rows, max_width, act_dtype,
-                     vec4, scratch, step_ptr):
+                     vec4, scratch, step_ptr, table_dtype=0):
     self._count("segment_update")
-    if step_ptr and kind == 3:
-      t = float(self.world.tensor(int(step_ptr), torch.float32, 1, "adam step")[0])
-      bias1, bias2 = 1.0 - beta1**t, 1.0 - beta2**t
+    tdt = self._ADT[int(table_dtype)]
+    tsz = 4 if int(table_dtype) == 0 else 2
+    step = 0
+    if step_ptr:
+      t = float(self.world.tensor(int(step_ptr), torch.float32, 1, "optimizer step")[0])
+      step = int(t)
+      if kind == 3:
+        bias1, bias2 = 1.0 - beta1**t, 1.0 - beta2**t
     D = self._descs(descs, 1 << 30)
     T = self._descs(tables, n_tables, TABLE_DESC)
     if lr_ptr:
@@ -508,7 +522,10 @@ class DryOps:
         emit_keys[u] = key
         emit_rows[u, :width] = g
         continue
-      wt = self.world.tensor(int(t["weight"]) + row * width * 4, torch.float32, width, "weight")
+      wt = self.world.tensor(int(t["weight"]) + row * width * tsz, tdt, width, "weight")
+      if tsz == 2:
+        # 16-bit table: fp32 math on an fp32 copy of the row, stochastic rounding back
+        w16, wt = wt, wt.float()
       if weight_decay:
         g = g + weight_decay * wt
       if kind == 0:
@@ -529,6 +546,8 @@ class DryOps:
         wt -= lr * (mm / bias1) / ((vv / bias2).sqrt() + eps)
       else:
         raise ValueError(f"optimizer kind {kind}")
+      if tsz == 2:
+        w16.copy_(stochastic_round(wt, tdt, step, key))
 
 
 class DryRank:

@@ -131,6 +131,9 @@ class FusedEngine:
     if self.compute_dtype not in DTYPE_CODE:
       raise ValueError("fused back end supports fp32, bf16 and fp16 activations")
     self.act = DTYPE_CODE[self.compute_dtype]  # dtype code of activations / gradients on the wire
+    # storage of the model-parallel tables (one dtype for all of them); replicated tables are fp32
+    self.table_dtype = getattr(de, "table_dtype", torch.float32)
+    self.tab = DTYPE_CODE[self.table_dtype]
     self._key = None
     self._gen = 0          # forward generation (see _FusedFn)
     self._pending = None   # weakref to the autograd node of the last forward
@@ -618,6 +621,11 @@ class FusedEngine:
             list(ddesc["dst_col"]) + list(mp["dst_col"])]
     self.vec4 = all(w % 4 == 0 for w in widths) and all(c % 4 == 0 for c in cols) and \
         tw % 4 == 0 and self.rs_width % 4 == 0 and self.recv_width % 4 == 0 and ostride % 4 == 0
+    # 16-bit tables: 8 columns (one 16-byte load) per lane in the model-parallel lookups
+    fw = [int(x) for x in list(self.fwd_main_np["width"]) + list(self.fwd_rs_np["width"])]
+    fc = [int(x) for x in list(self.fwd_main_np["dst_col"]) + list(self.fwd_rs_np["dst_col"])]
+    self.fwd_vec8 = self.tab != 0 and self.vec4 and all(w % 8 == 0 for w in fw) and \
+        all(c % 8 == 0 for c in fc) and ostride % 8 == 0 and self.rs_width % 8 == 0
     # 16-byte gradient loads (8 columns per lane) in the SGD update: DE_B200_VEC8_GRAD=1
     self.vec8 = os.environ.get("DE_B200_VEC8_GRAD", "0") == "1" and self.vec4 and \
         all(w % 8 == 0 for w in widths) and all(c % 8 == 0 for c in cols) and \
@@ -889,12 +897,13 @@ class FusedEngine:
       last = k == len(self.fwd_launches) - 1 and self.fwd_rs is None
       ops.lookup_fwd(descs, n, B, B, lb, self.out_stride, [], self.out_ptrs, rank, self.ids64,
                      self.act, self.vec4,
-                     self._sync(wait=wait_ids, signal=CH_OUT if last else -1), tile)
+                     self._sync(wait=wait_ids, signal=CH_OUT if last else -1), tile, self.tab,
+                     self.fwd_vec8)
       wait_ids = -1  # later launches of this stream are ordered behind the wait
     if self.fwd_rs is not None:
       ops.lookup_fwd(self.fwd_rs, len(self.fwd_rs_np), B, B, lb, self.rs_width, [], self.rs_ptrs,
                      rank, self.ids64, 0, self.vec4, self._sync(wait=wait_ids, signal=CH_OUT),
-                     self.fwd_rs_tile)
+                     self.fwd_rs_tile, self.tab, self.fwd_vec8)
 
   def sync_out_wait(self):
     """``sync`` spec that makes a consumer kernel wait for the owners' "output ready" signals."""
@@ -1021,8 +1030,12 @@ class FusedEngine:
       self._refresh_tables()
     B = self.B
     gscale = 0.0 if self._dry_updates else de.mp_grad_scale
+    # 16-bit tables always take the sorted, deduplicated update, SGD included: each row then has
+    # exactly one writer per step and is stochastically rounded once.  An atomic 16-bit add would
+    # round to nearest on every duplicate id (dropping sub-half-ulp updates) and its result
+    # would depend on the order of the adds.
     if opt is not None and opt["kind"] == "sgd" and not opt.get("deterministic", False) and \
-        not self.has_offload:
+        not self.has_offload and self.tab == 0:
       # head: every requester's gradient rows have landed; tail: ids + gradients are consumed
       ops.scatter_add_bwd(self.mpdesc, self.n_mp_inputs, B, B, B, self.recv_width, [],
                           self.recv_ptr, 0, -gscale, self.lr_t.data_ptr(), self.ids64,
@@ -1044,7 +1057,8 @@ class FusedEngine:
                          keys, items, seg, n_unique, kind, opt["lr"],
                          opt["eps"], opt["beta1"], opt["beta2"], 1.0, 1.0, gscale,
                          opt["weight_decay"], self.lr_t.data_ptr(), None, None, self.max_width,
-                         self.act, self.vec4, self._balanced_scratch(), self.step_t.data_ptr())
+                         self.act, self.vec4, self._balanced_scratch(), self.step_t.data_ptr(),
+                         self.tab)
       if multi:
         ops.sync_only(self._sync(signal=CH_CONSUMED))
       return [None] * n_mp
@@ -1069,7 +1083,8 @@ class FusedEngine:
       # a fresh [nnz, width] buffer with canonical strides: for nnz == 1 ``.contiguous()`` is a
       # no-op on the padded view (row stride max_width) and PyTorch's sparse -> dense kernels
       # then address the destination with that stride (heap overflow found by the plan fuzzer)
-      rows = torch.empty(hi - lo, w.shape[1], dtype=torch.float32, device=emit_rows.device)
+      # (in the table's dtype: autograd hands a parameter gradients of its own dtype)
+      rows = torch.empty(hi - lo, w.shape[1], dtype=w.dtype, device=emit_rows.device)
       rows.copy_(emit_rows[lo:hi, :w.shape[1]])
       rows = rows.to(w.device)
       out.append(torch.sparse_coo_tensor(ids, rows, size=tuple(w.shape), is_coalesced=True,

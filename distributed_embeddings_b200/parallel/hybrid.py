@@ -18,6 +18,7 @@ import torch
 import torch.distributed as dist
 from torch import nn
 
+from ..ops.stochastic_rounding import HALF_DTYPES, stochastic_round
 from .comm import CommContext, dist_ready
 from .dist_model_parallel import _is_mp, broadcast_variables
 
@@ -257,7 +258,11 @@ class SparseRowOptimizer:
   baseline, which has no fused update.  Same math as the fused kernels
   (``ops/csrc/sparse_update_kernels.cu``): ``sgd`` | ``adagrad`` | ``rowwise_adagrad`` | ``adam``
   (lazy: only the touched rows advance).  Counterpart of the Keras sparse-apply kernels the
-  reference relies on (examples/benchmarks/synthetic_models/main.py:96-101)."""
+  reference relies on (examples/benchmarks/synthetic_models/main.py:96-101).
+
+  bf16 / fp16 parameters keep fp32 state; their touched rows are updated in fp32 and written
+  back with stochastic rounding keyed by (step, row, column), the rule of the fused kernels
+  (``ops/stochastic_rounding.py``)."""
 
   def __init__(self, params: Sequence[nn.Parameter], kind: str = "sgd", lr: float = 0.01,
                eps: Optional[float] = None, beta1: float = 0.9, beta2: float = 0.999,
@@ -272,13 +277,14 @@ class SparseRowOptimizer:
     self.step_count = 0
     self.state = []
     for p in self.params:
+      sdt = torch.float32 if p.dtype in HALF_DTYPES else p.dtype  # half tables: fp32 state
       if kind == "adagrad":
-        self.state.append([torch.full_like(p, initial_accumulator_value)])
+        self.state.append([torch.full_like(p, initial_accumulator_value, dtype=sdt)])
       elif kind == "rowwise_adagrad":
-        self.state.append([torch.full((p.shape[0],), initial_accumulator_value, dtype=p.dtype,
+        self.state.append([torch.full((p.shape[0],), initial_accumulator_value, dtype=sdt,
                                       device=p.device)])
       elif kind == "adam":
-        self.state.append([torch.zeros_like(p), torch.zeros_like(p)])
+        self.state.append([torch.zeros_like(p, dtype=sdt), torch.zeros_like(p, dtype=sdt)])
       else:
         self.state.append([])
 
@@ -298,6 +304,10 @@ class SparseRowOptimizer:
       else:
         idx = torch.arange(p.shape[0], device=p.device)
         val = g.to(p.dtype)
+      if p.dtype in HALF_DTYPES:
+        self._step_half(p, st, idx, val.float())
+        p.grad = None
+        continue
       if self.weight_decay:
         val = val + self.weight_decay * p[idx]
       if self.kind == "sgd":
@@ -318,3 +328,27 @@ class SparseRowOptimizer:
         b2 = 1 - self.beta2**self.step_count
         p.index_add_(0, idx, (m / b1) / ((v / b2).sqrt() + self.eps), alpha=-self.lr)
       p.grad = None
+
+  def _step_half(self, p, st, idx, val):
+    """fp32 update of the rows ``idx`` of a bf16 / fp16 table, stochastically rounded back."""
+    w = p[idx].float()
+    if self.weight_decay:
+      val = val + self.weight_decay * w
+    if self.kind == "sgd":
+      w = w - self.lr * val
+    elif self.kind == "adagrad":
+      acc = st[0][idx] + val * val
+      st[0][idx] = acc
+      w = w - self.lr * val / (acc.sqrt() + self.eps)
+    elif self.kind == "rowwise_adagrad":
+      acc = st[0][idx] + (val * val).mean(dim=1)
+      st[0][idx] = acc
+      w = w - self.lr * val / (acc.sqrt().unsqueeze(1) + self.eps)
+    else:
+      m = self.beta1 * st[0][idx] + (1 - self.beta1) * val
+      v = self.beta2 * st[1][idx] + (1 - self.beta2) * val * val
+      st[0][idx], st[1][idx] = m, v
+      b1 = 1 - self.beta1**self.step_count
+      b2 = 1 - self.beta2**self.step_count
+      w = w - self.lr * (m / b1) / ((v / b2).sqrt() + self.eps)
+    p[idx] = stochastic_round(w, p.dtype, self.step_count, idx).to(p.device)

@@ -43,6 +43,8 @@ def main():
                  help="placement; traffic_balanced evens out the per-rank lookups of the "
                  "multi-hot features (memory_balanced is what the reference benchmark uses)")
   p.add_argument("--amp", action="store_true", help="bf16 activations / MLP")
+  p.add_argument("--table_dtype", default="fp32", choices=["bf16", "fp16", "fp32"],
+                 help="storage of the model-parallel embedding tables (--embedding_api de)")
   p.add_argument("--backend", default="auto", choices=["auto", "fused", "torch"])
   p.add_argument("--row_scale", type=float, default=1.0, help="shrink tables (smoke runs)")
   p.add_argument("--device", default=None)
@@ -75,7 +77,9 @@ def main():
                            dp_input=args.dp_input, device=device, compute_dtype=dtype,
                            backend=args.backend, row_slice_threshold=args.row_slice_threshold,
                            data_parallel_threshold=args.data_parallel_threshold,
-                           strategy=args.dist_strategy)
+                           strategy=args.dist_strategy,
+                           table_dtype={"fp32": torch.float32, "bf16": torch.bfloat16,
+                                        "fp16": torch.float16}[args.table_dtype])
     mp_ids = None if args.dp_input else model.embedding.strategy.input_ids_list[rank]
   else:
     if not args.dp_input or args.column_slice_threshold is not None:

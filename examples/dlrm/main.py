@@ -29,6 +29,9 @@ from distributed_embeddings_b200.utils.lr_schedule import LearningRateScheduler
 from distributed_embeddings_b200.utils.metrics import binary_auc
 
 
+TABLE_DTYPES = {"fp32": torch.float32, "bf16": torch.bfloat16, "fp16": torch.float16}
+
+
 def parse():
   p = argparse.ArgumentParser()
   p.add_argument("--dataset_path", default=None, help="dir with model_size.json + train/ test/")
@@ -45,6 +48,9 @@ def parse():
   p.add_argument("--dist_strategy", default="memory_balanced")
   p.add_argument("--fast", action="store_true", help="hand-scheduled step + CUDA graph")
   p.add_argument("--amp", action="store_true", default=True)
+  p.add_argument("--table_dtype", default="fp32", choices=sorted(TABLE_DTYPES),
+                 help="storage of the model-parallel embedding tables (bf16 / fp16: half the "
+                      "memory, stochastically rounded updates)")
   p.add_argument("--warmup_steps", type=int, default=8000)
   p.add_argument("--decay_start_step", type=int, default=48000)
   p.add_argument("--decay_steps", type=int, default=24000)
@@ -80,7 +86,8 @@ def main():
                top_mlp_dims=[int(d) for d in args.top_mlp_dims.split(",")],
                num_numerical_features=args.num_numerical_features, dp_input=args.dp_input,
                dist_strategy=args.dist_strategy, test_combiner=args.test_combiner, device=device,
-               compute_dtype=torch.bfloat16 if (args.amp and cuda) else torch.float32)
+               compute_dtype=torch.bfloat16 if (args.amp and cuda) else torch.float32,
+               table_dtype=TABLE_DTYPES[args.table_dtype])
   table_ids = list(range(len(table_sizes))) if args.dp_input else \
       model.embedding.strategy.input_ids_list[rank]
   lbs = args.batch_size // world

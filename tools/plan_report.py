@@ -60,6 +60,10 @@ def main(argv=None):
   ap.add_argument("--hbm-gib", type=float, default=79.0, help="per-GPU memory to check against")
   ap.add_argument("--optimizer-slots", type=int, default=0,
                   help="fp32 state copies per table element (adagrad 1, adam 2)")
+  ap.add_argument("--table-dtype", default="fp32", choices=["fp32", "bf16", "fp16"],
+                  help="storage of the model-parallel tables (DistributedEmbedding(table_dtype="
+                       "...)): their table and gather bytes at its element size; optimizer slots "
+                       "and replicated tables stay fp32")
   ap.add_argument("--json", action="store_true")
   args = ap.parse_args(argv)
 
@@ -74,21 +78,31 @@ def main(argv=None):
                              input_hotness=hots, **kw)
   mem = st.memory_report()
   tr = st.traffic_report(args.global_batch, hots)
-  per_elem = 4 * (1 + args.optimizer_slots)
+  esz = 4 if args.table_dtype == "fp32" else 2
+  per_elem = esz + 4 * args.optimizer_slots       # model-parallel tables
+  per_elem_dp = 4 * (1 + args.optimizer_slots)    # replicated tables are always fp32
+  dp_elems = sum(int(c["input_dim"]) * int(c["output_dim"]) for c in st.dp_configs)
+  hot = hots or [1] * len(st.input_table_map)
+  dp_gather = 0  # bytes gathered from the replicated tables per rank (local batch, fp32 rows)
+  for j, gi in enumerate(st.input_groups[0]):
+    t = st.table_groups[0][st.map_groups[0][j]]
+    dp_gather += args.global_batch // args.world * hot[gi] * int(st.global_configs[t]["output_dim"]) * 4
   ranks = []
   for r in range(args.world):
     n_tab = len(st.local_configs[r]) if st.table_groups[1] else 0
     cols = sum(int(st.local_configs[r][m]["output_dim"]) for m in st.local_maps[r]) \
         if st.table_groups[1] else 0
-    gib = mem[r]["hbm_elements"] * per_elem / 2**30
+    gib = ((mem[r]["hbm_elements"] - dp_elems) * per_elem + dp_elems * per_elem_dp) / 2**30
+    gather = (tr["ranks"][r]["gather_bytes"] - dp_gather) * esz / 4 + dp_gather
     ranks.append({"rank": r, "fused_tables": n_tab, "inputs": len(st.input_ids_list[r]),
                   "exchanged_columns": cols, "hbm_gib": round(gib, 2),
                   "host_gib": round(mem[r]["host_elements"] * per_elem / 2**30, 2),
-                  "gather_mb": round(tr["ranks"][r]["gather_bytes"] / 1e6, 1),
+                  "gather_mb": round(gather / 1e6, 1),
                   "nvlink_out_mb": round(tr["ranks"][r]["nvlink_out_bytes"] / 1e6, 1),
                   "lookups": int(tr["ranks"][r]["lookups"]),
                   "fits": gib <= args.hbm_gib})
   rep = {"world": args.world, "strategy": args.strategy, "column_slice_threshold": cst,
+         "table_dtype": args.table_dtype,
          "tables": len(cfgs), "replicated": len(st.table_groups[0]),
          "table_parallel": len(st.table_groups[1]), "row_sliced": len(st.table_groups[2]),
          "gather_imbalance": round(tr["gather_imbalance"], 3),
@@ -97,7 +111,7 @@ def main(argv=None):
     print(json.dumps(rep))
     return rep
   print(f"{len(cfgs)} tables on {args.world} ranks, strategy {args.strategy}, "
-        f"column_slice_threshold {cst}: {rep['replicated']} replicated, "
+        f"column_slice_threshold {cst}, {args.table_dtype} tables: {rep['replicated']} replicated, "
         f"{rep['table_parallel']} table-parallel, {rep['row_sliced']} row-sliced")
   print(f"{'rank':>4} {'tables':>7} {'inputs':>7} {'columns':>8} {'HBM GiB':>9} {'host GiB':>9} "
         f"{'gather MB':>10} {'NVLink out MB':>14} {'lookups':>12}")
