@@ -97,6 +97,14 @@ class DryWorld:
     raw = (ctypes.c_char * nbytes).from_address(int(ptr))
     return torch.frombuffer(raw, dtype=dtype, count=count)
 
+  def make_ops(self, rank: int) -> "DryOps":
+    """The ops object every engine of ``rank`` calls (a subclass may replay them elsewhere)."""
+    return DryOps(self, rank)
+
+  def run_rank(self, fn, rank: int):
+    """Body of the thread of ``rank`` (see :func:`run_ranks`)."""
+    return fn(rank)
+
   def barrier(self):
     self._barrier.wait(timeout=120)
 
@@ -284,8 +292,8 @@ class DryOps:
         seg = self._pool_index(lens)
         pooled = torch.zeros(ns, width).index_add_(0, seg, rows)
         hits = torch.zeros(ns, dtype=torch.int64).index_add_(0, seg, ok.to(torch.int64))
-        if int(d["combiner"]) == 1:
-          pooled = pooled / lens.clamp(min=1).unsqueeze(1).to(pooled.dtype)
+        if int(d["combiner"]) == 1:  # the kernels multiply by the fp32 reciprocal of n
+          pooled = pooled * (1.0 / lens.clamp(min=1).to(pooled.dtype)).unsqueeze(1)
         # the destination row block of requester dd: rows [0, ns) x columns [col, col + width)
         last = (ns - 1) * dst_stride + col + width
         out = self.world.tensor(int(dst_ptrs[dd]), odt, last, "lookup destination")
@@ -476,11 +484,15 @@ class DryOps:
     tdt = self._ADT[int(table_dtype)]
     tsz = 4 if int(table_dtype) == 0 else 2
     step = 0
+    # the kernels take the optimizer constants in fp32 and form 1 - beta and the bias
+    # corrections in fp32 from them
+    beta1, beta2 = float(np.float32(beta1)), float(np.float32(beta2))
     if step_ptr:
       t = float(self.world.tensor(int(step_ptr), torch.float32, 1, "optimizer step")[0])
       step = int(t)
       if kind == 3:
-        bias1, bias2 = 1.0 - beta1**t, 1.0 - beta2**t
+        bias1 = float(np.float32(1) - np.float32(beta1)**np.float32(t))
+        bias2 = float(np.float32(1) - np.float32(beta2)**np.float32(t))
     D = self._descs(descs, 1 << 30)
     T = self._descs(tables, n_tables, TABLE_DESC)
     if lr_ptr:
@@ -541,8 +553,8 @@ class DryOps:
       elif kind == 3:
         mm = self.world.tensor(int(t["state0"]) + row * width * 4, torch.float32, width, "adam m")
         vv = self.world.tensor(int(t["state1"]) + row * width * 4, torch.float32, width, "adam v")
-        mm.mul_(beta1).add_((1 - beta1) * g)
-        vv.mul_(beta2).add_((1 - beta2) * g * g)
+        mm.mul_(beta1).add_(float(np.float32(1) - np.float32(beta1)) * g)
+        vv.mul_(beta2).add_(float(np.float32(1) - np.float32(beta2)) * g * g)
         wt -= lr * (mm / bias1) / ((vv / bias2).sqrt() + eps)
       else:
         raise ValueError(f"optimizer kind {kind}")
@@ -555,7 +567,7 @@ class DryRank:
 
   def __init__(self, world: DryWorld, rank: int):
     self.ctx = DryCtx(world, rank)
-    self.ops = DryOps(world, rank)
+    self.ops = world.make_ops(rank)
 
   def attach(self, engine):
     self.ops.engine = engine
@@ -568,7 +580,7 @@ def run_ranks(world: DryWorld, fn, timeout: float = 300.0):
 
   def body(r):
     try:
-      results[r] = fn(r)
+      results[r] = world.run_rank(fn, r)
     except BaseException as e:  # pylint: disable=broad-except
       errors[r] = e
       world._barrier.abort()
@@ -594,12 +606,13 @@ def run_ranks(world: DryWorld, fn, timeout: float = 300.0):
   return results
 
 
-def build_engines(embeddings: Sequence[dict], world_size: int, **kwargs):
+def build_engines(embeddings: Sequence[dict], world_size: int, world_cls=DryWorld, **kwargs):
   """One ``DistributedEmbedding`` + dry fused engine per rank of the plan (host memory).
-  ``embeddings`` are config dicts; ``kwargs`` go to ``DistributedEmbedding``."""
+  ``embeddings`` are config dicts; ``world_cls(world_size)`` makes the :class:`DryWorld`;
+  ``kwargs`` go to ``DistributedEmbedding``."""
   from .dist_model_parallel import DistributedEmbedding  # pylint: disable=import-outside-toplevel
   assert world_size <= MAX_PEERS
-  world = DryWorld(world_size)
+  world = world_cls(world_size)
   des = []
   for r in range(world_size):
     de = DistributedEmbedding([dict(e) for e in embeddings], device="cpu", backend="torch",

@@ -13,11 +13,11 @@ from distributed_embeddings_b200.parallel import dry_run
 def _dense_grad(p):
   g = p.grad
   if g is None:
-    return torch.zeros_like(p)
-  return g.to_dense() if g.is_sparse else g
+    return torch.zeros_like(p, dtype=torch.float32)
+  return (g.to_dense() if g.is_sparse else g).float()
 
 
-def assemble(des, get=lambda p: p.detach()):
+def assemble(des, get=lambda p: p.detach().float()):
   """Global tables from the local shards of all ranks (what get_weights does with collectives);
   ``get`` picks what to read from every local parameter (the weights, or their gradients)."""
   st = des[0].strategy
@@ -65,11 +65,15 @@ def reference_step(tables, imap, glob_ids, combiners, grads, lr, world, kind, st
         np.add.at(dense[t], np.asarray(row, dtype=np.int64), grads[i][b] * scale)
       outs.append(out)
       continue
-    rows = tables[t][ids]  # [B, h, w]
+    # ids outside the table (fed to row-sliced tables) pool to zero and get no gradient
+    ok = (ids >= 0) & (ids < tables[t].shape[0])
+    rows = tables[t][np.where(ok, ids, 0)] * ok[..., None]  # [B, h, w]
     n = ids.shape[1]
     outs.append(rows.sum(1) / (n if combiners[t] == "mean" else 1))
     g = grads[i] / (n if combiners[t] == "mean" else 1)
-    np.add.at(dense[t], ids.reshape(-1), np.repeat(g, n, axis=0))
+    per_id = np.repeat(g, n, axis=0)
+    flat_ok = ok.reshape(-1)
+    np.add.at(dense[t], ids.reshape(-1)[flat_ok], per_id[flat_ok])
   if kind == "none":
     return outs, [g / world for g in dense]
   for t, g in enumerate(dense):
@@ -90,19 +94,59 @@ def reference_step(tables, imap, glob_ids, combiners, grads, lr, world, kind, st
   return outs
 
 
-def run_plan(seed, world, kind="sgd", dtype=torch.float32, ragged=False):
+# Size profile of the random plans.  The default keeps the interpreter fast; other profiles (the
+# GPU kernel conformance tests) draw larger shapes from the same generator.
+#   rows / widths / hotness / local_batch: (lo, hi) range of table rows, choices for the others;
+#   ragged_len: most ids of a ragged sample; power_law: skewed ids (hot rows) instead of uniform;
+#   dyadic: tables, gradients and mean weights on a coarse power-of-two grid, so that every fp32
+#     sum is exact in any order; out_of_table: one-hot inputs of row-sliced tables also get ids
+#     below / above the table (they pool to zero); table_dtype: storage of model-parallel tables.
+SMALL_PROFILE = {"rows": (3, 50), "widths": (4, 8, 12, 16), "hotness": (1, 1, 2, 3),
+                 "local_batch": (2, 3, 5), "ragged_len": 4, "power_law": False, "dyadic": False,
+                 "out_of_table": False, "table_dtype": torch.float32}
+
+
+def _pow2_floor(n):
+  return 1 << (int(n).bit_length() - 1) if n > 0 else 0
+
+
+def _draw_ids(nrng, rows, size, power_law):
+  if power_law:  # P(id < k) = (k / rows)^(1/4): a few very hot rows, a long tail
+    return np.minimum((rows * nrng.random(size)**4).astype(np.int64), rows - 1)
+  return nrng.integers(0, rows, size=size)
+
+
+def _draw_tables(nrng, sizes, dyadic):
+  tables = [nrng.standard_normal(s).astype(np.float32) for s in sizes]
+  if dyadic:  # multiples of 1/16 in [-4, 4]: exact in bf16 / fp16 as well; "+ 0" drops the
+    # sign of -0.0 (the kernels keep it through a one-id pool, the interpreter's sum does not)
+    tables = [np.clip(np.round(t * 16) / 16, -4, 4).astype(np.float32) + 0 for t in tables]
+  return tables
+
+
+def _draw_grads(nrng, shapes, dyadic):
+  if dyadic:  # multiples of 1/64
+    return [(np.round(nrng.standard_normal(s) * 8) / 64).astype(np.float32) + 0 for s in shapes]
+  return [nrng.standard_normal(s).astype(np.float32) * 0.1 for s in shapes]
+
+
+def run_plan(seed, world, kind="sgd", dtype=torch.float32, ragged=False, profile=None,
+             world_cls=dry_run.DryWorld):
+  prof = dict(SMALL_PROFILE, **(profile or {}))
   rng = random.Random(seed)
   nrng = np.random.default_rng(seed)
   n_tables = rng.randint(max(1, world // 2), 2 * world + 2)
   if kind == "rowwise_adagrad":
     n_tables = max(n_tables, world)  # no automatic column slicing (see below)
-  sizes = [(rng.randint(3, 50), rng.choice([4, 8, 12, 16])) for _ in range(n_tables)]
+  sizes = [(rng.randint(*prof["rows"]), rng.choice(prof["widths"])) for _ in range(n_tables)]
   combiners = [rng.choice(["sum", "mean"]) for _ in sizes]
   imap = list(range(n_tables)) + [rng.randint(0, n_tables - 1) for _ in range(rng.randint(0, 3))]
   rng.shuffle(imap)
   if sorted(set(imap)) != list(range(n_tables)):
     imap = list(range(n_tables))
-  hots = {t: rng.choice([1, 1, 2, 3]) for t in range(n_tables)}
+  hots = {t: rng.choice(prof["hotness"]) for t in range(n_tables)}
+  if prof["dyadic"]:  # mean pooling by a power of two
+    hots = {t: _pow2_floor(h) if combiners[t] == "mean" else h for t, h in hots.items()}
   kw = {"strategy": rng.choice(["basic", "memory_balanced", "memory_optimized",
                                  "traffic_balanced"]),
         "input_table_map": imap}
@@ -121,30 +165,41 @@ def run_plan(seed, world, kind="sgd", dtype=torch.float32, ragged=False):
     kw["data_parallel_threshold"] = rng.choice([30, 80])
   if dp_input and world > 1 and rng.random() < 0.4 and not plain:
     kw["row_slice_threshold"] = rng.choice([300, 500])
+  if prof["table_dtype"] != torch.float32:
+    kw["table_dtype"] = prof["table_dtype"]
   embs = [{"input_dim": r, "output_dim": w, "combiner": c} for (r, w), c in zip(sizes, combiners)]
   try:
-    sim, des = dry_run.build_engines(embs, world, compute_dtype=dtype, **kw)
+    sim, des = dry_run.build_engines(embs, world, world_cls, compute_dtype=dtype, **kw)
   except ValueError as e:
     if "Not enough table" in str(e):
       return "infeasible"
     raise
-  tables = [nrng.standard_normal(s).astype(np.float32) for s in sizes]
+  tables = _draw_tables(nrng, sizes, prof["dyadic"])
   for de in des:
     de.set_weights(tables)
     if kind != "none":
       de.set_optimizer(kind, lr=0.5)
-  lb = rng.choice([2, 3, 5])
+  lb = rng.choice(prof["local_batch"])
   B = lb * world
-  glob = [nrng.integers(0, sizes[t][0], size=(B, hots[t])) for t in imap]
+  glob = [_draw_ids(nrng, sizes[t][0], (B, hots[t]), prof["power_law"]) for t in imap]
   id_dtype = rng.choice([np.int64, np.int32])
   rag = [ragged and rng.random() < 0.6 for _ in imap]
   for i, t in enumerate(imap):
     if rag[i]:
       # 0 ids is legal: the sample pools to zero and contributes no gradient
-      glob[i] = [list(nrng.integers(0, sizes[t][0], size=rng.randint(0, 4))) for _ in range(B)]
+      lens = [rng.randint(0, prof["ragged_len"]) for _ in range(B)]
+      if prof["dyadic"] and combiners[t] == "mean":
+        lens = [_pow2_floor(n) for n in lens]
+      glob[i] = [list(_draw_ids(nrng, sizes[t][0], n, prof["power_law"])) for n in lens]
   if ragged:
     for de in des:
-      de.ragged_capacity = 4
+      de.ragged_capacity = prof["ragged_len"]
+  if prof["out_of_table"]:
+    row_sliced = set(des[0].strategy.table_groups[2])
+    for i, t in enumerate(imap):
+      if t in row_sliced and not rag[i] and hots[t] == 1:
+        bad = nrng.random(B) < 0.15
+        glob[i][bad, 0] = nrng.choice([-7, -1, sizes[t][0], sizes[t][0] + 3], size=int(bad.sum()))
 
   def as_input(i, lo, hi):
     from distributed_embeddings_b200.ops.ragged import RaggedIds
@@ -156,7 +211,7 @@ def run_plan(seed, world, kind="sgd", dtype=torch.float32, ragged=False):
     return torch.from_numpy(glob[i][lo:hi].astype(id_dtype))
 
   widths = [sizes[t][1] for t in imap]
-  grads = [nrng.standard_normal((B, w)).astype(np.float32) * 0.1 for w in widths]
+  grads = _draw_grads(nrng, [(B, w) for w in widths], prof["dyadic"])
   st = des[0].strategy
   dp_tables = set(st.table_groups[0])
 
@@ -182,6 +237,9 @@ def run_plan(seed, world, kind="sgd", dtype=torch.float32, ragged=False):
   if kind == "none":
     ref_outs, ref_grads = ref_outs
   tol = 1e-4 if dtype == torch.float32 else 3e-2
+  # 16-bit tables: one stochastic rounding per element, within one ulp of the fp32 result
+  half = {torch.bfloat16: 2.0**-7, torch.float16: 2.0**-10}.get(prof["table_dtype"])
+  tab_rtol, tab_atol = (2 * half, 1e-3) if half else (10 * tol, 10 * tol)
   for r, (out, dp_grads) in enumerate(results):
     exp = np.concatenate([o[r * lb:(r + 1) * lb] for o in ref_outs], 1)
     np.testing.assert_allclose(out, exp, rtol=tol, atol=tol, err_msg=f"forward, rank {r}")
@@ -190,14 +248,14 @@ def run_plan(seed, world, kind="sgd", dtype=torch.float32, ragged=False):
     got_g = assemble(des, _dense_grad)
     for t in range(n_tables):
       if t not in dp_tables:
-        np.testing.assert_allclose(got_g[t], ref_grads[t], rtol=10 * tol, atol=10 * tol,
+        np.testing.assert_allclose(got_g[t], ref_grads[t], rtol=tab_rtol, atol=tab_atol,
                                    err_msg=f"sparse gradient of table {t}")
   got = assemble(des)
   for t in range(n_tables):
     if t in dp_tables:
       np.testing.assert_allclose(got[t], tables[t], rtol=0, atol=0)  # untouched by the engine
       continue
-    np.testing.assert_allclose(got[t], ref_tables[t], rtol=10 * tol, atol=10 * tol,
+    np.testing.assert_allclose(got[t], ref_tables[t], rtol=tab_rtol, atol=tab_atol,
                                err_msg=f"table {t} after the {kind} step")
   # dense gradients of replicated tables: local-batch contribution of each rank
   for j, t in enumerate(st.table_groups[0]):
@@ -696,15 +754,19 @@ def test_output_row_stride(world):
     col += w
 
 
-def run_inplace_plan(seed, world, streamed):
+def run_inplace_plan(seed, world, streamed, profile=None, world_cls=dry_run.DryWorld):
   """Random plan for the hand-scheduled steps' backward (``routes_all`` / ``routes_stage`` +
   ``backward_inplace``): column slices, shared tables, multi-hot sum / mean pooling, replicated
-  tables, one SGD step against the unsharded model."""
+  tables, one SGD step against the unsharded model.  ``profile``: see ``SMALL_PROFILE`` (rows,
+  widths, hotness, dyadic)."""
+  prof = {**SMALL_PROFILE, "rows": (3, 60), "local_batch": (3, 5, 8), **(profile or {})}
   rng = random.Random(seed)
   nrng = np.random.default_rng(seed)
   n_tables = rng.randint(max(2, world // 2), 2 * world + 2)
-  sizes = [(rng.randint(3, 60), rng.choice([4, 8, 12, 16])) for _ in range(n_tables)]
-  hot = rng.choice([1, 1, 2, 3])
+  sizes = [(rng.randint(*prof["rows"]), rng.choice(prof["widths"])) for _ in range(n_tables)]
+  hot = rng.choice(prof["hotness"])
+  if prof["dyadic"]:
+    hot = _pow2_floor(hot)
   combiners = [rng.choice(["sum", "mean"]) if hot > 1 else None for _ in sizes]
   imap = list(range(n_tables)) + [rng.randint(0, n_tables - 1) for _ in range(rng.randint(0, 2))]
   kw = {"strategy": rng.choice(["basic", "memory_balanced", "memory_optimized"]),
@@ -715,14 +777,14 @@ def run_inplace_plan(seed, world, streamed):
     kw["data_parallel_threshold"] = rng.choice([40, 100])
   embs = [{"input_dim": r, "output_dim": w, "combiner": c} for (r, w), c in zip(sizes, combiners)]
   try:
-    sim, des = dry_run.build_engines(embs, world, **kw)
+    sim, des = dry_run.build_engines(embs, world, world_cls, **kw)
   except ValueError as e:
     if "Not enough table" in str(e):
       return "infeasible"
     raise
-  tables = [nrng.standard_normal(s).astype(np.float32) for s in sizes]
+  tables = _draw_tables(nrng, sizes, prof["dyadic"])
   lr = 0.5
-  lb = rng.choice([3, 5, 8])
+  lb = rng.choice(prof["local_batch"])
   chunk = rng.choice([2, 3, 8])
   B = lb * world
   st = des[0].strategy
@@ -735,9 +797,9 @@ def run_inplace_plan(seed, world, streamed):
     if streamed:
       de._engine.enable_streamed_push(chunk)
   shape = (B,) if hot == 1 and rng.random() < 0.5 else (B, hot)
-  glob = [nrng.integers(0, sizes[t][0], size=shape) for t in imap]
+  glob = [_draw_ids(nrng, sizes[t][0], shape, prof["power_law"]) for t in imap]
   widths = [sizes[t][1] for t in imap]
-  grads = [nrng.standard_normal((B, w)).astype(np.float32) * 0.1 for w in widths]
+  grads = _draw_grads(nrng, [(B, w) for w in widths], prof["dyadic"])
 
   def rank_fn(r):
     de, eng = des[r], des[r]._engine
