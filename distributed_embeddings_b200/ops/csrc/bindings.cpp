@@ -767,6 +767,16 @@ void check_bf16_2d(const Tensor& t, const char* name) {
               name, " must be a 2-D bf16 CUDA tensor with unit inner stride");
 }
 
+// rows that start on `bytes`-byte boundaries (the interaction kernels stage feature rows with
+// 16-byte cp.async and store gradient pairs as 4-byte words).  Messages carry strings only: with
+// torch 2.11 an integer formatted into a TORCH_CHECK message crashes the process (SIGSEGV).
+void check_row_alignment(const Tensor& t, int64_t bytes, const char* name) {
+  TORCH_CHECK((t.stride(0) * 2) % bytes == 0 &&
+                  reinterpret_cast<uintptr_t>(t.data_ptr()) % static_cast<uintptr_t>(bytes) == 0,
+              name, bytes == 16 ? " rows must start on 16-byte boundaries"
+                                : " rows must start on 4-byte boundaries");
+}
+
 // z[s] = [strict lower triangle of F F^T | bottom | zero pad], F = [bottom ; emb_0 ; ...]
 void interact_fwd(const Tensor& bottom, const Tensor& emb, int64_t n_emb, Tensor z,
                   at::IntArrayRef sync) {
@@ -775,7 +785,11 @@ void interact_fwd(const Tensor& bottom, const Tensor& emb, int64_t n_emb, Tensor
   check_bf16_2d(z, "z");
   c10::cuda::CUDAGuard guard(bottom.device());
   const int64_t dim = bottom.size(1);
-  TORCH_CHECK(emb.size(1) == n_emb * dim);
+  TORCH_CHECK(emb.size(1) == n_emb * dim, "emb must be [batch, n_emb * dim]");
+  TORCH_CHECK(emb.size(0) >= bottom.size(0) && z.size(0) >= bottom.size(0),
+              "emb and z need a row per row of bottom");
+  check_row_alignment(bottom, 16, "bottom");
+  check_row_alignment(emb, 16, "emb");
   const int64_t need = (n_emb + 1) * n_emb / 2 + dim;
   TORCH_CHECK(z.size(1) >= need, "z is too narrow");
   bool ok = de::launch_interact_fwd(bottom.data_ptr(), bottom.stride(0), emb.data_ptr(),
@@ -794,11 +808,34 @@ void interact_bwd(const Tensor& bottom, const Tensor& emb, int64_t n_emb, const 
   check_bf16_2d(emb, "emb");
   check_bf16_2d(dz, "dz");
   check_bf16_2d(dbottom, "dbottom");
-  if (routes.has_value())
+  if (routes.has_value()) {
     TORCH_CHECK(routes->is_cuda() && routes->scalar_type() == at::kByte &&
                 routes->numel() >= n_routes * static_cast<int64_t>(sizeof(de::GradRoute)));
-  c10::cuda::CUDAGuard guard(bottom.device());
+  } else {
+    TORCH_CHECK(demb_ptr != 0, "interact_bwd needs an embedding-gradient buffer or routes");
+  }
   const int64_t dim = bottom.size(1);
+  const int64_t batch = bottom.size(0);
+  TORCH_CHECK(emb.size(1) == n_emb * dim, "emb must be [batch, n_emb * dim]");
+  TORCH_CHECK((n_emb + 1) * n_emb / 2 + dim <= dz.size(1), "dz is too narrow");
+  TORCH_CHECK(dbottom.size(1) == dim, "dbottom must be [batch, dim]");
+  TORCH_CHECK(emb.size(0) >= batch && dz.size(0) >= batch && dbottom.size(0) >= batch,
+              "emb, dz and dbottom need a row per row of bottom");
+  check_row_alignment(bottom, 16, "bottom");
+  check_row_alignment(emb, 16, "emb");
+  check_row_alignment(dbottom, 4, "dbottom");
+  if (!routes.has_value())
+    TORCH_CHECK(demb_stride % 2 == 0 && demb_ptr % 4 == 0,
+                "embedding-gradient rows must start on 4-byte boundaries");
+  if (done_counters.has_value()) {
+    TORCH_CHECK(done_counters->is_cuda() && done_counters->scalar_type() == at::kInt &&
+                    done_counters->is_contiguous(),
+                "done_counters must be a contiguous int32 CUDA tensor");
+    TORCH_CHECK(chunk_rows > 0, "chunk_rows must be positive with done_counters");
+    TORCH_CHECK(done_counters->numel() >= (batch + chunk_rows - 1) / chunk_rows,
+                "done_counters needs one counter per chunk of chunk_rows samples");
+  }
+  c10::cuda::CUDAGuard guard(bottom.device());
   bool ok = de::launch_interact_bwd(bottom.data_ptr(), bottom.stride(0), emb.data_ptr(),
                                     emb.stride(0), static_cast<int>(n_emb), static_cast<int>(dim),
                                     dz.data_ptr(), dz.stride(0), dbottom.data_ptr(),
@@ -851,6 +888,9 @@ void relu_bwd_bias(Tensor dy, const Tensor& y, Tensor db) {
   check_bf16_2d(dy, "dy");
   check_bf16_2d(y, "y");
   TORCH_CHECK(dy.is_contiguous() && y.is_contiguous() && dy.size(1) % 8 == 0);
+  TORCH_CHECK(y.sizes() == dy.sizes(), "y must have the shape of dy");
+  // one thread per 8 columns in a 256-thread block
+  TORCH_CHECK(dy.size(1) >= 8 && dy.size(1) <= 2048, "relu_bwd_bias supports 8..2048 columns");
   TORCH_CHECK(db.is_cuda() && db.scalar_type() == at::kFloat && db.numel() >= dy.size(1));
   c10::cuda::CUDAGuard guard(dy.device());
   de::launch_relu_bwd_bias(dy.data_ptr(), y.data_ptr(), db.data_ptr<float>(), dy.size(0),
@@ -865,6 +905,22 @@ void head_loss(const Tensor& x, const Tensor& w, const Tensor& bias, const Tenso
   TORCH_CHECK(x.is_contiguous() && dx.is_contiguous());
   TORCH_CHECK(w.scalar_type() == at::kBFloat16 && bias.scalar_type() == at::kBFloat16);
   TORCH_CHECK(labels.scalar_type() == at::kFloat && labels.is_contiguous());
+  const int64_t batch = x.size(0), k = x.size(1);
+  auto f32 = [](const Tensor& t, int64_t n, const char* name) {
+    TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kFloat && t.is_contiguous() &&
+                    t.numel() >= n,
+                name, " must be a contiguous fp32 CUDA tensor with enough elements");
+  };
+  TORCH_CHECK(w.is_cuda() && w.is_contiguous() && w.numel() == k, "w must hold K elements");
+  TORCH_CHECK(bias.is_cuda() && bias.numel() >= 1, "bias must hold one element");
+  TORCH_CHECK(labels.is_cuda() && labels.numel() == batch, "labels must hold one value per row");
+  TORCH_CHECK(dx.is_cuda() && dx.scalar_type() == at::kBFloat16 && dx.sizes() == x.sizes(),
+              "dx must be a bf16 tensor of the shape of x");
+  f32(dw, k, "dw");
+  f32(db, 1, "db");
+  f32(dbias_prev, k, "dbias_prev");
+  f32(loss_sum, 1, "loss_sum");
+  if (logits.has_value()) f32(*logits, batch, "logits");
   c10::cuda::CUDAGuard guard(x.device());
   bool ok = de::launch_head_loss(x.data_ptr(), static_cast<int>(x.size(1)), w.data_ptr(),
                                  bias.data_ptr(), labels.data_ptr<float>(), x.size(0),
