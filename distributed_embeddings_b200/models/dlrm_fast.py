@@ -32,6 +32,7 @@ from ..parallel.comm import CommContext
 from ..parallel.fused import FusedEngine
 from ..utils import nvtx
 from ..utils.lr_schedule import LearningRateScheduler
+from ..utils.metrics import BinnedAUC, auc_from_histogram
 from .dlrm import DLRM
 
 
@@ -58,7 +59,7 @@ class DLRMTrainStep:
   def __init__(self, model: DLRM, lr: float = 24.0, embedding_optimizer: str = "sgd",
                scheduler: Optional[LearningRateScheduler] = None, use_cuda_graph: bool = True,
                embedding_optimizer_kwargs: Optional[dict] = None, overlap: bool = True,
-               gemm: str = "cublas"):
+               gemm: str = "cublas", eval_thresholds: int = 8000):
     if gemm not in ("cublas", "fused_dgrad", "tcgen05", "tcgen05_pair"):
       raise ValueError("gemm must be cublas | fused_dgrad | tcgen05 | tcgen05_pair")
     # cublas: cuBLASLt everywhere.  fused_dgrad: forward/wgrad on cuBLASLt, dgrad on the
@@ -187,6 +188,11 @@ class DLRMTrainStep:
     ar_on = ar_env == "1" or (ar_env == "auto" and self.world >= 4)
     self._ar_stream = torch.cuda.Stream(device=dev) if (overlap and self.world > 1 and ar_on) \
         else None
+    # evaluation metrics, accumulated on the device by the head_eval kernel (see evaluate())
+    self.eval_auc = BinnedAUC(eval_thresholds, device=dev)
+    self._eval_loss = torch.zeros(1, dtype=torch.float64, device=dev)
+    self._eval_count = torch.zeros(1, dtype=torch.int64, device=dev)
+    self._eval_graph = None
 
   def _refresh_transposes(self):
     """K-major copies of W^T for the dgrad GEMMs (2.4 M elements, a few microseconds)."""
@@ -243,6 +249,9 @@ class DLRMTrainStep:
     self.dz = torch.empty(b, self.top[0].in_pad, dtype=bf, device=dev)
     self._batch = b
     self._graph = None
+    self._eval_graph = None
+    self._n_valid = torch.zeros(1, dtype=torch.int64, device=dev)
+    self._probs = torch.zeros(b, dtype=torch.float32, device=dev)
     # double-buffered device staging for the asynchronous input pipeline (prefetch())
     self._stage = [(torch.zeros_like(self.cat_stage), torch.zeros_like(self.num_in),
                     torch.zeros_like(self.lab_in)) for _ in range(2)]
@@ -255,12 +264,14 @@ class DLRMTrainStep:
     self._use_stage = False
 
   # ------------------------------------------------------------------ the step
+  def _select_stage(self):
+    a, b_ = self._stage
+    self.ops.select_copy([a[0], a[1], a[2]], [b_[0], b_[1], b_[2]],
+                         [self.cat_stage, self.num_in, self.lab_in], self._slot_dev)
+
   def _forward(self):
+    """Forward up to the top MLP output on the inputs in ``cat_stage`` / ``num_in``."""
     ops = self.ops
-    if self._use_stage:
-      a, b_ = self._stage
-      ops.select_copy([a[0], a[1], a[2]], [b_[0], b_[1], b_[2]],
-                      [self.cat_stage, self.num_in, self.lab_in], self._slot_dev)
     # the embedding exchange (id push, gather + NVLink push of the pooled rows; all signalling
     # folded into those kernels) runs on the side stream while the bottom MLP runs on the main
     # stream; they meet at the interaction, whose head waits for the owners' "output ready"
@@ -378,6 +389,8 @@ class DLRMTrainStep:
 
   def _step_impl(self):
     with nvtx.range("dlrm_forward"):
+      if self._use_stage:
+        self._select_stage()
       self._forward()
     with nvtx.range("dlrm_backward_update"):
       self._backward()
@@ -390,7 +403,9 @@ class DLRMTrainStep:
 
   def load_batch(self, numerical, categorical, labels):
     """Copy one batch into the static input buffers (host pinned or device tensors).
-    ``categorical``: ``[n_features, batch]`` tensor (feature major) or list of ``[batch]``."""
+    ``categorical``: ``[n_features, batch]`` tensor (feature major) or list of ``[batch]``.
+    :meth:`evaluate` / :meth:`predict` overwrite these buffers: do not evaluate between this
+    call and the :meth:`run` that consumes the batch."""
     b = int(numerical.shape[0])
     if b != self._batch:
       self._alloc(b)
@@ -468,3 +483,111 @@ class DLRMTrainStep:
   def step(self, numerical, categorical, labels) -> torch.Tensor:
     self.load_batch(numerical, categorical, labels)
     return self.run()
+
+  # ------------------------------------------------------------------ evaluation
+  # The forward-only schedule reuses the step's input and activation buffers and its GEMM back
+  # end, and ends in head_eval instead of head_loss + backward.  It changes nothing a training
+  # step owns (tables, optimizer state, step_t, p32 / p16 / g32, lr_t, the scheduler, the
+  # prefetch slots), so evaluations may sit between run() / run_prefetched() calls and the
+  # training graph stays valid.  It does overwrite the static inputs, so an evaluation must not
+  # separate load_batch() from the run() that consumes it.
+  #
+  # At world size > 1 it is collective (every rank runs the same number of chunks) and needs no
+  # signal of its own: a requester's next id push is ordered behind its interaction forward,
+  # which waited for every owner's "output ready" signal, and each owner sends that from the tail
+  # of the lookup that read the ids.  No rank signals "consumed" during an evaluation, so those
+  # counts stay equal on all ranks and the next training step's id push waits as before.
+  def _eval_impl(self):
+    with nvtx.range("dlrm_eval"):
+      self._forward()
+      H = self.head
+      self.ops.head_eval(self.top[-1].y, H.w16.view(-1), H.b16, self.lab_in, self._n_valid,
+                         self._probs, self.eval_auc.hist, self._eval_loss, self._eval_count)
+
+  def _eval_ready(self):
+    if self._batch is None:
+      raise RuntimeError("evaluation runs in chunks of the training batch: load or run a "
+                         "training batch first")
+    if self.engine.out_needs_reduce:
+      raise NotImplementedError("evaluation does not support multi-hot row-sliced inputs")
+    if not self.use_cuda_graph or self._eval_graph is not None:
+      return
+    # warm up with no valid rows (metrics untouched), then capture the forward-only schedule
+    self._n_valid.zero_()
+    s = torch.cuda.Stream(device=self.dev)
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+      self._eval_impl()
+    torch.cuda.current_stream().wait_stream(s)
+    torch.cuda.synchronize()
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+      self._eval_impl()
+    self._eval_graph = g
+
+  def _eval_chunks(self, numerical, categorical, labels, out=None):
+    """Run the forward-only schedule over ``n`` samples in chunks of the training batch; the
+    last chunk is padded with id 0 and zero numerical features."""
+    n = int(numerical.shape[0])
+    if n < 1:
+      raise ValueError("evaluation needs at least one sample")
+    self._eval_ready()
+    b = self._batch
+    lab = labels.reshape(-1) if labels is not None else None
+    if isinstance(categorical, (list, tuple)):
+      cats = [c.reshape(-1) for c in categorical]
+    else:
+      cats = None
+    for s in range(0, n, b):
+      m = min(b, n - s)
+      self.num_in[:m].copy_(numerical[s:s + m], non_blocking=True)
+      if cats is None:
+        self.cat_stage[:, :m].copy_(categorical[:, s:s + m], non_blocking=True)
+      else:
+        for f, c in enumerate(cats):
+          self.cat_stage[f, :m].copy_(c[s:s + m], non_blocking=True)
+      if m < b:
+        self.num_in[m:].zero_()
+        self.cat_stage[:, m:].zero_()
+      if lab is not None:
+        self.lab_in[:m].copy_(lab[s:s + m], non_blocking=True)
+      self._n_valid.fill_(m if lab is not None else 0)
+      if self.use_cuda_graph:
+        self._eval_graph.replay()
+      else:
+        self._eval_impl()
+      if out is not None:
+        out[s:s + m].copy_(self._probs[:m])
+
+  def evaluate(self, numerical, categorical, labels):
+    """Accumulate the evaluation metrics (binned ROC AUC, log loss) over ``n >= 1`` local
+    samples: ``numerical [n, 13]``, ``categorical`` ``[n_features, n]`` or a list of ``[n]``,
+    ``labels [n]``.  Nothing is copied to the host; read the result with :meth:`eval_metrics`."""
+    self._eval_chunks(numerical, categorical, labels)
+
+  def predict(self, numerical, categorical) -> torch.Tensor:
+    """fp32 click probabilities ``[n]`` (device) of ``n >= 1`` local samples; the metrics are
+    left unchanged."""
+    out = torch.empty(int(numerical.shape[0]), dtype=torch.float32, device=self.dev)
+    self._eval_chunks(numerical, categorical, None, out)
+    return out
+
+  def eval_metrics(self, reset: bool = True) -> dict:
+    """``{"auc", "tie_bound", "log_loss", "samples"}`` over everything :meth:`evaluate` saw since
+    the last reset, summed over all ranks (collective at world size > 1: one all-reduce).
+    ``tie_bound`` bounds ``|auc - exact AUC|`` (see ``utils.metrics.BinnedAUC``)."""
+    hist = self.eval_auc.hist.view(-1)
+    packed = torch.cat([hist.double(), self._eval_loss, self._eval_count.double()])
+    if self.world > 1:
+      import torch.distributed as dist
+      dist.all_reduce(packed, group=self.emb.group)
+    packed = packed.cpu()  # counts stay exact in float64 below 2^53
+    nb = hist.numel()
+    res = auc_from_histogram(packed[:nb].round().long().view(2, -1))
+    loss, count = float(packed[nb]), int(round(float(packed[nb + 1])))
+    if reset:
+      self.eval_auc.reset()
+      self._eval_loss.zero_()
+      self._eval_count.zero_()
+    return {"auc": res.auc, "tie_bound": res.tie_bound,
+            "log_loss": loss / count if count else float("nan"), "samples": count}

@@ -933,6 +933,48 @@ void head_loss(const Tensor& x, const Tensor& w, const Tensor& bias, const Tenso
   check_launch();
 }
 
+// Evaluation head: probs = sigmoid(<x, w> + b); rows below *n_valid accumulate (+=) into the
+// BinnedAUC histogram, the fp64 loss sum and the sample count.
+void head_eval(const Tensor& x, const Tensor& w, const Tensor& bias, const Tensor& labels,
+               const Tensor& n_valid, Tensor probs, Tensor hist, Tensor loss_sum, Tensor count) {
+  check_bf16_2d(x, "x");
+  TORCH_CHECK(x.is_contiguous(), "x must be contiguous");
+  const int64_t batch = x.size(0), k = x.size(1);
+  TORCH_CHECK(k == 64 || k == 128 || k == 256 || k == 512 || k == 1024,
+              "head_eval supports K in {64,128,256,512,1024}");
+  const auto dev = x.device();
+  auto on_dev = [&](const Tensor& t, at::ScalarType dt, const char* name, const char* what) {
+    TORCH_CHECK(t.device() == dev && t.scalar_type() == dt && t.is_contiguous(), name, what);
+  };
+  on_dev(w, at::kBFloat16, "w", " must be a contiguous bf16 tensor on the device of x");
+  TORCH_CHECK(w.numel() == k, "w must hold K elements");
+  on_dev(bias, at::kBFloat16, "bias", " must be a contiguous bf16 tensor on the device of x");
+  TORCH_CHECK(bias.numel() >= 1, "bias must hold one element");
+  on_dev(labels, at::kFloat, "labels", " must be a contiguous fp32 tensor on the device of x");
+  TORCH_CHECK(labels.numel() == batch, "labels must hold one value per row");
+  on_dev(n_valid, at::kLong, "n_valid", " must be an int64 tensor on the device of x");
+  TORCH_CHECK(n_valid.numel() == 1, "n_valid must be one int64 word");
+  on_dev(probs, at::kFloat, "probs", " must be a contiguous fp32 tensor on the device of x");
+  TORCH_CHECK(probs.numel() == batch, "probs must hold one value per row");
+  on_dev(hist, at::kLong, "hist", " must be a contiguous int64 tensor on the device of x");
+  // T - 1 buckets with T >= 2; the bucket scale T - 1 must be exact in fp32
+  TORCH_CHECK(hist.dim() == 2 && hist.size(0) == 2 && hist.size(1) >= 1 &&
+                  hist.size(1) <= (int64_t{1} << 24),
+              "hist must be [2, T - 1] with 2 <= T <= 2^24 + 1");
+  on_dev(loss_sum, at::kDouble, "loss_sum", " must be an fp64 tensor on the device of x");
+  TORCH_CHECK(loss_sum.numel() == 1, "loss_sum must hold one element");
+  on_dev(count, at::kLong, "count", " must be an int64 tensor on the device of x");
+  TORCH_CHECK(count.numel() == 1, "count must hold one element");
+  c10::cuda::CUDAGuard guard(dev);
+  bool ok = de::launch_head_eval(x.data_ptr(), static_cast<int>(k), w.data_ptr(), bias.data_ptr(),
+                                 labels.data_ptr<float>(), batch, n_valid.data_ptr<int64_t>(),
+                                 probs.data_ptr<float>(), hist.data_ptr<int64_t>(),
+                                 static_cast<int>(hist.size(1)), loss_sum.data_ptr<double>(),
+                                 count.data_ptr<int64_t>(), sm_count(), cur_stream());
+  TORCH_CHECK(ok, "head_eval supports K in {64,128,256,512,1024}");
+  check_launch();
+}
+
 void dense_sgd(Tensor p32, Tensor p16, Tensor g32, const Tensor& lr, double grad_scale) {
   TORCH_CHECK(p32.is_cuda() && p32.scalar_type() == at::kFloat && g32.scalar_type() == at::kFloat &&
               p16.scalar_type() == at::kBFloat16 && lr.scalar_type() == at::kFloat);
@@ -1155,6 +1197,10 @@ TORCH_LIBRARY(de_b200, m) {
       "Tensor(b!) dw, Tensor(c!) db, Tensor(d!) dbias_prev, Tensor(e!) loss_sum, Tensor? logits) "
       "-> ()",
       &head_loss);
+  m.def(
+      "head_eval(Tensor x, Tensor w, Tensor bias, Tensor labels, Tensor n_valid, Tensor(a!) probs, "
+      "Tensor(b!) hist, Tensor(c!) loss_sum, Tensor(d!) count) -> ()",
+      &head_eval);
   m.def(
       "dense_sgd(Tensor(a!) p32, Tensor(b!) p16, Tensor(c!) g32, Tensor lr, float grad_scale) "
       "-> ()",

@@ -269,6 +269,11 @@ bool launch_head_loss(const void* x, int K, const void* w, const void* bias, con
                       int64_t batch, float inv_batch, void* dx, float* dw, float* db,
                       float* dbias_prev, float* loss_sum, float* logits_out, int sm_count,
                       cudaStream_t stream);
+// Forward-only head for evaluation: probs = sigmoid(<x, w> + b) for every row; rows below
+// *n_valid (device word) also add into hist [2, nb] (int64), loss_sum (fp64) and count (int64).
+bool launch_head_eval(const void* x, int K, const void* w, const void* bias, const float* labels,
+                      int64_t batch, const int64_t* n_valid, float* probs, int64_t* hist, int nb,
+                      double* loss_sum, int64_t* count, int sm_count, cudaStream_t stream);
 void launch_sgd_update(float* p32, void* p16, float* g32, const float* lr_ptr, float grad_scale,
                        int64_t n, int sm_count, cudaStream_t stream);
 void launch_cast_pad(const float* src, int src_cols, void* dst, int dst_cols, int64_t rows,

@@ -585,6 +585,77 @@ head_loss_kernel(const bf16* __restrict__ x, int K, const bf16* __restrict__ w,
   }
 }
 
+// Forward-only counterpart of head_loss_kernel (evaluation).  Each warp takes groups of 32
+// samples; every sample's logit is computed by the whole warp exactly as head_loss computes it
+// (lane-strided fmaf, the same shuffle reduction, bias added last), so the logits are bit
+// identical, and lane j keeps the logit of sample j of the group.  Per sample:
+//   probs[s] = sigmoid(logit)                                    (every row s < batch)
+//   rows s < *n_valid only: hist[label > 0.5][k(p)] += 1, loss_sum += BCE-with-logits, count += 1
+// with k(p) = clamp(ceil(fp32(p * nb)) - 1, 0, nb - 1), nb = hist columns (utils/metrics.py,
+// BinnedAUC).  Histogram adds are warp aggregated: one atomic per distinct bucket per group.
+template <int PL>
+__global__ void __launch_bounds__(256)
+head_eval_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w,
+                 const bf16* __restrict__ bias, const float* __restrict__ labels, int64_t batch,
+                 const int64_t* __restrict__ n_valid, float* __restrict__ probs,
+                 unsigned long long* __restrict__ hist, int nb, double* __restrict__ loss_sum,
+                 unsigned long long* __restrict__ count) {
+  constexpr int K = 32 * PL;
+  __shared__ float s_loss;
+  if (threadIdx.x == 0) s_loss = 0.f;
+  __syncthreads();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wpb = blockDim.x >> 5;
+  int64_t nv = *n_valid;
+  nv = nv < 0 ? 0 : (nv > batch ? batch : nv);
+  const float b0 = __bfloat162float(bias[0]);
+  const float nbf = static_cast<float>(nb);
+  float wreg[PL];
+#pragma unroll
+  for (int i = 0; i < PL; ++i) wreg[i] = __bfloat162float(w[lane + 32 * i]);
+  float loss_acc = 0.f;
+  for (int64_t g0 = (static_cast<int64_t>(blockIdx.x) * wpb + warp) * 32; g0 < batch;
+       g0 += static_cast<int64_t>(gridDim.x) * wpb * 32) {
+    const int rows = batch - g0 < 32 ? static_cast<int>(batch - g0) : 32;
+    float my_logit = 0.f;
+#pragma unroll 4
+    for (int j = 0; j < rows; ++j) {
+      const bf16* xr = x + (g0 + j) * K;
+      float dot = 0.f;
+#pragma unroll
+      for (int i = 0; i < PL; ++i) dot = fmaf(__bfloat162float(xr[lane + 32 * i]), wreg[i], dot);
+#pragma unroll
+      for (int off = 16; off > 0; off >>= 1) dot += __shfl_xor_sync(0xffffffffu, dot, off);
+      if (lane == j) my_logit = dot + b0;
+    }
+    const int64_t s = g0 + lane;
+    const bool has_row = lane < rows;
+    const bool valid = s < nv;  // implies has_row
+    const float logit = my_logit;
+    const float p = 1.f / (1.f + __expf(-logit));
+    if (has_row) probs[s] = p;
+    int key = -1;
+    if (valid) {
+      const float label = labels[s];
+      loss_acc += fmaxf(logit, 0.f) - logit * label + log1pf(__expf(-fabsf(logit)));
+      int k = static_cast<int>(ceilf(__fmul_rn(p, nbf))) - 1;
+      k = k < 0 ? 0 : (k > nb - 1 ? nb - 1 : k);
+      key = (label > 0.5f ? nb : 0) + k;
+    }
+    const unsigned peers = __match_any_sync(0xffffffffu, key);
+    if (key >= 0 && lane == __ffs(peers) - 1)
+      atomicAdd(hist + key, static_cast<unsigned long long>(__popc(peers)));
+  }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) loss_acc += __shfl_xor_sync(0xffffffffu, loss_acc, off);
+  if (lane == 0) atomicAdd(&s_loss, loss_acc);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    atomicAdd(loss_sum, static_cast<double>(s_loss));
+    if (blockIdx.x == 0) atomicAdd(count, static_cast<unsigned long long>(nv));
+  }
+}
+
 // p32 -= lr * g32 ; p16 = bf16(p32) ; g32 = 0   (lr read from device memory: graph replay safe)
 __global__ void __launch_bounds__(256)
 sgd_update_kernel(float* __restrict__ p32, bf16* __restrict__ p16, float* __restrict__ g32,
@@ -816,6 +887,31 @@ bool launch_head_loss(const void* x, int K, const void* w, const void* bias, con
     default: return false;
   }
 #undef DE_HEAD
+  return true;
+}
+
+bool launch_head_eval(const void* x, int K, const void* w, const void* bias, const float* labels,
+                      int64_t batch, const int64_t* n_valid, float* probs, int64_t* hist, int nb,
+                      double* loss_sum, int64_t* count, int sm_count, cudaStream_t stream) {
+  if (K != 64 && K != 128 && K != 256 && K != 512 && K != 1024) return false;
+  if (batch <= 0) return true;
+  const int threads = 256;  // 8 warps, 32 samples per warp and group
+  int64_t blocks = (batch + 255) / 256;
+  if (blocks > sm_count * 4) blocks = sm_count * 4;
+#define DE_HEAD_EVAL(PL)                                                                         \
+  head_eval_kernel<PL><<<static_cast<unsigned>(blocks), threads, 0, stream>>>(                  \
+      reinterpret_cast<const bf16*>(x), reinterpret_cast<const bf16*>(w),                        \
+      reinterpret_cast<const bf16*>(bias), labels, batch, n_valid, probs,                        \
+      reinterpret_cast<unsigned long long*>(hist), nb, loss_sum,                                 \
+      reinterpret_cast<unsigned long long*>(count))
+  switch (K) {
+    case 64: DE_HEAD_EVAL(2); break;
+    case 128: DE_HEAD_EVAL(4); break;
+    case 256: DE_HEAD_EVAL(8); break;
+    case 512: DE_HEAD_EVAL(16); break;
+    default: DE_HEAD_EVAL(32); break;
+  }
+#undef DE_HEAD_EVAL
   return true;
 }
 

@@ -47,6 +47,11 @@ def parse():
   p.add_argument("--test_combiner", action="store_true")
   p.add_argument("--dist_strategy", default="memory_balanced")
   p.add_argument("--fast", action="store_true", help="hand-scheduled step + CUDA graph")
+  p.add_argument("--eval_interval", type=int, default=0,
+                 help="with --fast: every N training steps, evaluate --eval_batches batches of "
+                      "the eval split on the GPU (binned AUC, log loss); 0 = off")
+  p.add_argument("--eval_batches", type=int, default=8,
+                 help="eval batches per periodic evaluation (--eval_interval)")
   p.add_argument("--amp", action="store_true", default=True)
   p.add_argument("--table_dtype", default="fp32", choices=sorted(TABLE_DTYPES),
                  help="storage of the model-parallel embedding tables (bf16 / fp16: half the "
@@ -108,7 +113,11 @@ def main():
                                 decay_start_step=args.decay_start_step,
                                 decay_steps=args.decay_steps)
   de.broadcast_variables(model)
-  if args.fast and cuda and args.dp_input:
+  fast = args.fast and cuda and args.dp_input
+  if args.eval_interval > 0 and not fast:
+    raise SystemExit("--eval_interval needs the hand-scheduled step: --fast with --dp_input on "
+                     "a GPU")
+  if fast:
     from distributed_embeddings_b200.models.dlrm_fast import DLRMTrainStep
     trainer = DLRMTrainStep(model, lr=args.learning_rate, scheduler=sched)
     step = lambda n, c, l: trainer.step(n, torch.stack([x.to(torch.int32) for x in c]), l)
@@ -119,6 +128,22 @@ def main():
   def batches():
     for _ in range(args.epochs):
       yield from train
+
+  def periodic_eval(i):
+    """Binned AUC (8000 thresholds, as the reference reports) and log loss on the GPU."""
+    for k, (num, cat, lab) in enumerate(evald):
+      if k >= args.eval_batches:
+        break
+      num = num.to(device).float()
+      lab = lab.reshape(-1)
+      if lab.numel() > num.shape[0]:  # global labels: this rank's slice
+        lab = lab[rank * num.shape[0]:(rank + 1) * num.shape[0]]
+      trainer.evaluate(num, torch.stack([c.to(device).to(torch.int32).reshape(-1) for c in cat]),
+                       lab.to(device).float())
+    m = trainer.eval_metrics()  # collective
+    if rank == 0:
+      print(f"eval step: {i} AUC: {m['auc']:.6f} tie_bound: {m['tie_bound']:.2e} "
+            f"log_loss: {m['log_loss']:.6f}", flush=True)
 
   for i, (num, cat, lab) in enumerate(batches()):
     num, lab = num.to(device).float(), lab.to(device)
@@ -133,6 +158,8 @@ def main():
         loss /= world
       if rank == 0:
         print("step: ", i, " loss: ", float(loss))
+    if args.eval_interval > 0 and (i + 1) % args.eval_interval == 0:
+      periodic_eval(i + 1)
 
   # evaluation: predictions of the local batch gathered on every rank, AUC on rank 0
   preds, labels = [], []

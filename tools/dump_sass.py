@@ -46,6 +46,7 @@ HOT = [
     ("integer_lookup", r"integer_lookup_kernel"),
     ("relu_bwd_bias", r"relu_bwd_bias_kernel"),
     ("head_loss_8", r"head_loss_kernel<8>"),
+    ("head_eval_8", r"head_eval_kernel<8>"),
     ("sgd_update", r"sgd_update_kernel"),
 ]
 
