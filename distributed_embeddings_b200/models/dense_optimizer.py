@@ -1,0 +1,128 @@
+"""Dense optimizer of the trainers: SGD, Adagrad or Adam on the data-parallel parameters (the MLPs
+and any replicated embedding tables).
+
+The reference applies one optimizer to every trainable variable; ``dense_optimizer`` lets the
+trainers do the same.  The math is that of the fused embedding update (``apply_update`` in
+``ops/csrc/sparse_update_kernels.cu``), with the defaults of
+:meth:`DistributedEmbedding.set_optimizer`:
+
+* Adagrad: ``acc += g * g; p -= lr * g / (sqrt(acc) + eps)`` (``eps=1e-7``,
+  ``initial_accumulator_value=0.1``);
+* Adam: ``m = b1 m + (1 - b1) g; v = b2 v + (1 - b2) g^2;
+  p -= lr * (m / (1 - b1^t)) / (sqrt(v / (1 - b2^t)) + eps)`` (``beta1=0.9``, ``beta2=0.999``,
+  ``eps=1e-8``).
+
+The learning rate is the trainer's device-resident ``lr_t`` word and Adam's step count ``t`` is a
+device-resident fp32 word advanced inside the step, so both follow a scheduler under CUDA-graph
+replay.
+
+Checkpoints have one format for every trainer: ``{"kind", "step", "slots"}`` where ``slots`` maps
+each dense parameter name (``model.named_parameters()``) to its state tensors shaped like the
+parameter (Adagrad ``[acc]``, Adam ``[m, v]``, SGD none) and ``step`` is Adam's ``t`` (0 for the
+kinds that keep no step count).
+"""
+from __future__ import annotations
+
+from typing import Dict, List, Optional, Sequence, Tuple
+
+import torch
+from torch import nn
+
+KINDS = ("sgd", "adagrad", "adam")
+_DEFAULTS = {
+    "sgd": {},
+    "adagrad": {"eps": 1e-7, "initial_accumulator_value": 0.1},
+    "adam": {"beta1": 0.9, "beta2": 0.999, "eps": 1e-8},
+}
+
+
+def dense_optimizer_config(kind: str, kwargs: Optional[dict] = None) -> dict:
+  """``{"kind", **hyperparameters}`` with the defaults of the embedding optimizer filled in."""
+  kind = str(kind).lower()
+  if kind not in KINDS:
+    raise ValueError(f"dense_optimizer must be one of {', '.join(KINDS)}, got {kind!r}")
+  cfg = dict(_DEFAULTS[kind])
+  unknown = sorted(set(kwargs or {}) - set(cfg))
+  if unknown:
+    raise ValueError(f"dense optimizer {kind!r} takes no argument(s) {', '.join(unknown)}")
+  cfg.update({k: float(v) for k, v in (kwargs or {}).items()})
+  cfg["kind"] = kind
+  return cfg
+
+
+def slot_init(cfg: dict) -> List[float]:
+  """Initial value of each state slot: Adagrad ``[acc]``, Adam ``[m, v]``, SGD none."""
+  return {"sgd": [], "adagrad": [cfg.get("initial_accumulator_value")],
+          "adam": [0.0, 0.0]}[cfg["kind"]]
+
+
+def dense_named_parameters(model: nn.Module) -> List[Tuple[str, nn.Parameter]]:
+  """The data-parallel parameters by name (model-parallel tables are tagged ``de_local``)."""
+  return [(n, p) for n, p in model.named_parameters() if not getattr(p, "de_local", False)]
+
+
+def check_state(cfg: dict, state: dict, names: Sequence[str]):
+  if state.get("kind") != cfg["kind"]:
+    raise ValueError(f"dense optimizer state of kind {state.get('kind')!r} cannot be loaded into "
+                     f"a {cfg['kind']!r} dense optimizer")
+  slots = state.get("slots", {})
+  missing = sorted(set(names) - set(slots))
+  if slot_init(cfg) and missing:
+    raise ValueError(f"dense optimizer state misses parameter(s) {', '.join(missing)}")
+
+
+class FlatDenseOptimizer:
+  """Adagrad / Adam state laid out like a trainer's flat fp32 master buffer ``p32`` and the fused
+  update over it (``dense_adagrad`` / ``dense_adam``); SGD keeps no state and launches
+  ``dense_sgd``.  Pad elements keep ``g = 0``, so they stay at ``p = 0`` and their state at its
+  initial value."""
+
+  def __init__(self, cfg: dict, p32: torch.Tensor):
+    self.cfg = cfg
+    self.kind = cfg["kind"]
+    self.p32 = p32
+    self.state = [torch.full_like(p32, v) for v in slot_init(cfg)]
+    self.step_t = torch.zeros(1, dtype=torch.float32, device=p32.device) \
+        if self.kind == "adam" else None
+
+  def apply(self, ops, p16: torch.Tensor, g32: torch.Tensor, lr_t: torch.Tensor):
+    """p32 update + ``p16 = bf16(p32)`` + ``g32 = 0``, one launch (Adam: plus the step word)."""
+    c = self.cfg
+    if self.kind == "sgd":
+      ops.dense_sgd(self.p32, p16, g32, lr_t, 1.0)
+    elif self.kind == "adagrad":
+      ops.dense_adagrad(self.p32, p16, g32, self.state[0], lr_t, c["eps"])
+    else:
+      self.step_t.add_(1.0)  # device counter: the bias corrections stay right under graph replay
+      ops.dense_adam(self.p32, p16, g32, self.state[0], self.state[1], lr_t, self.step_t,
+                     c["beta1"], c["beta2"], c["eps"])
+
+  def snapshot(self) -> List[torch.Tensor]:
+    return [s.clone() for s in self.state] + ([self.step_t.clone()] if self.step_t is not None
+                                              else [])
+
+  def restore(self, snap: Sequence[torch.Tensor]):
+    for dst, src in zip(self.state + ([self.step_t] if self.step_t is not None else []), snap):
+      dst.copy_(src)
+
+  def _slot_view(self, s: torch.Tensor, p: torch.Tensor) -> torch.Tensor:
+    """The elements of ``s`` that hold the state of parameter ``p`` (a view into ``p32``)."""
+    if p.untyped_storage().data_ptr() != self.p32.untyped_storage().data_ptr():
+      raise RuntimeError("dense parameter does not live in the flat master buffer")
+    return s.as_strided(p.shape, p.stride(), p.storage_offset())
+
+  def state_dict(self, model: nn.Module) -> Dict:
+    step = int(round(float(self.step_t.item()))) if self.step_t is not None else 0
+    slots = {n: [self._slot_view(s, p).clone() for s in self.state]
+             for n, p in dense_named_parameters(model)} if self.state else {}
+    return {"kind": self.kind, "step": step, "slots": slots}
+
+  def load_state_dict(self, model: nn.Module, state: Dict):
+    named = dense_named_parameters(model)
+    check_state(self.cfg, state, [n for n, _ in named])
+    if self.state:
+      for n, p in named:
+        for s, src in zip(self.state, state["slots"][n]):
+          self._slot_view(s, p).copy_(src)
+    if self.step_t is not None:
+      self.step_t.fill_(float(state.get("step", 0)))

@@ -18,6 +18,7 @@ math as one static schedule over preallocated buffers:
 * the whole step is captured in a CUDA graph and replayed (launch bound otherwise).
 
 Same model/optimizer as the reference example (examples/dlrm/main.py:76-209): SGD, shared lr.
+``dense_optimizer`` swaps the fused dense SGD for fused Adagrad or Adam (see ``dense_optimizer``).
 """
 from __future__ import annotations
 
@@ -33,6 +34,7 @@ from ..parallel.fused import FusedEngine
 from ..utils import nvtx
 from ..utils.lr_schedule import LearningRateScheduler
 from ..utils.metrics import BinnedAUC, auc_from_histogram
+from .dense_optimizer import FlatDenseOptimizer, dense_optimizer_config
 from .dlrm import DLRM
 
 
@@ -54,12 +56,18 @@ class _Layer:
 
 
 class DLRMTrainStep:
-  """Static-schedule training step for :class:`DLRM` on the fused embedding back end."""
+  """Static-schedule training step for :class:`DLRM` on the fused embedding back end.
+
+  ``dense_optimizer`` (``sgd`` | ``adagrad`` | ``adam``, hyperparameters in
+  ``dense_optimizer_kwargs``) updates the MLPs and any replicated tables with the shared
+  learning rate.  Replicated tables (``data_parallel_threshold``) need
+  ``dense_optimizer == embedding_optimizer``."""
 
   def __init__(self, model: DLRM, lr: float = 24.0, embedding_optimizer: str = "sgd",
                scheduler: Optional[LearningRateScheduler] = None, use_cuda_graph: bool = True,
                embedding_optimizer_kwargs: Optional[dict] = None, overlap: bool = True,
-               gemm: str = "cublas", eval_thresholds: int = 8000):
+               gemm: str = "cublas", eval_thresholds: int = 8000, dense_optimizer: str = "sgd",
+               dense_optimizer_kwargs: Optional[dict] = None):
     if gemm not in ("cublas", "fused_dgrad", "tcgen05", "tcgen05_pair"):
       raise ValueError("gemm must be cublas | fused_dgrad | tcgen05 | tcgen05_pair")
     # cublas: cuBLASLt everywhere.  fused_dgrad: forward/wgrad on cuBLASLt, dgrad on the
@@ -67,6 +75,7 @@ class DLRMTrainStep:
     # tcgen05: forward layers on the first-party kernel as well.  tcgen05_pair: same, with the
     # 2-CTA cluster kernel for layers at least 256 wide.  (The option names are historical.)
     self.gemm = gemm
+    self.dense_cfg = dense_optimizer_config(dense_optimizer, dense_optimizer_kwargs)
     self.model = model
     self.emb = model.embedding
     if self.emb.backend != "fused":
@@ -103,15 +112,18 @@ class DLRMTrainStep:
     layers = self.bottom + self.top + [self.head]
     # replicated (data-parallel) embedding tables live in the flat dense buffers too: their
     # local-batch gradient is scattered into the gradient bucket, all-reduced with the MLP
-    # gradients and applied by the same fused SGD kernel.  They come first so that they belong to
-    # the bucket that is reduced last (DE_B200_AR_OVERLAP).  Covered by the 2- and 8-GPU tests
-    # (tests/test_dist_gpu.py: replicated-table cases); bench.py replicates the < 2500-row tables.
+    # gradients and applied densely by the fused dense optimizer kernel (the reference's
+    # sparse_as_dense), so the dense and embedding optimizers must agree.  They come first so that
+    # they belong to the bucket that is reduced last (DE_B200_AR_OVERLAP).  Covered by the 2- and
+    # 8-GPU tests (tests/test_dist_gpu.py: replicated-table cases); bench.py replicates the
+    # < 2500-row tables.
     self._dp_slots = []
     pos = 0
     if len(self.emb.dp_layers):
-      if embedding_optimizer != "sgd":
-        raise ValueError("replicated tables in the fast step are updated by the dense SGD "
-                         "kernel: use embedding_optimizer='sgd' or data_parallel_threshold=None")
+      if embedding_optimizer.lower() != self.dense_cfg["kind"]:
+        raise ValueError("replicated tables in the fast step are updated by the dense optimizer "
+                         "kernel: use the same embedding_optimizer and dense_optimizer ('sgd', "
+                         "'adagrad' or 'adam') or data_parallel_threshold=None")
       for layer in self.emb.dp_layers:
         w = layer.embeddings
         self._dp_slots.append((pos, tuple(w.shape)))
@@ -162,8 +174,9 @@ class DLRMTrainStep:
         L.w16T = torch.empty(L.in_pad, L.out_f, dtype=torch.bfloat16, device=dev)
       self.p16.copy_(self.p32)
       self._refresh_transposes()
+    self.dense_opt = FlatDenseOptimizer(self.dense_cfg, self.p32)
     self.lr_t = torch.full((1,), float(lr), dtype=torch.float32, device=dev)
-    self.engine.share_lr(self.lr_t)  # dense SGD and the fused embedding update read one word
+    self.engine.share_lr(self.lr_t)  # dense optimizer and fused embedding update read one word
     self.lr = float(lr)
     self.loss = torch.zeros(1, dtype=torch.float32, device=dev)
     self._batch = None
@@ -365,7 +378,7 @@ class DLRMTrainStep:
       self._wgrad(L, x)
       if i > 0:
         self._dgrad_relu(L, x, self.bottom[i - 1].dy, self.bottom[i - 1].gb)
-    # dense gradient all-reduce (one NVLink kernel, averaged) + fused SGD / re-cast / zero
+    # dense gradient all-reduce (one NVLink kernel, averaged) + fused optimizer / re-cast / zero
     if self._dp_slots and self._side is not None:
       # the replicated tables' gradients are produced by the embedding backward on the side stream
       torch.cuda.current_stream().wait_stream(self._side)
@@ -382,7 +395,7 @@ class DLRMTrainStep:
         torch.cuda.current_stream().wait_stream(ar)
       else:
         self.ctx.allreduce_(self.gsym, self.n_flat, torch.float32, scale=1.0 / self.world)
-    ops.dense_sgd(self.p32, self.p16, self.g32, self.lr_t, 1.0)
+    self.dense_opt.apply(ops, self.p16, self.g32, self.lr_t)
     self._refresh_transposes()
     if self._side is not None:
       torch.cuda.current_stream().wait_stream(self._side)
@@ -464,6 +477,8 @@ class DLRMTrainStep:
       # is zero while warming up so the extra passes leave the weights untouched.
       self.lr_t.zero_()
       self.engine.dry_updates(True)  # optimizer state (Adagrad / Adam) stays untouched as well
+      # a zero rate still moves the dense Adagrad / Adam state and step word: put them back
+      dense_snap = self.dense_opt.snapshot()
       s = torch.cuda.Stream(device=self.dev)
       s.wait_stream(torch.cuda.current_stream())
       with torch.cuda.stream(s):
@@ -472,6 +487,7 @@ class DLRMTrainStep:
       torch.cuda.current_stream().wait_stream(s)
       torch.cuda.synchronize()
       self.engine.dry_updates(False)
+      self.dense_opt.restore(dense_snap)
       g = torch.cuda.CUDAGraph()
       with torch.cuda.graph(g):
         self._step_impl()
@@ -483,6 +499,16 @@ class DLRMTrainStep:
   def step(self, numerical, categorical, labels) -> torch.Tensor:
     self.load_batch(numerical, categorical, labels)
     return self.run()
+
+  # ------------------------------------------------------------------ checkpoint
+  def dense_optimizer_state(self) -> dict:
+    """``{"kind", "step", "slots": {param_name: [tensor, ...]}}``: the dense optimizer state,
+    each slot shaped like its parameter (no padding); the format of every trainer."""
+    return self.dense_opt.state_dict(self.model)
+
+  def load_dense_optimizer_state(self, state: dict):
+    """Restore :meth:`dense_optimizer_state` output (of any trainer); another kind raises."""
+    self.dense_opt.load_state_dict(self.model, state)
 
   # ------------------------------------------------------------------ evaluation
   # The forward-only schedule reuses the step's input and activation buffers and its GEMM back

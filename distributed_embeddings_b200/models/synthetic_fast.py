@@ -10,7 +10,7 @@ buffers:
   the module costs no kernel, the numerical features are cast into their columns;
 * dense parameters live in one flat fp32 master buffer with a bf16 shadow, gradients in one flat
   (symmetric) buffer reduced by the one-kernel NVLink all-reduce, one fused kernel does
-  SGD + re-cast + gradient zeroing;
+  SGD (or Adagrad / Adam, ``dense_optimizer``) + re-cast + gradient zeroing;
 * forward layers: bf16 GEMMs with fused bias + ReLU epilogues; backward: weight-gradient and
   data-gradient GEMMs + the fused ReLU-backward / bias-gradient kernel; final layer + BCE loss
   + their backward in one kernel;
@@ -35,15 +35,22 @@ from ..parallel.comm import CommContext
 from ..parallel.fused import FusedEngine
 from ..ops.ragged import RaggedIds
 from ..utils import nvtx
+from .dense_optimizer import FlatDenseOptimizer, dense_optimizer_config
 from .dlrm_fast import _Layer, _pad8
 from .synthetic import SyntheticModel
 
 
 class SyntheticTrainStep:
-  """Static-schedule training step for :class:`SyntheticModel` on the fused embedding back end."""
+  """Static-schedule training step for :class:`SyntheticModel` on the fused embedding back end.
+
+  ``dense_optimizer`` (``sgd`` | ``adagrad`` | ``adam``, hyperparameters in
+  ``dense_optimizer_kwargs``) updates the MLP with the shared learning rate; the reference's
+  configuration is ``embedding_optimizer="adagrad", dense_optimizer="adagrad"``."""
 
   def __init__(self, model: SyntheticModel, lr: float = 0.001, embedding_optimizer: str = "adagrad",
-               use_cuda_graph: bool = True, embedding_optimizer_kwargs: Optional[dict] = None):
+               use_cuda_graph: bool = True, embedding_optimizer_kwargs: Optional[dict] = None,
+               dense_optimizer: str = "sgd", dense_optimizer_kwargs: Optional[dict] = None):
+    self.dense_cfg = dense_optimizer_config(dense_optimizer, dense_optimizer_kwargs)
     self.model = model
     self.emb = model.embedding
     why = self.unsupported_reason(model)
@@ -103,6 +110,7 @@ class SyntheticTrainStep:
         L.gw = self.g32[L.w_off:L.w_off + L.w_numel].view(L.out_f, L.in_pad)
         L.gb = self.g32[L.b_off:L.b_off + L.b_numel]
       self.p16.copy_(self.p32)
+    self.dense_opt = FlatDenseOptimizer(self.dense_cfg, self.p32)
     self.lr = float(lr)
     self.lr_t = torch.full((1,), float(lr), dtype=torch.float32, device=dev)
     self.loss = torch.zeros(1, dtype=torch.float32, device=dev)
@@ -204,7 +212,7 @@ class SyntheticTrainStep:
       eng._backward_mp()
     if self.world > 1:
       self.ctx.allreduce_(self.gsym, self.n_flat, torch.float32, scale=1.0 / self.world)
-    ops.dense_sgd(self.p32, self.p16, self.g32, self.lr_t, 1.0)
+    self.dense_opt.apply(ops, self.p16, self.g32, self.lr_t)
     torch.cuda.current_stream().wait_stream(side)
 
   def _step_impl(self):
@@ -243,10 +251,12 @@ class SyntheticTrainStep:
       return self.loss
     if self._graph is None:
       # warm up on a side stream with a zero learning rate and dry embedding updates (cuBLAS
-      # workspaces, lazy kernel loading; neither weights nor optimizer state move), then capture
+      # workspaces, lazy kernel loading; neither weights nor optimizer state move), then capture.
+      # A zero rate still moves the dense Adagrad / Adam state and step word: they are put back.
       self.lr_t.zero_()
       eng.update_lr(0.0)
       eng.dry_updates(True)
+      dense_snap = self.dense_opt.snapshot()
       s = torch.cuda.Stream(device=self.dev)
       s.wait_stream(torch.cuda.current_stream())
       with torch.cuda.stream(s):
@@ -255,6 +265,7 @@ class SyntheticTrainStep:
       torch.cuda.current_stream().wait_stream(s)
       torch.cuda.synchronize()
       eng.dry_updates(False)
+      self.dense_opt.restore(dense_snap)
       g = torch.cuda.CUDAGraph()
       with torch.cuda.graph(g):
         self._step_impl()
@@ -266,3 +277,12 @@ class SyntheticTrainStep:
   def step(self, numerical, categorical, labels) -> torch.Tensor:
     self.load_batch(numerical, categorical, labels)
     return self.run()
+
+  def dense_optimizer_state(self) -> dict:
+    """``{"kind", "step", "slots": {param_name: [tensor, ...]}}``: the dense optimizer state,
+    each slot shaped like its parameter (no padding); the format of every trainer."""
+    return self.dense_opt.state_dict(self.model)
+
+  def load_dense_optimizer_state(self, state: dict):
+    """Restore :meth:`dense_optimizer_state` output (of any trainer); another kind raises."""
+    self.dense_opt.load_state_dict(self.model, state)

@@ -15,6 +15,7 @@ from torch import nn
 from ..parallel.comm import CommContext
 from ..parallel.hybrid import GradBucket, SparseRowOptimizer
 from ..utils.lr_schedule import LearningRateScheduler
+from .dense_optimizer import check_state, dense_optimizer_config, slot_init
 
 
 class HybridTrainer:
@@ -27,13 +28,20 @@ class HybridTrainer:
     lr: learning rate (dense SGD and fused embedding optimizer share it like the reference).
     embedding_optimizer: ``sgd`` | ``adagrad`` | ``rowwise_adagrad`` | ``adam``.
     scheduler: optional :class:`LearningRateScheduler`.
+    dense_optimizer: ``sgd`` | ``adagrad`` | ``adam`` for the dense parameters (MLPs and
+      replicated tables), hyperparameters in ``dense_optimizer_kwargs`` (see
+      ``models/dense_optimizer.py``); ``momentum`` applies to ``sgd`` only.
   """
 
   def __init__(self, model: nn.Module, lr: float = 24.0, embedding_optimizer: str = "sgd",
                scheduler: Optional[LearningRateScheduler] = None, momentum: float = 0.0,
                embedding_optimizer_kwargs: Optional[dict] = None,
                loss_fn: Optional[Callable] = None, use_cuda_graph: bool = False,
-               graph_warmup_steps: int = 3):
+               graph_warmup_steps: int = 3, dense_optimizer: str = "sgd",
+               dense_optimizer_kwargs: Optional[dict] = None):
+    self.dense_cfg = dense_optimizer_config(dense_optimizer, dense_optimizer_kwargs)
+    if momentum != 0.0 and self.dense_cfg["kind"] != "sgd":
+      raise ValueError("momentum applies to dense_optimizer='sgd' only")
     self.model = model
     self.emb = model.embedding
     self.emb.set_optimizer(embedding_optimizer, lr=lr, **(embedding_optimizer_kwargs or {}))
@@ -57,6 +65,13 @@ class HybridTrainer:
     # value while the embedding lr (device resident as well) keeps changing
     self.momentum = momentum
     self.lr_t = torch.full((), float(lr), dtype=torch.float32, device=dev)
+    # dense Adagrad / Adam: state per bucket parameter, Adam's step count as a device word (both
+    # follow a scheduler under graph replay); the gradients are the all-reduced bucket views
+    names = {id(p): n for n, p in model.named_parameters()}
+    self._dense_names = [names[id(p)] for p in self.bucket.params]
+    self.dense_state = [[torch.full_like(p, v, memory_format=torch.contiguous_format)
+                         for p in self.bucket.params] for v in slot_init(self.dense_cfg)]
+    self.dense_step_t = torch.zeros((), dtype=torch.float32, device=dev)
     self.loss_fn = loss_fn or nn.BCEWithLogitsLoss()
     # whole-step CUDA graph: the first `graph_warmup_steps` calls run eagerly (real steps), the
     # next call captures forward + backward + all-reduce + optimizer and every call replays it
@@ -78,6 +93,9 @@ class HybridTrainer:
     self.emb.set_learning_rate(lr)
 
   def _dense_step(self):
+    if self.dense_cfg["kind"] != "sgd":
+      self._adaptive_dense_step()
+      return
     if self.momentum != 0.0:
       if self._graph is not None or (self.use_cuda_graph and self.scheduler is not None):
         raise RuntimeError("momentum SGD keeps its learning rate on the host: it cannot follow a "
@@ -96,6 +114,51 @@ class HybridTrainer:
       else:
         for p, g in zip(params, grads):
           p.sub_(g * self.lr_t)
+
+  def _adaptive_dense_step(self):
+    """Dense Adagrad / Adam with the expressions of the fused kernels, on device words."""
+    c, params, grads = self.dense_cfg, self.bucket.params, self.bucket.views
+    if not params:
+      return
+    with torch.no_grad():
+      if c["kind"] == "adagrad":
+        acc = self.dense_state[0]
+        torch._foreach_addcmul_(acc, grads, grads)
+        num = grads
+        den = torch._foreach_sqrt(acc)
+      else:
+        m, v = self.dense_state
+        self.dense_step_t.add_(1.0)
+        torch._foreach_mul_(m, c["beta1"])
+        torch._foreach_add_(m, grads, alpha=1.0 - c["beta1"])
+        torch._foreach_mul_(v, c["beta2"])
+        torch._foreach_addcmul_(v, grads, grads, value=1.0 - c["beta2"])
+        bias1 = 1.0 - torch.pow(c["beta1"], self.dense_step_t)
+        bias2 = 1.0 - torch.pow(c["beta2"], self.dense_step_t)
+        num = torch._foreach_div(m, bias1)
+        den = torch._foreach_div(v, bias2)
+        torch._foreach_sqrt_(den)
+      torch._foreach_add_(den, c["eps"])
+      upd = torch._foreach_mul(num, self.lr_t)
+      torch._foreach_div_(upd, den)
+      torch._foreach_sub_(params, upd)
+
+  def dense_optimizer_state(self) -> dict:
+    """``{"kind", "step", "slots": {param_name: [tensor, ...]}}``: the dense optimizer state,
+    each slot shaped like its parameter; the format of every trainer."""
+    slots = {n: [s[i].detach().clone() for s in self.dense_state]
+             for i, n in enumerate(self._dense_names)} if self.dense_state else {}
+    step = int(round(float(self.dense_step_t))) if self.dense_cfg["kind"] == "adam" else 0
+    return {"kind": self.dense_cfg["kind"], "step": step, "slots": slots}
+
+  def load_dense_optimizer_state(self, state: dict):
+    """Restore :meth:`dense_optimizer_state` output (of any trainer); another kind raises."""
+    check_state(self.dense_cfg, state, self._dense_names)
+    if self.dense_state:
+      for i, n in enumerate(self._dense_names):
+        for s, src in zip(self.dense_state, state["slots"][n]):
+          s[i].copy_(src)
+    self.dense_step_t.fill_(float(state.get("step", 0)))
 
   def step(self, numerical, categorical, labels, staged: bool = False) -> torch.Tensor:
     if self.scheduler is not None:

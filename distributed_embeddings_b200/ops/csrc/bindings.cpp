@@ -986,6 +986,58 @@ void dense_sgd(Tensor p32, Tensor p16, Tensor g32, const Tensor& lr, double grad
   check_launch();
 }
 
+// Host checks shared by dense_adagrad / dense_adam: flat fp32 buffers (bf16 for p16) of one size,
+// a multiple of 4 elements, 16-byte aligned (the kernel moves float4 / 4 x bf16); scalar device
+// words for the learning rate and the step.  Messages carry strings only.
+void check_dense_opt(const Tensor& p32, const Tensor& p16, const Tensor& g32,
+                     const std::vector<std::pair<const Tensor*, const char*>>& state,
+                     const Tensor& lr, const Tensor* step) {
+  TORCH_CHECK(p32.is_cuda(), "p32 must be a CUDA tensor");
+  const auto dev = p32.device();
+  const int64_t n = p32.numel();
+  TORCH_CHECK(n % 4 == 0, "the flat buffers must hold a multiple of 4 elements");
+  auto flat = [&](const Tensor& t, at::ScalarType dt, const char* name, const char* what) {
+    TORCH_CHECK(t.device() == dev && t.scalar_type() == dt, name, what);
+    TORCH_CHECK(t.is_contiguous(), name, " must be contiguous");
+    TORCH_CHECK(t.numel() == n, name, " must have as many elements as p32");
+    TORCH_CHECK((reinterpret_cast<uintptr_t>(t.data_ptr()) & 15) == 0, name,
+                " must be 16-byte aligned");
+  };
+  flat(p32, at::kFloat, "p32", " must be an fp32 tensor");
+  flat(p16, at::kBFloat16, "p16", " must be a bf16 tensor on the device of p32");
+  flat(g32, at::kFloat, "g32", " must be an fp32 tensor on the device of p32");
+  for (const auto& s : state)
+    flat(*s.first, at::kFloat, s.second, " must be an fp32 tensor on the device of p32");
+  auto word = [&](const Tensor& t, const char* name) {
+    TORCH_CHECK(t.device() == dev && t.scalar_type() == at::kFloat && t.numel() == 1, name,
+                " must be a one-element fp32 tensor on the device of p32");
+  };
+  word(lr, "lr");
+  if (step != nullptr) word(*step, "step");
+}
+
+void dense_adagrad(Tensor p32, Tensor p16, Tensor g32, Tensor acc, const Tensor& lr, double eps) {
+  check_dense_opt(p32, p16, g32, {{&acc, "acc"}}, lr, nullptr);
+  c10::cuda::CUDAGuard guard(p32.device());
+  de::launch_dense_opt(de::kOptAdagrad, p32.data_ptr<float>(), p16.data_ptr(),
+                       g32.data_ptr<float>(), acc.data_ptr<float>(), nullptr,
+                       lr.data_ptr<float>(), nullptr, 0.f, 0.f, static_cast<float>(eps),
+                       p32.numel(), sm_count(), cur_stream());
+  check_launch();
+}
+
+void dense_adam(Tensor p32, Tensor p16, Tensor g32, Tensor m, Tensor v, const Tensor& lr,
+                const Tensor& step, double beta1, double beta2, double eps) {
+  check_dense_opt(p32, p16, g32, {{&m, "m"}, {&v, "v"}}, lr, &step);
+  c10::cuda::CUDAGuard guard(p32.device());
+  de::launch_dense_opt(de::kOptAdam, p32.data_ptr<float>(), p16.data_ptr(),
+                       g32.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(),
+                       lr.data_ptr<float>(), step.data_ptr<float>(), static_cast<float>(beta1),
+                       static_cast<float>(beta2), static_cast<float>(eps), p32.numel(),
+                       sm_count(), cur_stream());
+  check_launch();
+}
+
 void cast_pad(const Tensor& src, Tensor dst) {
   TORCH_CHECK(src.is_cuda() && src.scalar_type() == at::kFloat && src.is_contiguous());
   TORCH_CHECK(dst.scalar_type() == at::kBFloat16 && dst.is_contiguous() &&
@@ -1205,6 +1257,14 @@ TORCH_LIBRARY(de_b200, m) {
       "dense_sgd(Tensor(a!) p32, Tensor(b!) p16, Tensor(c!) g32, Tensor lr, float grad_scale) "
       "-> ()",
       &dense_sgd);
+  m.def(
+      "dense_adagrad(Tensor(a!) p32, Tensor(b!) p16, Tensor(c!) g32, Tensor(d!) acc, Tensor lr, "
+      "float eps) -> ()",
+      &dense_adagrad);
+  m.def(
+      "dense_adam(Tensor(a!) p32, Tensor(b!) p16, Tensor(c!) g32, Tensor(d!) m, Tensor(e!) v, "
+      "Tensor lr, Tensor step, float beta1, float beta2, float eps) -> ()",
+      &dense_adam);
   m.def("cast_pad(Tensor src, Tensor(a!) dst) -> ()", &cast_pad);
   m.def(
       "gemm_tn_bias_act(Tensor a, Tensor b, Tensor? bias, Tensor(a!) out, bool relu, int block_n) "

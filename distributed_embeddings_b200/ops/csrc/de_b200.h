@@ -276,6 +276,12 @@ bool launch_head_eval(const void* x, int K, const void* w, const void* bias, con
                       double* loss_sum, int64_t* count, int sm_count, cudaStream_t stream);
 void launch_sgd_update(float* p32, void* p16, float* g32, const float* lr_ptr, float grad_scale,
                        int64_t n, int sm_count, cudaStream_t stream);
+// Fused dense Adagrad (kind kOptAdagrad, s0 = accumulator) or Adam (kOptAdam, s0 / s1 = m / v,
+// *step_ptr = t after this step) + bf16 re-cast + gradient zeroing over n (multiple of 4) fp32
+// elements; false for another kind.
+bool launch_dense_opt(int kind, float* p32, void* p16, float* g32, float* s0, float* s1,
+                      const float* lr_ptr, const float* step_ptr, float beta1, float beta2,
+                      float eps, int64_t n, int sm_count, cudaStream_t stream);
 void launch_cast_pad(const float* src, int src_cols, void* dst, int dst_cols, int64_t rows,
                      cudaStream_t stream);
 

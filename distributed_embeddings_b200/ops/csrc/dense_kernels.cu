@@ -680,6 +680,63 @@ sgd_update_kernel(float* __restrict__ p32, bf16* __restrict__ p16, float* __rest
   }
 }
 
+// Adagrad / Adam over the flat dense buffers, element by element with the expressions of the
+// embedding update (apply_update in sparse_update_kernels.cu), then p16 = bf16(p32) and g32 = 0
+// (the next step's gradient kernels accumulate into g32).  lr and Adam's step count t are device
+// words: graph replay safe.  s0 = Adagrad accumulator or Adam m, s1 = Adam v.
+template <int KIND>
+__device__ __forceinline__ void dense_opt_elem(float& p, float& a, float& v, float g, float lr,
+                                               float beta1, float beta2, float bias1, float bias2,
+                                               float eps) {
+  if constexpr (KIND == kOptAdagrad) {
+    a = fmaf(g, g, a);
+    p -= lr * g / (sqrtf(a) + eps);
+  } else {
+    a = beta1 * a + (1.f - beta1) * g;
+    v = beta2 * v + (1.f - beta2) * g * g;
+    const float mh = a / bias1;
+    const float vh = v / bias2;
+    p -= lr * mh / (sqrtf(vh) + eps);
+  }
+}
+
+template <int KIND>
+__global__ void __launch_bounds__(256)
+dense_opt_kernel(float* __restrict__ p32, bf16* __restrict__ p16, float* __restrict__ g32,
+                 float* __restrict__ s0, float* __restrict__ s1, const float* __restrict__ lr_ptr,
+                 const float* __restrict__ step_ptr, float beta1, float beta2, float eps,
+                 int64_t n_vec4) {
+  const float lr = *lr_ptr;
+  float bias1 = 1.f, bias2 = 1.f;
+  if constexpr (KIND == kOptAdam) {  // bias corrections as resolve_step computes them
+    const float t = *step_ptr;
+    bias1 = 1.f - powf(beta1, t);
+    bias2 = 1.f - powf(beta2, t);
+  }
+  const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n_vec4;
+       i += stride) {
+    float4 p = reinterpret_cast<float4*>(p32)[i];
+    const float4 g = reinterpret_cast<const float4*>(g32)[i];
+    float4 a = reinterpret_cast<float4*>(s0)[i];
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if constexpr (KIND == kOptAdam) v = reinterpret_cast<float4*>(s1)[i];
+    dense_opt_elem<KIND>(p.x, a.x, v.x, g.x, lr, beta1, beta2, bias1, bias2, eps);
+    dense_opt_elem<KIND>(p.y, a.y, v.y, g.y, lr, beta1, beta2, bias1, bias2, eps);
+    dense_opt_elem<KIND>(p.z, a.z, v.z, g.z, lr, beta1, beta2, bias1, bias2, eps);
+    dense_opt_elem<KIND>(p.w, a.w, v.w, g.w, lr, beta1, beta2, bias1, bias2, eps);
+    reinterpret_cast<float4*>(p32)[i] = p;
+    reinterpret_cast<float4*>(s0)[i] = a;
+    if constexpr (KIND == kOptAdam) reinterpret_cast<float4*>(s1)[i] = v;
+    reinterpret_cast<float4*>(g32)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    __nv_bfloat162 lo = __floats2bfloat162_rn(p.x, p.y), hi = __floats2bfloat162_rn(p.z, p.w);
+    uint2 o;
+    o.x = *reinterpret_cast<uint32_t*>(&lo);
+    o.y = *reinterpret_cast<uint32_t*>(&hi);
+    reinterpret_cast<uint2*>(p16)[i] = o;
+  }
+}
+
 // dst[r, 0:dst_cols] = bf16(src[r, 0:src_cols]) zero padded
 __global__ void cast_pad_kernel(const float* __restrict__ src, int src_cols, bf16* __restrict__ dst,
                                 int dst_cols, int64_t rows) {
@@ -923,6 +980,25 @@ void launch_sgd_update(float* p32, void* p16, float* g32, const float* lr_ptr, f
   if (blocks > sm_count * 8) blocks = sm_count * 8;
   sgd_update_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
       p32, reinterpret_cast<bf16*>(p16), g32, lr_ptr, grad_scale, n_vec4);
+}
+
+bool launch_dense_opt(int kind, float* p32, void* p16, float* g32, float* s0, float* s1,
+                      const float* lr_ptr, const float* step_ptr, float beta1, float beta2,
+                      float eps, int64_t n, int sm_count, cudaStream_t stream) {
+  if (kind != kOptAdagrad && kind != kOptAdam) return false;
+  const int64_t n_vec4 = n / 4;  // buffers are padded to 16 bytes
+  if (n_vec4 <= 0) return true;
+  int64_t blocks = (n_vec4 + 255) / 256;
+  if (blocks > sm_count * 8) blocks = sm_count * 8;
+  if (kind == kOptAdagrad)
+    dense_opt_kernel<kOptAdagrad><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
+        p32, reinterpret_cast<bf16*>(p16), g32, s0, nullptr, lr_ptr, nullptr, 0.f, 0.f, eps,
+        n_vec4);
+  else
+    dense_opt_kernel<kOptAdam><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
+        p32, reinterpret_cast<bf16*>(p16), g32, s0, s1, lr_ptr, step_ptr, beta1, beta2, eps,
+        n_vec4);
+  return true;
 }
 
 void launch_cast_pad(const float* src, int src_cols, void* dst, int dst_cols, int64_t rows,

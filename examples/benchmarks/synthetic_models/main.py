@@ -2,7 +2,11 @@
 """Benchmark of the synthetic model zoo (reference examples/benchmarks/synthetic_models/main.py).
 
   torchrun --nproc-per-node 8 --master-addr 127.0.0.1 examples/benchmarks/synthetic_models/main.py \
-      --model small --optimizer adagrad --batch_size 65536 --alpha 1.05
+      --model small --optimizer adagrad --dense_optimizer adagrad --batch_size 65536 --alpha 1.05
+
+The reference applies one optimizer to every variable: its configuration is
+``--optimizer adagrad --dense_optimizer adagrad``.  The default ``--dense_optimizer sgd`` updates
+the MLP with SGD at the embedding optimizer's learning rate.
 
 Differences from the reference driver: timing is on the device (CUDA events), max over ranks, and
 the embedding optimizer runs fused inside the backward kernels.
@@ -34,6 +38,8 @@ def main():
   p.add_argument("--dp_input", action="store_true")
   p.add_argument("--model", default="tiny", choices=sorted(synthetic_models_v3))
   p.add_argument("--optimizer", default="sgd", choices=["sgd", "adagrad", "rowwise_adagrad", "adam"])
+  p.add_argument("--dense_optimizer", default="sgd", choices=["sgd", "adagrad", "adam"],
+                 help="optimizer of the MLP (--embedding_api de); the reference uses --optimizer's")
   p.add_argument("--column_slice_threshold", type=int, default=None)
   p.add_argument("--row_slice_threshold", type=int, default=None)
   p.add_argument("--data_parallel_threshold", type=int, default=None)
@@ -99,11 +105,13 @@ def main():
       raise ValueError(f"--trainer fast: {why}")
     if args.trainer != "autograd" and not why:
       trainer = SyntheticTrainStep(model, lr=lr, embedding_optimizer=args.optimizer,
-                                   use_cuda_graph=bool(args.cuda_graph))
+                                   use_cuda_graph=bool(args.cuda_graph),
+                                   dense_optimizer=args.dense_optimizer)
       trainer_kind = "fast"
     else:
       trainer = HybridTrainer(model, lr=lr, embedding_optimizer=args.optimizer,
-                              use_cuda_graph=bool(args.cuda_graph) and use_cuda)
+                              use_cuda_graph=bool(args.cuda_graph) and use_cuda,
+                              dense_optimizer=args.dense_optimizer)
       trainer_kind = "autograd"
     step = lambda num, cat, lab: trainer.step(num, cat, lab)
   else:
@@ -159,6 +167,8 @@ def main():
     print(json.dumps({"model": args.model, "n_gpus": world, "batch_size": args.batch_size,
                       "ms_per_iter": ms, "samples_per_sec": args.batch_size / ms * 1e3,
                       "optimizer": args.optimizer,
+                      "dense_optimizer": args.dense_optimizer if args.embedding_api == "de"
+                                         else args.optimizer,
                       "trainer": trainer_kind if args.embedding_api == "de" else "native",
                       **summary(cfg)}))
   if world > 1:

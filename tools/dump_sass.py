@@ -48,6 +48,8 @@ HOT = [
     ("head_loss_8", r"head_loss_kernel<8>"),
     ("head_eval_8", r"head_eval_kernel<8>"),
     ("sgd_update", r"sgd_update_kernel"),
+    ("dense_opt_adagrad", r"dense_opt_kernel<1>"),
+    ("dense_opt_adam", r"dense_opt_kernel<3>"),
 ]
 
 
