@@ -37,6 +37,12 @@ from ..utils.metrics import BinnedAUC, auc_from_histogram
 from .dense_optimizer import FlatDenseOptimizer, dense_optimizer_config
 from .dlrm import DLRM
 
+# Tables with at least this many rows take their SGD update from the interaction backward
+# (fused_table_update).  Chosen by tools/bench_fused_table_update.py (DESIGN §8): the fastest of
+# 2500 / 20k / 100k / 1M / 20M rows on uniform and on power-law (alpha 1.05) ids alike.  Smaller
+# tables stay in L2 and keep the scatter, which merges repeated ids within a tile.
+FUSED_UPDATE_MIN_ROWS = 20000
+
 
 def _pad8(n: int) -> int:
   return (n + 7) // 8 * 8
@@ -61,13 +67,20 @@ class DLRMTrainStep:
   ``dense_optimizer`` (``sgd`` | ``adagrad`` | ``adam``, hyperparameters in
   ``dense_optimizer_kwargs``) updates the MLPs and any replicated tables with the shared
   learning rate.  Replicated tables (``data_parallel_threshold``) need
-  ``dense_optimizer == embedding_optimizer``."""
+  ``dense_optimizer == embedding_optimizer``.
+
+  ``fused_table_update``: on one GPU with the atomic SGD embedding update, the interaction
+  backward applies the update of the tables with at least ``fused_update_min_rows`` rows
+  itself, so their gradient rows skip the receive buffer (:meth:`FusedEngine.producer_update`).
+  Other configurations run the same schedule either way; ``False`` keeps every table on the
+  staged scatter."""
 
   def __init__(self, model: DLRM, lr: float = 24.0, embedding_optimizer: str = "sgd",
                scheduler: Optional[LearningRateScheduler] = None, use_cuda_graph: bool = True,
                embedding_optimizer_kwargs: Optional[dict] = None, overlap: bool = True,
                gemm: str = "cublas", eval_thresholds: int = 8000, dense_optimizer: str = "sgd",
-               dense_optimizer_kwargs: Optional[dict] = None):
+               dense_optimizer_kwargs: Optional[dict] = None, fused_table_update: bool = True,
+               fused_update_min_rows: int = FUSED_UPDATE_MIN_ROWS):
     if gemm not in ("cublas", "fused_dgrad", "tcgen05", "tcgen05_pair"):
       raise ValueError("gemm must be cublas | fused_dgrad | tcgen05 | tcgen05_pair")
     # cublas: cuBLASLt everywhere.  fused_dgrad: forward/wgrad on cuBLASLt, dgrad on the
@@ -75,6 +88,10 @@ class DLRMTrainStep:
     # tcgen05: forward layers on the first-party kernel as well.  tcgen05_pair: same, with the
     # 2-CTA cluster kernel for layers at least 256 wide.  (The option names are historical.)
     self.gemm = gemm
+    # single GPU with the atomic SGD update: the interaction backward updates the large tables
+    # itself (see FusedEngine.producer_update); False keeps every table on the staged scatter
+    self.fused_table_update = bool(fused_table_update)
+    self.fused_update_min_rows = int(fused_update_min_rows)
     self.dense_cfg = dense_optimizer_config(dense_optimizer, dense_optimizer_kwargs)
     self.model = model
     self.emb = model.embedding
@@ -343,6 +360,7 @@ class DLRMTrainStep:
     # the kernel's epilogue stores - and its tail signals "gradient ready" to the owners
     hb = self.bottom[-1]
     pushed = eng.streamed_push
+    applied = None
     if pushed:
       # pieces of remote owners are staged locally; the copy kernel (own stream, a few blocks)
       # forwards every finished chunk over NVLink while the interaction backward keeps computing.
@@ -358,19 +376,24 @@ class DLRMTrainStep:
       with torch.cuda.stream(self._push_stream):
         eng.launch_streamed_push()
     else:
+      # single GPU, SGD: the interaction backward also applies the update of the large tables
+      # (FusedEngine.producer_update); their gradient rows never go through the receive buffer
+      applied = eng.producer_update(self.dim, self.fused_update_min_rows) \
+          if self.fused_table_update else None
       ops.interact_bwd(hb.y, eng.out, self.n_emb, self.dz, hb.dy, 0, 0, 1.0, eng.routes_all,
-                       len(eng.routes_all_np), eng.sync_grad_signal(), None, 0)
+                       len(eng.routes_all_np), eng.sync_grad_signal(), None, 0,
+                       *(applied.interact_args() if applied else ()))
     # embedding exchange + fused table update, overlapped with the bottom MLP backward
     if self._side is not None:
       self._side.wait_stream(torch.cuda.current_stream())
       if pushed:  # the update's head waits for every rank's copy kernel: ours must be done first
         self._side.wait_stream(self._push_stream)
       with torch.cuda.stream(self._side):
-        eng.backward_inplace()
+        eng.backward_inplace(applied)
     else:
       if pushed:
         torch.cuda.current_stream().wait_stream(self._push_stream)
-      eng.backward_inplace()
+      eng.backward_inplace(applied)
     ops.relu_bwd_bias(hb.dy, hb.y, hb.gb)
     for i in range(len(self.bottom) - 1, -1, -1):
       L = self.bottom[i]

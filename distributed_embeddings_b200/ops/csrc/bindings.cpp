@@ -803,7 +803,45 @@ void interact_fwd(const Tensor& bottom, const Tensor& emb, int64_t n_emb, Tensor
 void interact_bwd(const Tensor& bottom, const Tensor& emb, int64_t n_emb, const Tensor& dz,
                   Tensor dbottom, int64_t demb_ptr, int64_t demb_stride, double emb_grad_scale,
                   const c10::optional<Tensor>& routes, int64_t n_routes, at::IntArrayRef sync,
-                  const c10::optional<Tensor>& done_counters, int64_t chunk_rows) {
+                  const c10::optional<Tensor>& done_counters, int64_t chunk_rows,
+                  const c10::optional<Tensor>& apply_descs, double apply_scale,
+                  int64_t apply_scale_ptr, bool apply_ids64) {
+  // apply_descs: host uint8 tensor of n_emb InputDesc records, one per embedding row of F; a
+  // record with a null table leaves that row to the routes, any other is updated in the kernel
+  de::InteractApply apply{};
+  if (apply_descs.has_value()) {
+    const Tensor& a = *apply_descs;
+    TORCH_CHECK(!a.is_cuda() && a.scalar_type() == at::kByte && a.is_contiguous(),
+                "apply_descs must be a contiguous uint8 CPU tensor of InputDesc records");
+    TORCH_CHECK(a.numel() == n_emb * static_cast<int64_t>(sizeof(de::InputDesc)),
+                "apply_descs needs one InputDesc per embedding row");
+    TORCH_CHECK(n_emb <= de::kMaxInteractApply, "apply_descs: at most 31 embedding rows");
+    TORCH_CHECK(apply_scale_ptr % 4 == 0, "apply_scale_ptr must be 4-byte aligned");
+    TORCH_CHECK(!done_counters.has_value(), "apply_descs cannot be combined with done_counters");
+    const auto* d = reinterpret_cast<const de::InputDesc*>(a.data_ptr());
+    for (int64_t f = 0; f < n_emb; ++f) {
+      if (d[f].table == nullptr) continue;
+      TORCH_CHECK(d[f].width == 128 && bottom.size(1) == 128,
+                  "apply_descs: applied tables must be 128 wide, like the interaction");
+      TORCH_CHECK(d[f].hotness == 1 && d[f].offsets == nullptr && d[f].ids != nullptr,
+                  "apply_descs: applied inputs must be one-hot with direct ids");
+      TORCH_CHECK(reinterpret_cast<uintptr_t>(d[f].table) % 16 == 0,
+                  "apply_descs: tables must be 16-byte aligned");
+      TORCH_CHECK(reinterpret_cast<uintptr_t>(d[f].ids) % (apply_ids64 ? 8 : 4) == 0,
+                  "apply_descs: ids must be aligned to their element size");
+      TORCH_CHECK(d[f].row_base >= 0 && d[f].sub_rows >= 0,
+                  "apply_descs: row_base and sub_rows must not be negative");
+      apply.table[f] = static_cast<float*>(const_cast<void*>(d[f].table));
+      apply.ids[f] = d[f].ids;
+      apply.row_base[f] = d[f].row_base;
+      apply.sub_rows[f] = d[f].sub_rows;
+      apply.id_shift[f] = d[f].id_shift;
+      apply.mask |= 1u << f;
+    }
+    apply.scale = static_cast<float>(apply_scale);
+    apply.scale_ptr = reinterpret_cast<const float*>(apply_scale_ptr);
+    apply.ids64 = apply_ids64 ? 1 : 0;
+  }
   check_bf16_2d(bottom, "bottom");
   check_bf16_2d(emb, "emb");
   check_bf16_2d(dz, "dz");
@@ -849,7 +887,8 @@ void interact_bwd(const Tensor& bottom, const Tensor& emb, int64_t n_emb, const 
                                     done_counters.has_value()
                                         ? reinterpret_cast<uint32_t*>(done_counters->data_ptr<int>())
                                         : nullptr,
-                                    static_cast<int>(chunk_rows));
+                                    static_cast<int>(chunk_rows),
+                                    apply.mask != 0 ? &apply : nullptr);
   TORCH_CHECK(ok, "unsupported interaction shape (n_emb <= 31, dim in {32,64,128}; routed / "
                   "signalling launches need dim in {64,128} and 16-byte aligned rows)");
   check_launch();
@@ -1239,7 +1278,8 @@ TORCH_LIBRARY(de_b200, m) {
   m.def(
       "interact_bwd(Tensor bottom, Tensor emb, int n_emb, Tensor dz, Tensor(a!) dbottom, "
       "int demb_ptr, int demb_stride, float emb_grad_scale, Tensor? routes, int n_routes, "
-      "int[] sync, Tensor? done_counters, int chunk_rows) -> ()",
+      "int[] sync, Tensor? done_counters, int chunk_rows, Tensor? apply_descs=None, "
+      "float apply_scale=0.0, int apply_scale_ptr=0, bool apply_ids64=False) -> ()",
       &interact_bwd);
   m.def("avgpool_fwd(Tensor x, int n, Tensor(a!) out, int stride) -> ()", &avgpool_fwd);
   m.def("avgpool_bwd(Tensor dout, Tensor(a!) dx, int n, int stride) -> ()", &avgpool_bwd);

@@ -250,13 +250,31 @@ bool launch_interact_fwd(const void* bottom, int64_t bottom_stride, const void* 
 // The embedding gradient goes either to one local buffer (demb, routes == nullptr) or, piece by
 // piece, straight into the owners' receive buffers over NVLink (routes: columns are relative to
 // the concatenated [n_emb * dim] embedding row).
+// Tables the interaction backward updates itself (single-GPU SGD step): the gradient of embedding
+// row f of F (bf16, as the routed copy-out would store it) is widened, scaled and reduced straight
+// into table[(row_base + id) * 128 + col] when bit f of `mask` is set; the other rows go through
+// the routes.  One-hot ids of feature f: ids[f][sample] + id_shift[f], valid below sub_rows[f]
+// (others are skipped).  scale *= *scale_ptr when scale_ptr is set (the device learning rate).
+constexpr int kMaxInteractApply = 31;
+struct InteractApply {
+  float* table[kMaxInteractApply];  // fused fp32 table, 128 columns, 16-byte aligned
+  const void* ids[kMaxInteractApply];
+  int64_t row_base[kMaxInteractApply];
+  int64_t sub_rows[kMaxInteractApply];
+  int64_t id_shift[kMaxInteractApply];
+  const float* scale_ptr;
+  float scale;
+  uint32_t mask;
+  int32_t ids64;
+};
+
 bool launch_interact_bwd(const void* bottom, int64_t bottom_stride, const void* emb,
                          int64_t emb_stride, int n_emb, int dim, const void* dz,
                          int64_t dz_stride, void* dbottom, int64_t dbottom_stride, void* demb,
                          int64_t demb_stride, float emb_grad_scale, int64_t batch, int sm_count,
                          cudaStream_t stream, const GradRoute* routes, int n_routes,
                          const SyncArgs& sync, uint32_t* done_counters = nullptr,
-                         int chunk_rows = 0);
+                         int chunk_rows = 0, const InteractApply* apply = nullptr);
 // 1-D average pooling over bf16 rows ("same" padding; the synthetic models' interaction)
 void launch_avgpool_fwd(const void* x, int64_t x_stride, int n, void* out, int64_t out_stride,
                         int out_len, int stride, int left, int64_t rows, cudaStream_t stream);

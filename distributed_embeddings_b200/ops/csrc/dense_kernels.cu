@@ -293,16 +293,21 @@ struct ChunkDst {
   long long stride;
 };
 
-template <int D>
-__global__ void __launch_bounds__(kWarps * 32)
-interact_bwd_v2_kernel(const bf16* __restrict__ bottom, int64_t bottom_stride,
-                       const bf16* __restrict__ emb, int64_t emb_stride, int n_emb,
-                       const bf16* __restrict__ dz, int64_t dz_stride, bf16* __restrict__ dbottom,
-                       int64_t dbottom_stride, bf16* __restrict__ demb, int64_t demb_stride,
-                       float emb_grad_scale, int64_t batch,
-                       const GradRoute* __restrict__ routes, int n_routes,
-                       const __grid_constant__ SyncArgs sync, uint32_t* __restrict__ done_counters,
-                       int chunk_rows) {
+__device__ __forceinline__ void prefetch_l2(const void* p) {
+  asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
+}
+
+// APPLY: rows of F flagged in `apply.mask` are reduced into their table rows (SGD) instead of
+// being stored through the routes; the routed rows are unchanged.
+template <int D, bool APPLY>
+__device__ __forceinline__ void
+interact_bwd_v2_body(const bf16* __restrict__ bottom, int64_t bottom_stride,
+                     const bf16* __restrict__ emb, int64_t emb_stride, int n_emb,
+                     const bf16* __restrict__ dz, int64_t dz_stride, bf16* __restrict__ dbottom,
+                     int64_t dbottom_stride, bf16* __restrict__ demb, int64_t demb_stride,
+                     float emb_grad_scale, int64_t batch, const GradRoute* __restrict__ routes,
+                     int n_routes, const SyncArgs& sync, uint32_t* __restrict__ done_counters,
+                     int chunk_rows, const InteractApply& apply) {
   constexpr int LD = D + 8;
   constexpr int LDG = 40;
   constexpr int kWarpElems = 2 * kMaxFeat * LD + 2 * kDzMax + kMaxFeat * LDG;
@@ -339,19 +344,56 @@ interact_bwd_v2_kernel(const bf16* __restrict__ bottom, int64_t bottom_stride,
   zero_pad_rows<D>(base + kMaxFeat * LD, LD, n_emb, lane);
   __syncthreads();
 
+  // APPLY: lane f holds the table row id of feature f for the current / next sample (-1: not
+  // applied or out of range)
+  float apply_scale = 0.f;
+  long long id_cur = -1, id_next = -1;
+  if constexpr (APPLY) {
+    apply_scale = apply.scale;
+    if (apply.scale_ptr != nullptr) apply_scale *= *apply.scale_ptr;
+  }
+  auto load_id = [&](int64_t smp) -> long long {
+    if (lane < n_emb && ((apply.mask >> lane) & 1u)) {
+      const long long raw = apply.ids64 ? static_cast<const int64_t*>(apply.ids[lane])[smp]
+                                        : static_cast<const int32_t*>(apply.ids[lane])[smp];
+      const long long id = raw + apply.id_shift[lane];
+      if (static_cast<unsigned long long>(id) < static_cast<unsigned long long>(apply.sub_rows[lane]))
+        return id;
+    }
+    return -1;
+  };
+  // the row this lane's feature reduces into: have it resident in L2 when the REDs arrive
+  auto prefetch_row = [&](long long id) {
+    if (id >= 0) {
+      const char* row = reinterpret_cast<const char*>(apply.table[lane] +
+                                                      (apply.row_base[lane] + id) * D);
+#pragma unroll
+      for (int l = 0; l < D * 4 / 128; ++l) prefetch_l2(row + (l << 7));
+    }
+  };
+
   const int64_t stride = static_cast<int64_t>(gridDim.x) * kWarps;
   int64_t s = static_cast<int64_t>(blockIdx.x) * kWarps + warp;
   int cur = 0;
-  if (s < batch)
+  if (s < batch) {
     issue_sample<D>(base, LD, sDz0, bottom + s * bottom_stride, emb + s * emb_stride,
                     dz + s * dz_stride, n_emb, dz_chunks, lane);
+    if constexpr (APPLY) {
+      id_cur = load_id(s);
+      prefetch_row(id_cur);
+    }
+  }
   cp_async_commit();
   for (; s < batch; s += stride, cur ^= 1) {
     const int64_t nxt = s + stride;
-    if (nxt < batch)
+    if (nxt < batch) {
       issue_sample<D>(base + (cur ^ 1) * (kMaxFeat * LD), LD, sDz0 + (cur ^ 1) * kDzMax,
                       bottom + nxt * bottom_stride, emb + nxt * emb_stride, dz + nxt * dz_stride,
                       n_emb, dz_chunks, lane);
+      if constexpr (APPLY) id_next = load_id(nxt);  // consumed after this sample's MMAs
+    } else if constexpr (APPLY) {
+      id_next = -1;
+    }
     cp_async_commit();        // possibly empty: keeps the group arithmetic uniform
     cp_async_wait_group<1>();  // everything but the prefetch just issued has landed
     __syncwarp();
@@ -422,16 +464,50 @@ interact_bwd_v2_kernel(const bf16* __restrict__ bottom, int64_t bottom_stride,
       }
     }
     __syncwarp();
+    if constexpr (APPLY) prefetch_row(id_next);
     // coalesced 16-byte copy-out: row 0 -> bottom-MLP gradient, rows 1.. -> the chunk's owner
     // (local buffer, or a peer's receive buffer over NVLink: 128-256 contiguous bytes per piece)
     if (lane < kRowChunks)
       *reinterpret_cast<uint4*>(dbottom + s * dbottom_stride + lane * 8) =
           *reinterpret_cast<const uint4*>(sF + lane * 8);
-    for (int c = lane; c < n_chunks; c += 32) {
-      const int row = 1 + c / kRowChunks, ch = c - (row - 1) * kRowChunks;
-      const ChunkDst d = sDst[c];
-      *reinterpret_cast<uint4*>(d.base + static_cast<unsigned long long>(s * d.stride)) =
-          *reinterpret_cast<const uint4*>(sF + row * LD + ch * 8);
+    if constexpr (APPLY) {
+      // applied rows: the bf16 gradient the routed store would write, widened and scaled like
+      // the scatter's (bf16 -> fp32, * scale), reduced into the table row
+      for (int c0 = 0; c0 < n_chunks; c0 += 32) {
+        const int c = c0 + lane;
+        const int f = c / kRowChunks, ch = c - f * kRowChunks;
+        const long long id = __shfl_sync(0xffffffffu, id_cur, f & 31);
+        if (c >= n_chunks) continue;
+        const uint4 v = *reinterpret_cast<const uint4*>(sF + (f + 1) * LD + ch * 8);
+        if ((apply.mask >> f) & 1u) {
+          if (id >= 0) {
+            const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&v);
+            FVec<4> lo, hi;
+#pragma unroll
+            for (int k = 0; k < 2; ++k) {
+              const float2 a = __bfloat1622float2(h[k]), b = __bfloat1622float2(h[k + 2]);
+              lo.v[2 * k] = a.x * apply_scale;
+              lo.v[2 * k + 1] = a.y * apply_scale;
+              hi.v[2 * k] = b.x * apply_scale;
+              hi.v[2 * k + 1] = b.y * apply_scale;
+            }
+            float* dst = apply.table[f] + (apply.row_base[f] + id) * D + ch * 8;
+            red_add_f32<4>(dst, lo);
+            red_add_f32<4>(dst + 4, hi);
+          }
+        } else {
+          const ChunkDst d = sDst[c];
+          *reinterpret_cast<uint4*>(d.base + static_cast<unsigned long long>(s * d.stride)) = v;
+        }
+      }
+      id_cur = id_next;
+    } else {
+      for (int c = lane; c < n_chunks; c += 32) {
+        const int row = 1 + c / kRowChunks, ch = c - (row - 1) * kRowChunks;
+        const ChunkDst d = sDst[c];
+        *reinterpret_cast<uint4*>(d.base + static_cast<unsigned long long>(s * d.stride)) =
+            *reinterpret_cast<const uint4*>(sF + row * LD + ch * 8);
+      }
     }
     __syncwarp();  // all lanes are done with buffer `cur` before the next iteration refills it
     if (done_counters != nullptr && lane == 0) {
@@ -442,6 +518,38 @@ interact_bwd_v2_kernel(const bf16* __restrict__ bottom, int64_t bottom_stride,
   }
   cp_async_wait_group<0>();
   sync_tail(sync);  // every gradient piece of this rank is on its way to its owner
+}
+
+template <int D>
+__global__ void __launch_bounds__(kWarps * 32)
+interact_bwd_v2_kernel(const bf16* __restrict__ bottom, int64_t bottom_stride,
+                       const bf16* __restrict__ emb, int64_t emb_stride, int n_emb,
+                       const bf16* __restrict__ dz, int64_t dz_stride, bf16* __restrict__ dbottom,
+                       int64_t dbottom_stride, bf16* __restrict__ demb, int64_t demb_stride,
+                       float emb_grad_scale, int64_t batch,
+                       const GradRoute* __restrict__ routes, int n_routes,
+                       const __grid_constant__ SyncArgs sync, uint32_t* __restrict__ done_counters,
+                       int chunk_rows) {
+  interact_bwd_v2_body<D, false>(bottom, bottom_stride, emb, emb_stride, n_emb, dz, dz_stride,
+                                 dbottom, dbottom_stride, demb, demb_stride, emb_grad_scale, batch,
+                                 routes, n_routes, sync, done_counters, chunk_rows,
+                                 InteractApply{});
+}
+
+// v2 with the table update of the features in `apply` (single-GPU SGD step)
+template <int D>
+__global__ void __launch_bounds__(kWarps * 32)
+interact_bwd_apply_kernel(const bf16* __restrict__ bottom, int64_t bottom_stride,
+                          const bf16* __restrict__ emb, int64_t emb_stride, int n_emb,
+                          const bf16* __restrict__ dz, int64_t dz_stride,
+                          bf16* __restrict__ dbottom, int64_t dbottom_stride,
+                          bf16* __restrict__ demb, int64_t demb_stride, float emb_grad_scale,
+                          int64_t batch, const GradRoute* __restrict__ routes, int n_routes,
+                          const __grid_constant__ SyncArgs sync,
+                          const __grid_constant__ InteractApply apply) {
+  interact_bwd_v2_body<D, true>(bottom, bottom_stride, emb, emb_stride, n_emb, dz, dz_stride,
+                                dbottom, dbottom_stride, demb, demb_stride, emb_grad_scale, batch,
+                                routes, n_routes, sync, nullptr, 0, apply);
 }
 
 // dy <- dy * (y > 0) (in place) ; db[c] += sum_rows dy   (db fp32, pre-zeroed)
@@ -843,8 +951,11 @@ bool launch_interact_bwd(const void* bottom, int64_t bottom_stride, const void* 
                          int64_t dz_stride, void* dbottom, int64_t dbottom_stride, void* demb,
                          int64_t demb_stride, float emb_grad_scale, int64_t batch, int sm_count,
                          cudaStream_t stream, const GradRoute* routes, int n_routes,
-                         const SyncArgs& sync, uint32_t* done_counters, int chunk_rows) {
+                         const SyncArgs& sync, uint32_t* done_counters, int chunk_rows,
+                         const InteractApply* apply) {
   if (n_emb + 1 > kMaxFeat || batch <= 0 || dim % 32 != 0) return false;
+  const bool applied = apply != nullptr && apply->mask != 0;
+  if (applied && (dim != 128 || done_counters != nullptr)) return false;
   int64_t blocks = (batch + kWarps - 1) / kWarps;
   const int64_t cap = static_cast<int64_t>(sm_count) * 8;
   if (blocks > cap) blocks = cap;
@@ -862,28 +973,30 @@ bool launch_interact_bwd(const void* bottom, int64_t bottom_stride, const void* 
         reinterpret_cast<uintptr_t>(emb) | reinterpret_cast<uintptr_t>(dbottom)) & 15) == 0 &&
       (dim == 128 || dim == 64) &&
       (routes != nullptr || (demb_stride % 8 == 0 && (reinterpret_cast<uintptr_t>(demb) & 15) == 0));
-  if ((routes != nullptr || done_counters != nullptr) && !v2_ok) return false;  // v2 only
+  if ((routes != nullptr || done_counters != nullptr || applied) && !v2_ok) return false;  // v2 only
   const bool has_sync = sync.state != nullptr && (sync.wait_ch >= 0 || sync.signal_ch >= 0);
-  if (v2_ok && (!force_v1 || routes != nullptr || has_sync || done_counters != nullptr)) {
+  if (v2_ok &&
+      (!force_v1 || routes != nullptr || has_sync || done_counters != nullptr || applied)) {
     // two resident blocks per SM, each warp streams its samples through a double buffer
     int64_t blocks2 = (batch + kWarps - 1) / kWarps;
     if (blocks2 > static_cast<int64_t>(sm_count) * 2) blocks2 = static_cast<int64_t>(sm_count) * 2;
-#define DE_IBWD2(DD)                                                                             \
+#define DE_IBWD2(KERNEL, DD, ...)                                                                \
   {                                                                                              \
     const size_t smem =                                                                          \
         kWarps * (2 * kMaxFeat * (DD + 8) + 2 * kDzMax + kMaxFeat * 40) * sizeof(bf16) +         \
         static_cast<size_t>(n_emb) * (DD / 8) * sizeof(ChunkDst);                                \
-    cudaFuncSetAttribute(interact_bwd_v2_kernel<DD>,                                             \
-                         cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));   \
-    interact_bwd_v2_kernel<DD><<<static_cast<unsigned>(blocks2), kWarps * 32, smem, stream>>>(   \
+    cudaFuncSetAttribute(KERNEL<DD>, cudaFuncAttributeMaxDynamicSharedMemorySize,                \
+                         static_cast<int>(smem));                                                \
+    KERNEL<DD><<<static_cast<unsigned>(blocks2), kWarps * 32, smem, stream>>>(                   \
         reinterpret_cast<const bf16*>(bottom), bottom_stride, reinterpret_cast<const bf16*>(emb), \
         emb_stride, n_emb, reinterpret_cast<const bf16*>(dz), dz_stride,                         \
         reinterpret_cast<bf16*>(dbottom), dbottom_stride, reinterpret_cast<bf16*>(demb),         \
-        demb_stride, emb_grad_scale, batch, routes, n_routes, sync, done_counters, chunk_rows);  \
+        demb_stride, emb_grad_scale, batch, routes, n_routes, sync, __VA_ARGS__);                \
     return true;                                                                                 \
   }
-    if (dim == 128) DE_IBWD2(128)
-    if (dim == 64) DE_IBWD2(64)
+    if (applied) DE_IBWD2(interact_bwd_apply_kernel, 128, *apply)
+    if (dim == 128) DE_IBWD2(interact_bwd_v2_kernel, 128, done_counters, chunk_rows)
+    if (dim == 64) DE_IBWD2(interact_bwd_v2_kernel, 64, done_counters, chunk_rows)
 #undef DE_IBWD2
   }
   if (has_sync) return false;

@@ -440,6 +440,29 @@ class DryOps:
         per_id = (g * w.unsqueeze(1))[self._pool_index(lens)]
         table.index_add_(0, int(d["row_base"]) + ids[ok], per_id[ok])
 
+  def interact_bwd_apply(self, demb, apply_descs, scale, scale_ptr, ids64):
+    """Stand-in for the table update of ``interact_bwd`` (the interpreter has no interaction
+    kernel): takes the embedding gradient ``demb`` ``[batch, n_feat * 128]`` (bf16, as the kernel
+    rounds it) in place of the interaction's operands, followed by ``interact_bwd``'s trailing
+    ``apply_descs, apply_scale, apply_scale_ptr, apply_ids64`` (``ProducerUpdate.interact_args``).
+    Feature f's rows are widened, scaled and added into the table rows of their ids; features
+    with a null table are left to the routes and the scatter."""
+    self._count("interact_bwd_apply")
+    if scale_ptr:
+      scale = scale * float(self.world.tensor(int(scale_ptr), torch.float32, 1, "lr")[0])
+    batch = demb.shape[0]
+    for f, d in enumerate(self._descs(apply_descs, apply_descs.numel() // INPUT_DESC.itemsize)):
+      if not int(d["table"]):
+        continue
+      assert int(d["width"]) == 128 and int(d["hotness"]) == 1 and not int(d["offsets"]) and \
+          int(d["ids"]), "applied inputs are one-hot, direct ids, 128 wide"
+      table = self._table(d)
+      vals, _ = self._ids_of(d, 0, batch, ids64, [], batch)
+      ids = vals + int(d["id_shift"])
+      ok = (ids >= 0) & (ids < int(d["sub_rows"]))
+      g = demb[:, f * 128:(f + 1) * 128].float() * float(scale)
+      table.index_add_(0, int(d["row_base"]) + ids[ok], g[ok])
+
   def sort_items(self, descs, tables, n_tables, n_inputs, batch, src_batch, src_ptrs, ids64,
                  n_items, total_rows, prefill_sentinel):
     self._count("sort_items")

@@ -36,7 +36,7 @@ from __future__ import annotations
 
 import os
 import weakref
-from typing import Any, Dict, List, Optional, Sequence, Tuple
+from typing import Any, Dict, List, NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -69,6 +69,24 @@ def _dev_ptr(t: torch.Tensor) -> int:
   if not t.is_pinned():
     raise RuntimeError("host-resident tables must live in pinned memory for the fused back end")
   return int(_native.require().host_device_pointer(t))
+
+
+class ProducerUpdate(NamedTuple):
+  """The SGD table update a gradient producer applies itself (:meth:`FusedEngine.producer_update`):
+  one host InputDesc record per feature for ``ops.interact_bwd`` (null table: left to the
+  scatter), the scale and learning-rate word of the update, and the descriptors of the tables the
+  scatter still updates."""
+  mpdesc: torch.Tensor       # the plan's model-parallel descriptors it was split from
+  apply_descs: torch.Tensor
+  scale: float
+  scale_ptr: int
+  ids64: bool
+  rest_descs: Optional[torch.Tensor]
+  n_rest: int
+
+  def interact_args(self) -> tuple:
+    """The trailing ``apply_*`` arguments of ``ops.interact_bwd``."""
+    return self.apply_descs, self.scale, self.scale_ptr, self.ids64
 
 
 class _FusedFn(torch.autograd.Function):
@@ -999,22 +1017,75 @@ class FusedEngine:
     signals "gradient ready" from its tail)."""
     return self._sync(signal=CH_GRAD) if (self.W > 1 and self.mpdesc is not None) else []
 
-  def backward_inplace(self):
+  def backward_inplace(self, producer: Optional["ProducerUpdate"] = None):
     """Backward when a fused producer (e.g. the DLRM interaction backward) already pushed the
     gradient through ``routes_all`` and signalled: fused table update; replicated tables
-    accumulate their dense gradient into the targets given to :meth:`set_dp_grad_targets`."""
+    accumulate their dense gradient into the targets given to :meth:`set_dp_grad_targets`.
+    ``producer``: the :meth:`producer_update` whose tables the producer updated itself; only the
+    remaining tables are scattered."""
     if len(self.de.dp_layers):
       if getattr(self, "_dp_targets", None) is None:
         raise RuntimeError("backward_inplace needs set_dp_grad_targets() for replicated tables")
       self._scatter_dp_grads()
-    self._backward_mp()
+    self._backward_mp(producer)
 
-  def _backward_mp(self) -> List[Optional[torch.Tensor]]:
+  def _atomic_sgd(self) -> bool:
+    """The SGD update is one atomic scatter of the gradient rows into the tables."""
+    opt = self.de._fused_optimizer
+    return opt is not None and opt["kind"] == "sgd" and not opt.get("deterministic", False) and \
+        not self.has_offload and self.tab == 0
+
+  def producer_update(self, dim: int, min_rows: int) -> Optional["ProducerUpdate"]:
+    """The SGD table update a single-GPU gradient producer can apply itself.
+
+    The producer (the DLRM interaction backward) holds every sample's finished gradient row of
+    feature ``f`` in columns ``[f * dim, (f + 1) * dim)`` of ``out``.  Reducing it straight into
+    the table row saves the write of the row into the receive buffer and the scatter's read of
+    it.  Tables with fewer than ``min_rows`` rows stay with the staged scatter, which sums the
+    samples of a 32-sample tile that hit the same row before it reduces them.
+
+    Returns a :class:`ProducerUpdate` (``interact_args()`` for ``ops.interact_bwd``; pass it to
+    :meth:`backward_inplace`), or None when the step does not qualify: one rank, the atomic SGD
+    update, one-hot 128-wide inputs of a single ``dim``-wide output row each, and at least one
+    table of ``min_rows`` rows or more."""
+    if self._key is None or self.W != 1 or not self._atomic_sgd() or not self.vec4 or \
+        self.any_ragged or dim != 128 or self.mpdesc is None or \
+        not any(_weight(l).requires_grad for l in self.mp_layers):
+      return None
+    cache = getattr(self, "_producer_split", None)
+    if cache is None or cache[0] != (self._key, dim, min_rows) or cache[1] is not self.mpdesc:
+      n_feat = len(self.out_cols) - 1
+      apply = np.zeros(n_feat, dtype=INPUT_DESC)
+      taken = np.zeros(self.n_mp_inputs, dtype=bool)
+      if self.out_cols == [dim * f for f in range(n_feat + 1)] and n_feat <= 31:
+        for i, d in enumerate(self.cdesc_np):
+          f, off = divmod(int(d["dst_col"]), dim)
+          if off == 0 and int(d["width"]) == dim and int(d["hotness"]) == 1 and \
+              int(d["offsets"]) == 0 and int(d["ids"]) != 0 and int(d["sub_rows"]) >= min_rows:
+            apply[f] = d
+            taken[i] = True
+      rest = self.mpdesc_np[~taken]
+      rest_dev = _native.upload_struct_array(rest, self.device) if len(rest) else None
+      apply_t = torch.from_numpy(apply.view(np.uint8).copy()) if taken.any() else None
+      self._producer_split = ((self._key, dim, min_rows), self.mpdesc, apply_t, rest_dev, len(rest))
+    _, mpdesc, apply_t, rest_dev, n_rest = self._producer_split
+    if apply_t is None:
+      return None
+    gscale = 0.0 if self._dry_updates else self.de.mp_grad_scale
+    return ProducerUpdate(mpdesc, apply_t, -gscale, self.lr_t.data_ptr(), self.ids64, rest_dev,
+                          n_rest)
+
+  def _backward_mp(self, producer: Optional["ProducerUpdate"] = None
+                   ) -> List[Optional[torch.Tensor]]:
     with nvtx.range("emb_backward_update"):
-      return self._backward_mp_impl()
+      return self._backward_mp_impl(producer)
 
-  def _backward_mp_impl(self) -> List[Optional[torch.Tensor]]:
+  def _backward_mp_impl(self, producer: Optional["ProducerUpdate"] = None
+                        ) -> List[Optional[torch.Tensor]]:
     ops, de = self.ops, self.de
+    if producer is not None and (producer.mpdesc is not self.mpdesc or not self._atomic_sgd()):
+      raise ValueError("the producer update was built for another plan or optimizer: call "
+                       "producer_update() for the current one")
     n_mp = len(self.mp_layers)
     if self.mpdesc is None:
       return [None] * n_mp
@@ -1034,10 +1105,14 @@ class FusedEngine:
     # exactly one writer per step and is stochastically rounded once.  An atomic 16-bit add would
     # round to nearest on every duplicate id (dropping sub-half-ulp updates) and its result
     # would depend on the order of the adds.
-    if opt is not None and opt["kind"] == "sgd" and not opt.get("deterministic", False) and \
-        not self.has_offload and self.tab == 0:
+    if self._atomic_sgd():
+      descs, n = self.mpdesc, self.n_mp_inputs
+      if producer is not None:  # the producer updated the large tables itself
+        descs, n = producer.rest_descs, producer.n_rest
+        if n == 0:
+          return [None] * n_mp
       # head: every requester's gradient rows have landed; tail: ids + gradients are consumed
-      ops.scatter_add_bwd(self.mpdesc, self.n_mp_inputs, B, B, B, self.recv_width, [],
+      ops.scatter_add_bwd(descs, n, B, B, B, self.recv_width, [],
                           self.recv_ptr, 0, -gscale, self.lr_t.data_ptr(), self.ids64,
                           self.act, self.vec4, self.vec8,
                           self._sync(wait=CH_GRAD, signal=CH_CONSUMED), self.staged_update)

@@ -30,6 +30,7 @@ HOT = [
     ("rowslice_reduce_bf16", r"rowslice_reduce_kernel<__nv_bfloat16>"),
     ("interact_fwd_128", r"interact_fwd_kernel<128>"),
     ("interact_bwd_v2_128", r"interact_bwd_v2_kernel<128>"),
+    ("interact_bwd_apply_128", r"interact_bwd_apply_kernel<128>"),
     ("allreduce_p2p_f32", r"allreduce_p2p_kernel<(false|0)>"),
     ("allreduce_multimem_f32", r"allreduce_multimem_kernel<(false|0)>"),
     ("segment_update_bf16_v4", r"segment_update_kernel<__nv_bfloat16, 4>"),
