@@ -17,6 +17,12 @@ math as one static schedule over preallocated buffers:
 * embedding forward/backward: the fused P2P engine (``parallel/fused.py``);
 * the whole step is captured in a CUDA graph and replayed (launch bound otherwise).
 
+DLRM-DCNv2 (``DLRM(interaction="dcnv2")``) swaps the dot interaction for the low-rank cross
+network: the lookups write straight into the columns of ``x0`` (``FusedEngine.set_out_row_stride``),
+each cross layer is two cuBLASLt GEMMs and the memory-bound ``cross_fwd`` kernel forward, and
+``cross_bwd`` + four GEMMs backward; ``cross_dx0`` gathers the gradient of ``x0``, whose embedding
+columns ``push_grad`` routes to the table owners (see :class:`DLRMTrainStep`).
+
 Same model/optimizer as the reference example (examples/dlrm/main.py:76-209): SGD, shared lr.
 ``dense_optimizer`` swaps the fused dense SGD for fused Adagrad or Adam (see ``dense_optimizer``).
 """
@@ -58,7 +64,7 @@ class _Layer:
     self.in_pad = _pad8(self.in_f)
     self.w_off = self.b_off = 0
     self.w_numel = self.out_f * self.in_pad
-    self.b_numel = _pad8(self.out_f)
+    self.b_numel = _pad8(self.out_f) if lin.bias is not None else 0  # bias-free: no slot
 
 
 class DLRMTrainStep:
@@ -73,7 +79,20 @@ class DLRMTrainStep:
   backward applies the update of the tables with at least ``fused_update_min_rows`` rows
   itself, so their gradient rows skip the receive buffer (:meth:`FusedEngine.producer_update`).
   Other configurations run the same schedule either way; ``False`` keeps every table on the
-  staged scatter."""
+  staged scatter.
+
+  DLRM-DCNv2 (``model.interaction == "dcnv2"``, cuBLASLt GEMMs only): the engine writes the
+  pooled (``sum``, ``model.multi_hot_sizes``) embeddings into the first ``26 * 128`` columns of
+  ``x0 = [emb_0 | ... | emb_25 | bottom]`` (``engine.out_full``) and the bottom-MLP output is
+  copied into its last 128.  Per cross layer ``l``, forward: ``u = x_l V^T``,
+  ``s = u W^T + b`` (cuBLASLt, bias epilogue), ``x_{l+1} = cross_fwd(x0, s, x_l)``; backward,
+  in reverse: ``g = cross_bwd(dy, x0)`` (also the bias gradient), ``gW = g^T u``, ``du = g W``,
+  ``gV = du^T x_l``, ``dx_l = dy + du V``; then ``cross_dx0`` sums the gradient of ``x0``, its
+  embedding columns go to the table owners through ``push_grad`` and its bottom columns into the
+  bottom-MLP backward.  The cross parameters live in the flat buffers between the bottom and the
+  top MLP.  ``fused_table_update`` does not apply: every table takes the engine's scatter /
+  sorted update.  Multi-hot inputs need the ``dcnv2`` model; multi-hot row-sliced tables are
+  not supported."""
 
   def __init__(self, model: DLRM, lr: float = 24.0, embedding_optimizer: str = "sgd",
                scheduler: Optional[LearningRateScheduler] = None, use_cuda_graph: bool = True,
@@ -88,6 +107,12 @@ class DLRMTrainStep:
     # tcgen05: forward layers on the first-party kernel as well.  tcgen05_pair: same, with the
     # 2-CTA cluster kernel for layers at least 256 wide.  (The option names are historical.)
     self.gemm = gemm
+    self.dcn = getattr(model, "interaction", "dot") == "dcnv2"
+    hots = getattr(model, "multi_hot_sizes", None)
+    if self.dcn and gemm != "cublas":
+      raise ValueError("the dcnv2 interaction runs its GEMMs on cuBLASLt: use gemm='cublas'")
+    if not self.dcn and hots is not None and any(h != 1 for h in hots):
+      raise ValueError("multi-hot features need the dcnv2 interaction in DLRMTrainStep")
     # single GPU with the atomic SGD update: the interaction backward updates the large tables
     # itself (see FusedEngine.producer_update); False keeps every table on the staged scatter
     self.fused_table_update = bool(fused_table_update)
@@ -110,6 +135,14 @@ class DLRMTrainStep:
     self.engine: FusedEngine = self.emb._engine
     self.n_emb = len(model.table_sizes)
     self.dim = model.embedding_dim
+    self.hots = list(hots) if hots is not None else [1] * self.n_emb
+    if self.dcn:
+      st = self.emb.strategy
+      if self.emb.dp_input and any(self.hots[i] != 1 for i in st.input_groups[2]):
+        raise NotImplementedError("the dcnv2 step does not support multi-hot row-sliced inputs")
+      if self.dim % 8 or any(l.V.out_features % 8 for l in model.cross_layers):
+        raise ValueError("the dcnv2 step needs an embedding width and a cross rank that are "
+                         "multiples of 8")
     # gradient all-to-all through local staging + a streaming copy kernel next to the interaction
     # backward (DE_B200_STREAM_PUSH=0: the interaction backward stores into peer memory itself)
     # on from 4 GPUs: at 2 GPUs the copy kernel competes with an interaction backward that keeps
@@ -126,7 +159,11 @@ class DLRMTrainStep:
     self.head = _Layer(lins_t[-1], False)
     if self.head.out_f != 1:
       raise ValueError("the top MLP must end in a single logit")
-    layers = self.bottom + self.top + [self.head]
+    # cross layers (V, W) of the dcnv2 model; after the bottom MLP in the flat buffers, so that
+    # they stay out of the top-MLP bucket that is all-reduced early
+    self.cross = [(_Layer(c.V, False), _Layer(c.W, False)) for c in model.cross_layers] \
+        if self.dcn else []
+    layers = self.bottom + [L for pair in self.cross for L in pair] + self.top + [self.head]
     # replicated (data-parallel) embedding tables live in the flat dense buffers too: their
     # local-batch gradient is scattered into the gradient bucket, all-reduced with the MLP
     # gradients and applied densely by the fused dense optimizer kernel (the reference's
@@ -181,9 +218,10 @@ class DLRMTrainStep:
         wv = self.p32[L.w_off:L.w_off + L.w_numel].view(L.out_f, L.in_pad)
         wv[:, :L.in_f].copy_(L.lin.weight)
         L.lin.weight.data = wv[:, :L.in_f]
-        bv = self.p32[L.b_off:L.b_off + L.out_f]
-        bv.copy_(L.lin.bias)
-        L.lin.bias.data = bv
+        if L.lin.bias is not None:
+          bv = self.p32[L.b_off:L.b_off + L.out_f]
+          bv.copy_(L.lin.bias)
+          L.lin.bias.data = bv
         L.w16 = self.p16[L.w_off:L.w_off + L.w_numel].view(L.out_f, L.in_pad)
         L.b16 = self.p16[L.b_off:L.b_off + L.out_f]
         L.gw = self.g32[L.w_off:L.w_off + L.w_numel].view(L.out_f, L.in_pad)
@@ -263,20 +301,24 @@ class DLRMTrainStep:
   # ------------------------------------------------------------------ buffers
   def _alloc(self, b: int):
     dev, bf = self.dev, torch.bfloat16
-    if self._stream_push:
-      # chunks of >= 1024 samples, at most 16 of them: the last chunk's transfer is the only part
-      # of the exchange that does not overlap the interaction backward
-      self.engine.enable_streamed_push(max(1024, -(-b // 16)))
-    self.engine.prepare(b, [1] * self.n_emb, ids64=False)
-    self.cat_stage = self.engine.in_flat[:self.n_emb * b].view(self.n_emb, b)
+    if self.dcn:
+      self._alloc_dcn(b)
+    else:
+      if self._stream_push:
+        # chunks of >= 1024 samples, at most 16 of them: the last chunk's transfer is the only
+        # part of the exchange that does not overlap the interaction backward
+        self.engine.enable_streamed_push(max(1024, -(-b // 16)))
+      self.engine.prepare(b, [1] * self.n_emb, ids64=False)
+      self.cat_stage = self.engine.in_flat[:self.n_emb * b].view(self.n_emb, b)
     self.num_in = torch.zeros(b, self.bottom[0].in_f, dtype=torch.float32, device=dev)
     self.lab_in = torch.zeros(b, dtype=torch.float32, device=dev)
     self.x0 = torch.zeros(b, self.bottom[0].in_pad, dtype=bf, device=dev)
     for L in self.bottom + self.top:
       L.y = torch.empty(b, L.out_f, dtype=bf, device=dev)
       L.dy = torch.empty(b, L.out_f, dtype=bf, device=dev)
-    self.z = torch.zeros(b, self.top[0].in_pad, dtype=bf, device=dev)
-    self.dz = torch.empty(b, self.top[0].in_pad, dtype=bf, device=dev)
+    if not self.dcn:
+      self.z = torch.zeros(b, self.top[0].in_pad, dtype=bf, device=dev)
+      self.dz = torch.empty(b, self.top[0].in_pad, dtype=bf, device=dev)
     self._batch = b
     self._graph = None
     self._eval_graph = None
@@ -292,6 +334,27 @@ class DLRMTrainStep:
     self._prefetched = 0   # batches handed to prefetch()
     self._consumed_n = 0   # batches run
     self._use_stage = False
+
+  def _alloc_dcn(self, b: int):
+    """Buffers of the cross network: x0 is the engine's output matrix; x_1..x_L, s_l and u_l are
+    kept for the backward; dX[l] is the gradient of x_l (dX[0]: the chain part of dx0)."""
+    dev, bf = self.dev, torch.bfloat16
+    eng = self.engine
+    D = self.model.cross_dim
+    eng.set_out_row_stride(D)
+    eng.prepare(b, self.hots, ids64=False)
+    if eng.out_needs_reduce:
+      raise NotImplementedError("the dcnv2 step does not support multi-hot row-sliced inputs")
+    # ids, feature-major and sample-major within a feature: [sum_f h_f * b] (see prefetch())
+    self.cat_stage = eng.in_flat[:sum(self.hots) * b]
+    self.emb_cols = eng.total_width
+    L = len(self.cross)
+    self.xs = [eng.out_full] + [torch.empty(b, D, dtype=bf, device=dev) for _ in range(L)]
+    self.ss = [torch.empty(b, D, dtype=bf, device=dev) for _ in range(L)]
+    self.us = [torch.empty(b, V.out_f, dtype=bf, device=dev) for V, _ in self.cross]
+    self.dX = [torch.empty(b, D, dtype=bf, device=dev) for _ in range(L + 1)]
+    self.g = torch.empty(b, D, dtype=bf, device=dev)  # cross_bwd output; dx0 at the end
+    self.du = torch.empty(b, max(V.out_f for V, _ in self.cross), dtype=bf, device=dev)
 
   # ------------------------------------------------------------------ the step
   def _select_stage(self):
@@ -327,6 +390,85 @@ class DLRMTrainStep:
     for L in self.top:
       x = self._linear_fwd(L, x)
 
+  def _forward_dcn(self):
+    """Forward of the dcnv2 model up to the top MLP output."""
+    ops, eng = self.ops, self.engine
+    # lookups (into x0's embedding columns) on the side stream under the bottom MLP
+    if self._side is not None:
+      self._side.wait_stream(torch.cuda.current_stream())
+      with torch.cuda.stream(self._side):
+        eng.launch_forward()
+    ops.cast_pad(self.num_in, self.x0)
+    x = self.x0
+    for L in self.bottom:
+      x = self._linear_fwd(L, x)
+    x0 = self.xs[0]
+    ops.copy_cast_2d(x, x0.data_ptr() + self.emb_cols * x0.element_size(), x0.stride(0), 1, 1.0)
+    if self._side is not None:
+      torch.cuda.current_stream().wait_stream(self._side)
+    else:
+      eng.launch_forward()
+    eng.wait_output()
+    x = x0
+    for l, (V, W) in enumerate(self.cross):
+      u, s_ = self.us[l], self.ss[l]
+      torch.mm(x, V.w16.t(), out=u)
+      torch.addmm(W.b16, u, W.w16.t(), out=s_)
+      ops.cross_fwd(x0, s_, x, self.xs[l + 1])
+      x = self.xs[l + 1]
+    for L in self.top:
+      x = self._linear_fwd(L, x)
+
+  def _backward_dcn(self):
+    ops, eng = self.ops, self.engine
+    b = self._batch
+    last = self.top[-1]
+    self.loss.zero_()
+    H = self.head
+    ops.head_loss(last.y, H.w16.view(-1), H.b16, self.lab_in, 1.0 / b, last.dy,
+                  H.gw.view(-1), H.gb, last.gb, self.loss, None)
+    nL = len(self.cross)
+    for i in range(len(self.top) - 1, -1, -1):
+      L = self.top[i]
+      x = self.top[i - 1].y if i > 0 else self.xs[nL]
+      self._wgrad(L, x)
+      if i > 0:
+        self._dgrad_relu(L, x, self.top[i - 1].dy, self.top[i - 1].gb)
+      else:  # x_L is no ReLU output: plain dgrad
+        torch.mm(L.dy, L.w16, out=self.dX[nL])
+    self._allreduce_top_early()
+    # cross layers in reverse; their weight gradients stay on this stream (g and du are reused)
+    x0 = self.xs[0]
+    for l in range(nL - 1, -1, -1):
+      V, W = self.cross[l]
+      dy = self.dX[l + 1]
+      du = self.du[:, :V.out_f]
+      ops.cross_bwd(dy, x0, self.g, W.gb)
+      torch.mm(self.g.t(), self.us[l], out_dtype=torch.float32, out=W.gw)
+      torch.mm(self.g, W.w16, out=du)
+      torch.mm(du.t(), self.xs[l], out_dtype=torch.float32, out=V.gw)
+      torch.addmm(dy, du, V.w16, out=self.dX[l])
+    # dx0 (into g): embedding columns to the table owners, bottom columns to the bottom MLP
+    hb = self.bottom[-1]
+    ops.cross_dx0(self.dX[0], self.dX[1:], self.ss, self.g, hb.dy)
+    if eng.routes_all is not None:
+      ops.push_grad(eng.routes_all, len(eng.routes_all_np), self.g[:, :self.emb_cols], eng.act,
+                    1.0, eng.sync_grad_signal())
+    self._backward_tail(None, False)
+
+  def _allreduce_top_early(self):
+    """Top-MLP + head bucket on the all-reduce stream (when enabled), under the rest of the
+    backward."""
+    if self._ar_stream is not None:
+      ar = self._ar_stream
+      ar.wait_stream(torch.cuda.current_stream())
+      if getattr(self, "_w_used", False):
+        ar.wait_stream(self._wstream)
+      off = self.top[0].w_off  # flat layout: bottom layers | cross layers | top layers | head
+      with torch.cuda.stream(ar):
+        self.ctx.allreduce_(self.gsym, self.n_flat - off, torch.float32, scale=1.0 / self.world,
+                            byte_offset=off * 4, max_blocks=32)
+
   def _backward(self):
     ops, eng = self.ops, self.engine
     b = self._batch
@@ -346,15 +488,7 @@ class DLRMTrainStep:
         self._dgrad_relu(L, x, dx, self.top[i - 1].gb)
       else:
         torch.mm(L.dy, L.w16, out=dx)
-    if self._ar_stream is not None:
-      ar = self._ar_stream
-      ar.wait_stream(torch.cuda.current_stream())
-      if getattr(self, "_w_used", False):
-        ar.wait_stream(self._wstream)
-      off = self.top[0].w_off  # flat layout: bottom layers | top layers | head
-      with torch.cuda.stream(ar):
-        self.ctx.allreduce_(self.gsym, self.n_flat - off, torch.float32, scale=1.0 / self.world,
-                            byte_offset=off * 4, max_blocks=32)
+    self._allreduce_top_early()
     # interaction backward: every piece of the embedding gradient is stored straight into the
     # receive buffer of the rank that owns the table (slice) - the gradient all-to-all rides on
     # the kernel's epilogue stores - and its tail signals "gradient ready" to the owners
@@ -383,6 +517,12 @@ class DLRMTrainStep:
       ops.interact_bwd(hb.y, eng.out, self.n_emb, self.dz, hb.dy, 0, 0, 1.0, eng.routes_all,
                        len(eng.routes_all_np), eng.sync_grad_signal(), None, 0,
                        *(applied.interact_args() if applied else ()))
+    self._backward_tail(applied, pushed)
+
+  def _backward_tail(self, applied, pushed: bool):
+    """Embedding update (side stream) under the bottom-MLP backward, all-reduce, optimizer."""
+    ops, eng = self.ops, self.engine
+    hb = self.bottom[-1]
     # embedding exchange + fused table update, overlapped with the bottom MLP backward
     if self._side is not None:
       self._side.wait_stream(torch.cuda.current_stream())
@@ -427,9 +567,9 @@ class DLRMTrainStep:
     with nvtx.range("dlrm_forward"):
       if self._use_stage:
         self._select_stage()
-      self._forward()
+      self._forward_dcn() if self.dcn else self._forward()
     with nvtx.range("dlrm_backward_update"):
-      self._backward()
+      self._backward_dcn() if self.dcn else self._backward()
 
   def set_lr(self, lr: float):
     self.lr = float(lr)
@@ -439,7 +579,9 @@ class DLRMTrainStep:
 
   def load_batch(self, numerical, categorical, labels):
     """Copy one batch into the static input buffers (host pinned or device tensors).
-    ``categorical``: ``[n_features, batch]`` tensor (feature major) or list of ``[batch]``.
+    ``categorical``: ``[n_features, batch]`` tensor (feature major) or list of ``[batch]``; for
+    the dcnv2 model a list of ``[batch, h_f]`` (or ``[batch]`` for h_f = 1) tensors, or the flat
+    layout of :meth:`prefetch`.
     :meth:`evaluate` / :meth:`predict` overwrite these buffers: do not evaluate between this
     call and the :meth:`run` that consumes the batch."""
     b = int(numerical.shape[0])
@@ -450,13 +592,20 @@ class DLRMTrainStep:
     if isinstance(categorical, (list, tuple)):
       for v, c in zip(self.engine.in_views, categorical):
         v.copy_(c.reshape(v.shape), non_blocking=True)
+    elif self.dcn:
+      self.cat_stage.copy_(categorical.reshape(-1), non_blocking=True)
     else:
       self.cat_stage.copy_(categorical, non_blocking=True)
 
   def prefetch(self, numerical, categorical, labels):
     """Asynchronous input pipeline: enqueue the H2D copy of the *next* batch (pinned host
     tensors; ``categorical`` as ``[n_features, batch]`` int32) on the copy stream while the
-    current step runs.  Consume with :meth:`run_prefetched` in the same order."""
+    current step runs.  Consume with :meth:`run_prefetched` in the same order.
+
+    dcnv2 model: ``categorical`` is the engine's packed id layout, one int32 tensor of
+    ``sum_f h_f * batch`` ids: feature-major, and within a feature sample-major (the ``h_f`` ids
+    of sample 0, then those of sample 1, ...), i.e. ``torch.cat([c.reshape(-1) for c in ids])``
+    of the ``[batch, h_f]`` tensors :meth:`step` takes."""
     b = int(numerical.shape[0])
     if b != self._batch:
       self._alloc(b)
@@ -470,7 +619,7 @@ class DLRMTrainStep:
       cs.wait_event(self._consumed[slot])  # the step that used this slot has been enqueued & done
     with torch.cuda.stream(cs):
       st = self._stage[slot]
-      st[0].copy_(categorical, non_blocking=True)
+      st[0].copy_(categorical.reshape(-1) if self.dcn else categorical, non_blocking=True)
       st[1].copy_(numerical, non_blocking=True)
       st[2].copy_(labels.reshape(-1), non_blocking=True)
       self._h2d_done[slot].record(cs)
@@ -548,7 +697,7 @@ class DLRMTrainStep:
   # counts stay equal on all ranks and the next training step's id push waits as before.
   def _eval_impl(self):
     with nvtx.range("dlrm_eval"):
-      self._forward()
+      self._forward_dcn() if self.dcn else self._forward()
       H = self.head
       self.ops.head_eval(self.top[-1].y, H.w16.view(-1), H.b16, self.lab_in, self._n_valid,
                          self._probs, self.eval_auc.hist, self._eval_loss, self._eval_count)
@@ -583,19 +732,28 @@ class DLRMTrainStep:
     self._eval_ready()
     b = self._batch
     lab = labels.reshape(-1) if labels is not None else None
-    if isinstance(categorical, (list, tuple)):
+    if self.dcn:
+      cats = None
+    elif isinstance(categorical, (list, tuple)):
       cats = [c.reshape(-1) for c in categorical]
     else:
       cats = None
     for s in range(0, n, b):
       m = min(b, n - s)
       self.num_in[:m].copy_(numerical[s:s + m], non_blocking=True)
-      if cats is None:
+      if self.dcn:
+        for v, c in zip(self.engine.in_views, categorical):
+          v[:m].copy_(c[s:s + m].reshape(m, -1), non_blocking=True)
+          if m < b:
+            v[m:].zero_()
+        if m < b:
+          self.num_in[m:].zero_()
+      elif cats is None:
         self.cat_stage[:, :m].copy_(categorical[:, s:s + m], non_blocking=True)
       else:
         for f, c in enumerate(cats):
           self.cat_stage[f, :m].copy_(c[s:s + m], non_blocking=True)
-      if m < b:
+      if m < b and not self.dcn:
         self.num_in[m:].zero_()
         self.cat_stage[:, m:].zero_()
       if lab is not None:
@@ -610,8 +768,9 @@ class DLRMTrainStep:
 
   def evaluate(self, numerical, categorical, labels):
     """Accumulate the evaluation metrics (binned ROC AUC, log loss) over ``n >= 1`` local
-    samples: ``numerical [n, 13]``, ``categorical`` ``[n_features, n]`` or a list of ``[n]``,
-    ``labels [n]``.  Nothing is copied to the host; read the result with :meth:`eval_metrics`."""
+    samples: ``numerical [n, 13]``, ``categorical`` ``[n_features, n]`` or a list of ``[n]``
+    (dcnv2 model: a list of ``[n, h_f]``), ``labels [n]``.  Nothing is copied to the host; read
+    the result with :meth:`eval_metrics`."""
     self._eval_chunks(numerical, categorical, labels)
 
   def predict(self, numerical, categorical) -> torch.Tensor:

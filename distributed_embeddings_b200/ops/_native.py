@@ -100,7 +100,7 @@ _KERNELS_PER_OP = {
     "embedding_lookup_fwd": 1, "embedding_scatter_add": 1, "embedding_lookup_grad": 14,
     "row_to_split": 1, "hash_init": 1, "integer_lookup": 1, "barrier": 1, "allreduce": 1,
     "gather_segments": 1, "gather_ragged": 1, "copy_cast_2d": 1, "dense_sgd": 1, "interact_fwd": 1, "interact_bwd": 1,
-    "dense_adagrad": 1, "dense_adam": 1,
+    "dense_adagrad": 1, "dense_adam": 1, "cross_fwd": 1, "cross_bwd": 1, "cross_dx0": 1,
     "relu_bwd_bias": 1, "head_loss": 1, "head_eval": 1, "select_copy": 1, "cast_pad": 1, "gemm_tn_bias_act": 1, "gemm_dgrad_relu_bias": 1,
 }
 _launches = 0

@@ -937,6 +937,77 @@ void relu_bwd_bias(Tensor dy, const Tensor& y, Tensor db) {
   check_launch();
 }
 
+// Host checks of the cross-network ops: a contiguous 2-D bf16 tensor on the device of `ref`,
+// 16-byte aligned, with `cols` columns (a multiple of 8) and the rows of `ref`.  Messages carry
+// strings only.
+void check_cross(const Tensor& t, const Tensor& ref, int64_t cols, const char* name) {
+  TORCH_CHECK(t.is_cuda() && t.device() == ref.device(), name, " must be on the device of x0");
+  TORCH_CHECK(t.dim() == 2 && t.scalar_type() == at::kBFloat16, name, " must be a 2-D bf16 tensor");
+  TORCH_CHECK(t.is_contiguous(), name, " must be contiguous");
+  TORCH_CHECK(t.size(0) == ref.size(0) && t.size(1) == cols, name, " has the wrong shape");
+  TORCH_CHECK(cols % 8 == 0 && cols > 0, name, " must have a positive multiple of 8 columns");
+  TORCH_CHECK((reinterpret_cast<uintptr_t>(t.data_ptr()) & 15) == 0, name,
+              " must be 16-byte aligned");
+}
+
+// out = x0 * s + xl
+void cross_fwd(const Tensor& x0, const Tensor& s, const Tensor& xl, Tensor out) {
+  TORCH_CHECK(x0.dim() == 2, "x0 must be a 2-D bf16 tensor");
+  const int64_t d = x0.size(1);
+  check_cross(x0, x0, d, "x0");
+  check_cross(s, x0, d, "s");
+  check_cross(xl, x0, d, "xl");
+  check_cross(out, x0, d, "out");
+  c10::cuda::CUDAGuard guard(x0.device());
+  de::launch_cross_fwd(x0.data_ptr(), s.data_ptr(), xl.data_ptr(), out.data_ptr(), x0.numel(),
+                       sm_count(), cur_stream());
+  check_launch();
+}
+
+// g = dy * x0 ; db += column sums of dy * x0 (fp32)
+void cross_bwd(const Tensor& dy, const Tensor& x0, Tensor g, Tensor db) {
+  TORCH_CHECK(x0.dim() == 2, "x0 must be a 2-D bf16 tensor");
+  const int64_t d = x0.size(1);
+  check_cross(x0, x0, d, "x0");
+  check_cross(dy, x0, d, "dy");
+  check_cross(g, x0, d, "g");
+  TORCH_CHECK(db.device() == x0.device() && db.scalar_type() == at::kFloat && db.is_contiguous(),
+              "db must be a contiguous fp32 tensor on the device of x0");
+  TORCH_CHECK(db.numel() == d, "db must hold one element per column");
+  c10::cuda::CUDAGuard guard(x0.device());
+  de::launch_cross_bwd(dy.data_ptr(), x0.data_ptr(), g.data_ptr(), db.data_ptr<float>(),
+                       x0.size(0), static_cast<int>(d), cur_stream());
+  check_launch();
+}
+
+// d_chain + sum_l dy[l] * s[l]: the first D - B columns into dx0, the last B into d_bottom [rows, B]
+void cross_dx0(const Tensor& d_chain, at::TensorList dy, at::TensorList s, Tensor dx0,
+               Tensor d_bottom) {
+  TORCH_CHECK(d_chain.dim() == 2, "d_chain must be a 2-D bf16 tensor");
+  const int64_t d = d_chain.size(1);
+  check_cross(d_chain, d_chain, d, "d_chain");
+  check_cross(dx0, d_chain, d, "dx0");
+  TORCH_CHECK(dy.size() == s.size(), "dy and s must have the same length");
+  TORCH_CHECK(!dy.empty() && dy.size() <= static_cast<size_t>(de::kMaxCrossLayers),
+              "cross_dx0 takes 1 to 8 layers");
+  TORCH_CHECK(d_bottom.dim() == 2 && d_bottom.size(1) <= d,
+              "d_bottom must be 2-D with at most the columns of d_chain");
+  check_cross(d_bottom, d_chain, d_bottom.size(1), "d_bottom");
+  de::CrossTerms terms{};
+  for (size_t l = 0; l < dy.size(); ++l) {
+    check_cross(dy[l], d_chain, d, "dy");
+    check_cross(s[l], d_chain, d, "s");
+    terms.dy[l] = dy[l].data_ptr();
+    terms.s[l] = s[l].data_ptr();
+  }
+  terms.n = static_cast<int>(dy.size());
+  c10::cuda::CUDAGuard guard(d_chain.device());
+  de::launch_cross_dx0(d_chain.data_ptr(), terms, dx0.data_ptr(), d_bottom.data_ptr(),
+                       d_chain.size(0), static_cast<int>(d),
+                       static_cast<int>(d - d_bottom.size(1)), cur_stream());
+  check_launch();
+}
+
 void head_loss(const Tensor& x, const Tensor& w, const Tensor& bias, const Tensor& labels,
                double inv_batch, Tensor dx, Tensor dw, Tensor db, Tensor dbias_prev,
                Tensor loss_sum, const c10::optional<Tensor>& logits) {
@@ -1284,6 +1355,12 @@ TORCH_LIBRARY(de_b200, m) {
   m.def("avgpool_fwd(Tensor x, int n, Tensor(a!) out, int stride) -> ()", &avgpool_fwd);
   m.def("avgpool_bwd(Tensor dout, Tensor(a!) dx, int n, int stride) -> ()", &avgpool_bwd);
   m.def("relu_bwd_bias(Tensor(a!) dy, Tensor y, Tensor(b!) db) -> ()", &relu_bwd_bias);
+  m.def("cross_fwd(Tensor x0, Tensor s, Tensor xl, Tensor(a!) out) -> ()", &cross_fwd);
+  m.def("cross_bwd(Tensor dy, Tensor x0, Tensor(a!) g, Tensor(b!) db) -> ()", &cross_bwd);
+  m.def(
+      "cross_dx0(Tensor d_chain, Tensor[] dy, Tensor[] s, Tensor(a!) dx0, Tensor(b!) d_bottom) "
+      "-> ()",
+      &cross_dx0);
   m.def(
       "head_loss(Tensor x, Tensor w, Tensor bias, Tensor labels, float inv_batch, Tensor(a!) dx, "
       "Tensor(b!) dw, Tensor(c!) db, Tensor(d!) dbias_prev, Tensor(e!) loss_sum, Tensor? logits) "

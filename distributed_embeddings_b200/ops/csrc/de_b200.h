@@ -283,6 +283,22 @@ void launch_avgpool_bwd(const void* dout, int64_t dout_stride, int out_len, void
                         cudaStream_t stream);
 void launch_relu_bwd_bias(void* dy, const void* y, float* db, int64_t rows, int cols,
                           cudaStream_t stream);
+// Low-rank cross network (DLRM-DCNv2), [rows, cols] bf16 row-major, cols a multiple of 8, 16-byte
+// aligned.  cross_fwd: out = x0 * s + xl over n elements.  cross_bwd: g = dy * x0,
+// db[c] += sum_rows dy * x0 (fp32).  cross_dx0: d_chain + sum_l dy_l * s_l, columns below
+// emb_cols into dx0, the rest into d_bottom [rows, cols - emb_cols].
+constexpr int kMaxCrossLayers = 8;
+struct CrossTerms {
+  const void* dy[kMaxCrossLayers];
+  const void* s[kMaxCrossLayers];
+  int n;
+};
+void launch_cross_fwd(const void* x0, const void* s, const void* xl, void* out, int64_t n,
+                      int sm_count, cudaStream_t stream);
+void launch_cross_bwd(const void* dy, const void* x0, void* g, float* db, int64_t rows, int cols,
+                      cudaStream_t stream);
+void launch_cross_dx0(const void* d_chain, const CrossTerms& terms, void* dx0, void* d_bottom,
+                      int64_t rows, int cols, int emb_cols, cudaStream_t stream);
 bool launch_head_loss(const void* x, int K, const void* w, const void* bias, const float* labels,
                       int64_t batch, float inv_batch, void* dx, float* dw, float* db,
                       float* dbias_prev, float* loss_sum, float* logits_out, int sm_count,

@@ -609,6 +609,137 @@ relu_bwd_bias_kernel(bf16* __restrict__ dy, const bf16* __restrict__ y, float* _
   }
 }
 
+// ---- low-rank cross network (DLRM-DCNv2): the element-wise parts of a layer ------------------
+// x_{l+1} = x0 * s_l + x_l with s_l = W_l (V_l x_l) + b_l (the GEMMs run on cuBLASLt).  All
+// tensors are [rows, D] bf16 with D a multiple of 8; each thread moves 16-byte vectors of 8
+// columns and does its math in fp32, rounding once per stored element.
+__device__ __forceinline__ void unpack8(const uint4& v, float (&f)[8]) {
+  const uint32_t* w = reinterpret_cast<const uint32_t*>(&v);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float2 t = unpack2<bf16>(w[i]);
+    f[2 * i] = t.x;
+    f[2 * i + 1] = t.y;
+  }
+}
+__device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
+  uint4 v;
+  uint32_t* w = reinterpret_cast<uint32_t*>(&v);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) w[i] = pack2<bf16>(f[2 * i], f[2 * i + 1]);
+  return v;
+}
+
+// out = x0 * s + xl (one fma per element); flat grid-stride over 8-column vectors
+__global__ void __launch_bounds__(256)
+cross_fwd_kernel(const uint4* __restrict__ x0, const uint4* __restrict__ s,
+                 const uint4* __restrict__ xl, uint4* __restrict__ out, int64_t n_vec) {
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n_vec;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    float a[8], b[8], c[8];
+    unpack8(x0[i], a);
+    unpack8(s[i], b);
+    unpack8(xl[i], c);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) c[k] = fmaf(a[k], b[k], c[k]);
+    out[i] = pack8(c);
+  }
+}
+
+// The row-tiled kernels below split the D / 8 vector columns of a row into `n_tiles` tiles of
+// `tile` vectors (blockIdx.y), so that rows of any width fit a 256-thread block the way
+// relu_bwd_bias lays them out: rows_par = 256 / tile rows in flight, kRbUnroll rows per thread
+// and iteration, rows_per_block rows per block (blockIdx.x).
+
+// g = bf16(dy * x0) ; db[c] += sum_rows dy * x0 (fp32 products; per-block partial sums reduced
+// in shared memory, then one atomic per column per block)
+__global__ void __launch_bounds__(256)
+cross_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x0, bf16* __restrict__ g,
+                 float* __restrict__ db, int64_t rows, int cols, int tile, int rows_per_block) {
+  extern __shared__ float s_part[];  // [rows_par][tile * 8]
+  const int tpr = cols >> 3;
+  const int v0 = blockIdx.y * tile;                // first vector column of this tile
+  const int tw = min(tile, tpr - v0);              // vector columns in this tile
+  const int rows_par = blockDim.x / tile;
+  const int tr = threadIdx.x / tile, tc = threadIdx.x - tr * tile;
+  const int64_t r0 = static_cast<int64_t>(blockIdx.x) * rows_per_block;
+  const int64_t r1 = min(rows, r0 + rows_per_block);
+  float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  const bool active = tr < rows_par && tc < tw;
+  if (active) {
+    const int64_t col = static_cast<int64_t>(v0 + tc) * 8;
+    for (int64_t r = r0 + tr; r < r1; r += static_cast<int64_t>(rows_par) * kRbUnroll) {
+      uint4 a[kRbUnroll], b[kRbUnroll];
+#pragma unroll
+      for (int u = 0; u < kRbUnroll; ++u) {
+        const int64_t rr = r + static_cast<int64_t>(u) * rows_par;
+        if (rr < r1) {
+          a[u] = *reinterpret_cast<const uint4*>(dy + rr * cols + col);
+          b[u] = *reinterpret_cast<const uint4*>(x0 + rr * cols + col);
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < kRbUnroll; ++u) {
+        const int64_t rr = r + static_cast<int64_t>(u) * rows_par;
+        if (rr < r1) {
+          float fa[8], fb[8];
+          unpack8(a[u], fa);
+          unpack8(b[u], fb);
+#pragma unroll
+          for (int k = 0; k < 8; ++k) {
+            fa[k] *= fb[k];
+            acc[k] += fa[k];
+          }
+          *reinterpret_cast<uint4*>(g + rr * cols + col) = pack8(fa);
+        }
+      }
+    }
+  }
+  if (tr < rows_par) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) s_part[tr * tile * 8 + tc * 8 + k] = acc[k];
+  }
+  __syncthreads();
+  for (int c = threadIdx.x; c < tw * 8; c += blockDim.x) {
+    float v = 0.f;
+    for (int t = 0; t < rows_par; ++t) v += s_part[t * tile * 8 + c];
+    atomicAdd(db + v0 * 8 + c, v);
+  }
+}
+
+// dx0 = d_chain + sum_l dy_l * s_l (fp32, rounded once).  Columns below emb_cols go to dx0, the
+// others (the bottom-MLP vector) to the contiguous d_bottom [rows, cols - emb_cols].
+__global__ void __launch_bounds__(256)
+cross_dx0_kernel(const bf16* __restrict__ d_chain, const __grid_constant__ CrossTerms terms,
+                 bf16* __restrict__ dx0, bf16* __restrict__ d_bottom, int64_t rows, int cols,
+                 int emb_cols, int tile, int rows_per_block) {
+  const int tpr = cols >> 3;
+  const int v0 = blockIdx.y * tile;
+  const int tw = min(tile, tpr - v0);
+  const int rows_par = blockDim.x / tile;
+  const int tr = threadIdx.x / tile, tc = threadIdx.x - tr * tile;
+  if (tr >= rows_par || tc >= tw) return;
+  const int col = (v0 + tc) * 8;
+  const int64_t r0 = static_cast<int64_t>(blockIdx.x) * rows_per_block;
+  const int64_t r1 = min(rows, r0 + rows_per_block);
+  const int bcols = cols - emb_cols;
+  bf16* dst = col < emb_cols ? dx0 + col : d_bottom + (col - emb_cols);
+  const int64_t dst_stride = col < emb_cols ? cols : bcols;
+  for (int64_t r = r0 + tr; r < r1; r += rows_par) {
+    const int64_t off = r * cols + col;
+    float acc[8];
+    unpack8(*reinterpret_cast<const uint4*>(d_chain + off), acc);
+    for (int l = 0; l < terms.n; ++l) {
+      float a[8], b[8];
+      unpack8(*(reinterpret_cast<const uint4*>(terms.dy[l]) + off / 8), a);
+      unpack8(*(reinterpret_cast<const uint4*>(terms.s[l]) + off / 8), b);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) acc[k] = fmaf(a[k], b[k], acc[k]);
+    }
+    *reinterpret_cast<uint4*>(dst + r * dst_stride) = pack8(acc);
+  }
+}
+
 // Final layer (K -> 1) + BCE-with-logits loss + backward of both, one warp per sample:
 //   logit = <x, w> + b ; loss += softplus terms ; dlogit = (sigmoid(logit) - label) * inv_batch
 //   dx = dlogit * w masked by (x > 0) (x is a ReLU output) ; dw += dlogit * x ; db += dlogit ;
@@ -1017,6 +1148,63 @@ bool launch_interact_bwd(const void* bottom, int64_t bottom_stride, const void* 
   if (dim == 32) DE_IBWD(32)
 #undef DE_IBWD
   return false;
+}
+
+// Tiling of the row-tiled cross kernels: the number of column tiles that keeps the most of a
+// 256-thread block busy (each tile holds at most 256 vector columns).
+static void cross_tiling(int cols, int* tile, int* n_tiles, int* rows_per_block) {
+  const int tpr = cols / 8;
+  int best_t = 0, best_n = 0;
+  double best = -1.0;
+  for (int n = (tpr + 255) / 256; n <= tpr && n <= 64; ++n) {
+    const int t = (tpr + n - 1) / n;
+    const int rows_par = 256 / t;
+    const double busy = static_cast<double>(rows_par * t) / 256.0 *
+                        static_cast<double>(tpr) / static_cast<double>(n * t);
+    if (busy > best + 1e-9) {
+      best = busy;
+      best_t = t;
+      best_n = n;
+    }
+  }
+  *tile = best_t;
+  *n_tiles = best_n;
+  // ~16 rows per thread, as relu_bwd_bias
+  *rows_per_block = (256 / best_t) * kRbUnroll * 4;
+}
+
+void launch_cross_fwd(const void* x0, const void* s, const void* xl, void* out, int64_t n,
+                      int sm_count, cudaStream_t stream) {
+  const int64_t n_vec = n / 8;
+  if (n_vec <= 0) return;
+  int64_t blocks = (n_vec + 255) / 256;
+  if (blocks > sm_count * 8) blocks = sm_count * 8;
+  cross_fwd_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
+      reinterpret_cast<const uint4*>(x0), reinterpret_cast<const uint4*>(s),
+      reinterpret_cast<const uint4*>(xl), reinterpret_cast<uint4*>(out), n_vec);
+}
+
+void launch_cross_bwd(const void* dy, const void* x0, void* g, float* db, int64_t rows, int cols,
+                      cudaStream_t stream) {
+  if (rows <= 0) return;
+  int tile, n_tiles, rpb;
+  cross_tiling(cols, &tile, &n_tiles, &rpb);
+  const dim3 grid(static_cast<unsigned>((rows + rpb - 1) / rpb), static_cast<unsigned>(n_tiles));
+  const size_t smem = static_cast<size_t>(256 / tile) * tile * 8 * sizeof(float);
+  cross_bwd_kernel<<<grid, 256, smem, stream>>>(
+      reinterpret_cast<const bf16*>(dy), reinterpret_cast<const bf16*>(x0),
+      reinterpret_cast<bf16*>(g), db, rows, cols, tile, rpb);
+}
+
+void launch_cross_dx0(const void* d_chain, const CrossTerms& terms, void* dx0, void* d_bottom,
+                      int64_t rows, int cols, int emb_cols, cudaStream_t stream) {
+  if (rows <= 0) return;
+  int tile, n_tiles, rpb;
+  cross_tiling(cols, &tile, &n_tiles, &rpb);
+  const dim3 grid(static_cast<unsigned>((rows + rpb - 1) / rpb), static_cast<unsigned>(n_tiles));
+  cross_dx0_kernel<<<grid, 256, 0, stream>>>(
+      reinterpret_cast<const bf16*>(d_chain), terms, reinterpret_cast<bf16*>(dx0),
+      reinterpret_cast<bf16*>(d_bottom), rows, cols, emb_cols, tile, rpb);
 }
 
 void launch_relu_bwd_bias(void* dy, const void* y, float* db, int64_t rows, int cols,

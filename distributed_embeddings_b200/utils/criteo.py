@@ -27,14 +27,20 @@ def get_categorical_feature_type(size: int):
 
 
 class DummyDataset:
-  """Constant synthetic batches (model-parallel categorical inputs unless ``dp_input``)."""
+  """Constant synthetic batches (model-parallel categorical inputs unless ``dp_input``).
+  ``hotness``: ids per sample of each of the ``num_tables`` features; given, every categorical
+  tensor is ``[b, h_f]`` (multi-hot), else ``[b]``."""
 
   def __init__(self, batch_size: int, num_numerical: int, num_workers: int, num_tables: int,
-               is_train: bool, dp_input: bool, num_batches: int):
+               is_train: bool, dp_input: bool, num_batches: int,
+               hotness: Optional[Sequence[int]] = None):
     lb = batch_size // num_workers
     self.numerical = torch.zeros(lb, num_numerical)
     cb = lb if dp_input else batch_size
-    self.categorical = [torch.zeros(cb, dtype=torch.int64) for _ in range(num_tables)]
+    if hotness is None:
+      self.categorical = [torch.zeros(cb, dtype=torch.int64) for _ in range(num_tables)]
+    else:
+      self.categorical = [torch.zeros(cb, int(h), dtype=torch.int64) for h in hotness]
     self.labels = torch.ones(lb if is_train else batch_size, 1)
     self.num_batches = num_batches
 

@@ -4,6 +4,7 @@
   torchrun --nproc-per-node 8 --master-addr 127.0.0.1 examples/dlrm/main.py \
       --dataset_path /data/criteo_split_binary        # real data (split binary Criteo)
   python examples/dlrm/main.py --num_batches 100                       # synthetic data
+  python examples/dlrm/main.py --interaction dcnv2 --multi_hot_sizes mlperf   # DLRM-DCNv2
 
 Embeddings are model parallel (memory_balanced placement), MLPs data parallel; SGD lr 24 with
 warm-up + polynomial decay; AUC on the eval split; embedding weights saved with np.savez in the
@@ -22,7 +23,7 @@ import torch
 import torch.distributed as dist
 
 import distributed_embeddings_b200 as de
-from distributed_embeddings_b200.models.dlrm import DLRM
+from distributed_embeddings_b200.models.dlrm import DLRM, MLPERF_DCNV2_MULTI_HOT_SIZES
 from distributed_embeddings_b200.models.trainer import HybridTrainer
 from distributed_embeddings_b200.utils.criteo import DummyDataset, RawBinaryDataset
 from distributed_embeddings_b200.utils.lr_schedule import LearningRateScheduler
@@ -46,6 +47,14 @@ def parse():
   p.add_argument("--dp_input", action="store_true")
   p.add_argument("--test_combiner", action="store_true")
   p.add_argument("--dist_strategy", default="memory_balanced")
+  p.add_argument("--interaction", default="dot", choices=["dot", "dcnv2"],
+                 help="pairwise dot interaction (DLRM) or low-rank cross network (DLRM-DCNv2)")
+  p.add_argument("--dcn_num_layers", type=int, default=3)
+  p.add_argument("--dcn_low_rank_dim", type=int, default=512)
+  p.add_argument("--multi_hot_sizes", default=None,
+                 help="ids per sample of every feature (comma-separated, or 'mlperf' for the "
+                      "MLPerf DLRM-DCNv2 hotness); synthetic data only, the split-binary reader "
+                      "is one-hot")
   p.add_argument("--fast", action="store_true", help="hand-scheduled step + CUDA graph")
   p.add_argument("--eval_interval", type=int, default=0,
                  help="with --fast: every N training steps, evaluate --eval_batches batches of "
@@ -85,6 +94,12 @@ def main():
       table_sizes = [s + 1 for s in json.load(f).values()]
   else:
     table_sizes = [int(s) for s in args.table_sizes.split(",")]
+  hotness = None
+  if args.multi_hot_sizes is not None:
+    if args.dataset_path is not None:
+      raise SystemExit("--multi_hot_sizes needs synthetic data: the split-binary reader is one-hot")
+    hotness = list(MLPERF_DCNV2_MULTI_HOT_SIZES) if args.multi_hot_sizes == "mlperf" else \
+        [int(h) for h in args.multi_hot_sizes.split(",")]
 
   model = DLRM(table_sizes, embedding_dim=args.embedding_dim,
                bottom_mlp_dims=[int(d) for d in args.bottom_mlp_dims.split(",")],
@@ -92,7 +107,9 @@ def main():
                num_numerical_features=args.num_numerical_features, dp_input=args.dp_input,
                dist_strategy=args.dist_strategy, test_combiner=args.test_combiner, device=device,
                compute_dtype=torch.bfloat16 if (args.amp and cuda) else torch.float32,
-               table_dtype=TABLE_DTYPES[args.table_dtype])
+               table_dtype=TABLE_DTYPES[args.table_dtype], interaction=args.interaction,
+               dcn_num_layers=args.dcn_num_layers, dcn_low_rank_dim=args.dcn_low_rank_dim,
+               multi_hot_sizes=hotness)
   table_ids = list(range(len(table_sizes))) if args.dp_input else \
       model.embedding.strategy.input_ids_list[rank]
   lbs = args.batch_size // world
@@ -104,10 +121,11 @@ def main():
     train = RawBinaryDataset(args.dataset_path, **kw)
     evald = RawBinaryDataset(args.dataset_path, valid=True, **kw)
   else:
+    hots = [hotness[t] for t in table_ids] if hotness is not None else None
     train = DummyDataset(args.batch_size, args.num_numerical_features, world, len(table_ids), True,
-                         args.dp_input, args.num_batches)
+                         args.dp_input, args.num_batches, hots)
     evald = DummyDataset(args.batch_size, args.num_numerical_features, world, len(table_ids),
-                         False, args.dp_input, max(1, args.num_batches // 10))
+                         False, args.dp_input, max(1, args.num_batches // 10), hots)
 
   sched = LearningRateScheduler(args.learning_rate, warmup_steps=args.warmup_steps,
                                 decay_start_step=args.decay_start_step,
@@ -120,7 +138,10 @@ def main():
   if fast:
     from distributed_embeddings_b200.models.dlrm_fast import DLRMTrainStep
     trainer = DLRMTrainStep(model, lr=args.learning_rate, scheduler=sched)
-    step = lambda n, c, l: trainer.step(n, torch.stack([x.to(torch.int32) for x in c]), l)
+    if args.interaction == "dcnv2":  # list of [b, h_f] ids
+      step = lambda n, c, l: trainer.step(n, [x.to(torch.int32) for x in c], l)
+    else:
+      step = lambda n, c, l: trainer.step(n, torch.stack([x.to(torch.int32) for x in c]), l)
   else:
     trainer = HybridTrainer(model, lr=args.learning_rate, scheduler=sched)
     step = trainer.step
@@ -138,8 +159,9 @@ def main():
       lab = lab.reshape(-1)
       if lab.numel() > num.shape[0]:  # global labels: this rank's slice
         lab = lab[rank * num.shape[0]:(rank + 1) * num.shape[0]]
-      trainer.evaluate(num, torch.stack([c.to(device).to(torch.int32).reshape(-1) for c in cat]),
-                       lab.to(device).float())
+      ids = [c.to(device).to(torch.int32) for c in cat]
+      trainer.evaluate(num, ids if args.interaction == "dcnv2" else
+                       torch.stack([c.reshape(-1) for c in ids]), lab.to(device).float())
     m = trainer.eval_metrics()  # collective
     if rank == 0:
       print(f"eval step: {i} AUC: {m['auc']:.6f} tie_bound: {m['tie_bound']:.2e} "

@@ -46,6 +46,9 @@ HOT = [
     ("gemm_tn_pair", r"gemm_tn_pair_kernel"),
     ("integer_lookup", r"integer_lookup_kernel"),
     ("relu_bwd_bias", r"relu_bwd_bias_kernel"),
+    ("cross_fwd", r"cross_fwd_kernel"),
+    ("cross_bwd", r"cross_bwd_kernel"),
+    ("cross_dx0", r"cross_dx0_kernel"),
     ("head_loss_8", r"head_loss_kernel<8>"),
     ("head_eval_8", r"head_eval_kernel<8>"),
     ("sgd_update", r"sgd_update_kernel"),
