@@ -128,9 +128,14 @@ class DLRM(nn.Module):
                interaction: str = "dot",
                dcn_num_layers: int = 3,
                dcn_low_rank_dim: int = 512,
-               multi_hot_sizes: Optional[Sequence[int]] = None):
+               multi_hot_sizes: Optional[Sequence[int]] = None,
+               gpu_embedding_size: Optional[int] = None,
+               offload_cache_size: Optional[int] = None):
     """``table_dtype``: storage of the model-parallel embedding tables (fp32, bf16 or fp16, see
-    :class:`DistributedEmbedding`); bf16 fits the 40M-row MLPerf tables on one 80 GB GPU."""
+    :class:`DistributedEmbedding`); bf16 fits the 40M-row MLPerf tables on one 80 GB GPU.
+    ``gpu_embedding_size`` / ``offload_cache_size``: per-rank HBM element budgets of the tables
+    and of the HBM cache of the tables beyond it (pinned host memory), see
+    :class:`DistributedEmbedding`."""
     super().__init__()
     if interaction not in ("dot", "dcnv2"):
       raise ValueError("interaction must be 'dot' or 'dcnv2'")
@@ -174,7 +179,9 @@ class DLRM(nn.Module):
                                           backend=backend,
                                           world_size=world_size,
                                           rank=rank,
-                                          table_dtype=table_dtype)
+                                          table_dtype=table_dtype,
+                                          gpu_embedding_size=gpu_embedding_size,
+                                          offload_cache_size=offload_cache_size)
     # the activation is consumed inside this module's step: no defensive copy of the engine buffer
     self.embedding.zero_copy_output = True
     if interaction == "dot":

@@ -362,8 +362,9 @@ class DLRMTrainStep:
     self.ops.select_copy([a[0], a[1], a[2]], [b_[0], b_[1], b_[2]],
                          [self.cat_stage, self.num_in, self.lab_in], self._slot_dev)
 
-  def _forward(self):
-    """Forward up to the top MLP output on the inputs in ``cat_stage`` / ``num_in``."""
+  def _forward(self, train: bool = True):
+    """Forward up to the top MLP output on the inputs in ``cat_stage`` / ``num_in``; ``train``:
+    a training step follows (False: evaluation)."""
     ops = self.ops
     # the embedding exchange (id push, gather + NVLink push of the pooled rows; all signalling
     # folded into those kernels) runs on the side stream while the bottom MLP runs on the main
@@ -372,7 +373,7 @@ class DLRMTrainStep:
     if self._side is not None:
       self._side.wait_stream(torch.cuda.current_stream())
       with torch.cuda.stream(self._side):
-        eng.launch_forward()
+        eng.launch_forward(train)
     ops.cast_pad(self.num_in, self.x0)
     x = self.x0
     for L in self.bottom:
@@ -380,7 +381,7 @@ class DLRMTrainStep:
     if self._side is not None:
       torch.cuda.current_stream().wait_stream(self._side)
     else:
-      eng.launch_forward()
+      eng.launch_forward(train)
     if eng.out_needs_reduce:  # multi-hot row slices: partial pools are summed first
       eng.wait_output()
       ops.interact_fwd(x, eng.out, self.n_emb, self.z, [])
@@ -390,14 +391,14 @@ class DLRMTrainStep:
     for L in self.top:
       x = self._linear_fwd(L, x)
 
-  def _forward_dcn(self):
+  def _forward_dcn(self, train: bool = True):
     """Forward of the dcnv2 model up to the top MLP output."""
     ops, eng = self.ops, self.engine
     # lookups (into x0's embedding columns) on the side stream under the bottom MLP
     if self._side is not None:
       self._side.wait_stream(torch.cuda.current_stream())
       with torch.cuda.stream(self._side):
-        eng.launch_forward()
+        eng.launch_forward(train)
     ops.cast_pad(self.num_in, self.x0)
     x = self.x0
     for L in self.bottom:
@@ -407,7 +408,7 @@ class DLRMTrainStep:
     if self._side is not None:
       torch.cuda.current_stream().wait_stream(self._side)
     else:
-      eng.launch_forward()
+      eng.launch_forward(train)
     eng.wait_output()
     x = x0
     for l, (V, W) in enumerate(self.cross):
@@ -697,7 +698,8 @@ class DLRMTrainStep:
   # counts stay equal on all ranks and the next training step's id push waits as before.
   def _eval_impl(self):
     with nvtx.range("dlrm_eval"):
-      self._forward_dcn() if self.dcn else self._forward()
+      # a forward-only pass: the offload cache marks no row dirty
+      self._forward_dcn(False) if self.dcn else self._forward(False)
       H = self.head
       self.ops.head_eval(self.top[-1].y, H.w16.view(-1), H.b16, self.lab_in, self._n_valid,
                          self._probs, self.eval_auc.hist, self._eval_loss, self._eval_count)

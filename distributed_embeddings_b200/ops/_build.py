@@ -24,7 +24,8 @@ BUILD_DIR = os.path.join(PKG_DIR, "ops", "_build")
 SO_PATH = os.path.join(PKG_DIR, "_C.so")
 
 CU_SOURCES = ["lookup_kernels.cu", "sparse_update_kernels.cu", "misc_kernels.cu", "comm_kernels.cu",
-              "dense_kernels.cu", "gemm_wgmma.cu", "radix_sort.cu"]
+              "dense_kernels.cu", "gemm_wgmma.cu", "radix_sort.cu",
+              "offload_cache.cu"]
 CPP_SOURCES = ["bindings.cpp"]
 
 ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]

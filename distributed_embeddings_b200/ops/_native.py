@@ -51,6 +51,15 @@ GRAD_ROUTE = np.dtype([
     ("dst_col", "<i4"),
     ("pad", "<i4"),
 ])
+# mirror of de::CacheRemap: one cached input of the offload cache's id remap (offload_cache.cu)
+CACHE_REMAP = np.dtype([
+    ("ids", "<u8"),
+    ("n", "<i8"),
+    ("id_shift", "<i8"),
+    ("sub_rows", "<i8"),
+    ("row_base", "<i8"),
+    ("out_off", "<i8"),
+])
 SYNC_STATE_WORDS = 64
 DTYPE_CODE = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
 
@@ -76,7 +85,7 @@ def load(required: bool = False) -> bool:
       torch.ops.load_library(SO_PATH)
       sizes = list(torch.ops.de_b200.struct_sizes())
       mine = [INPUT_DESC.itemsize, TABLE_DESC.itemsize, MAX_PEERS, GRAD_ROUTE.itemsize,
-              SYNC_STATE_WORDS]
+              SYNC_STATE_WORDS, CACHE_REMAP.itemsize]
       if sizes != mine:
         raise RuntimeError(f"descriptor layout mismatch: native {sizes} vs python {mine} "
                            "(stale _C.so? rebuild with python -m distributed_embeddings_b200.ops._build)")

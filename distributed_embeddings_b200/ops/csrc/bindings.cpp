@@ -131,7 +131,8 @@ void sync_only(at::IntArrayRef sync) {
 std::vector<int64_t> struct_sizes() {
   return {static_cast<int64_t>(sizeof(de::InputDesc)), static_cast<int64_t>(sizeof(de::TableDesc)),
           static_cast<int64_t>(de::kMaxPeers), static_cast<int64_t>(sizeof(de::GradRoute)),
-          static_cast<int64_t>(de::kSyncStateWords)};
+          static_cast<int64_t>(de::kSyncStateWords),
+          static_cast<int64_t>(sizeof(de::CacheRemap))};
 }
 
 void lookup_fwd(const Tensor& descs, int64_t n_inputs, int64_t batch, int64_t src_batch,
@@ -1241,6 +1242,158 @@ void ipc_close(int64_t ptr, int64_t device_index) {
   cudaIpcCloseMemHandle(reinterpret_cast<void*>(ptr));
 }
 
+// ------------------------------------------------------------------ offload cache
+// cache = [weight, state0, state1, tags, ticks, dirty, tick_word, stats] (absent states: empty
+// tensors); host = device-visible pointers of [weight, state0, state1] of the host table.
+de::CacheTable to_cache(at::TensorList cache, at::IntArrayRef host, int64_t n_sets,
+                        int64_t n_spill, int64_t rows) {
+  TORCH_CHECK(cache.size() == 8, "offload cache: 8 tensors expected");
+  TORCH_CHECK(host.size() == 3, "offload cache: 3 host pointers expected");
+  TORCH_CHECK(n_sets >= 1 && n_sets < (int64_t(1) << 31) && n_spill >= 0 && rows >= 1 &&
+                  rows < (int64_t(1) << 32) - 1,
+              "offload cache: bad geometry (n_sets ", n_sets, ", n_spill ", n_spill, ", rows ",
+              rows, ")");
+  const int64_t slots = n_sets * 32 + n_spill;
+  const Tensor& w = cache[0];
+  TORCH_CHECK(w.is_cuda() && w.scalar_type() == at::kFloat && w.is_contiguous() && w.dim() == 2 &&
+                  w.size(0) == slots && w.size(1) >= 1 && w.data_ptr() != nullptr,
+              "offload cache: weight must be a contiguous fp32 CUDA tensor [", slots, ", width]");
+  TORCH_CHECK(w.size(1) % 4 != 0 || (reinterpret_cast<uintptr_t>(w.data_ptr()) % 16 == 0 &&
+                                     host[0] % 16 == 0),
+              "offload cache: rows of width % 4 == 0 must be 16-byte aligned");
+  TORCH_CHECK(host[0] != 0, "offload cache: host table pointer is null");
+  de::CacheTable T{};
+  T.weight = w.data_ptr<float>();
+  T.host_weight = reinterpret_cast<float*>(host[0]);
+  T.width = static_cast<int32_t>(w.size(1));
+  float** cs[2] = {&T.state0, &T.state1};
+  float** hs[2] = {&T.host_state0, &T.host_state1};
+  int32_t* sw[2] = {&T.state0_width, &T.state1_width};
+  for (int k = 0; k < 2; ++k) {
+    const Tensor& s = cache[1 + k];
+    if (s.numel() == 0) {
+      TORCH_CHECK(host[1 + k] == 0, "offload cache: host state without a cache state");
+      continue;
+    }
+    TORCH_CHECK(s.is_cuda() && s.scalar_type() == at::kFloat && s.is_contiguous() &&
+                    s.size(0) == slots && (s.dim() == 1 || (s.dim() == 2 && s.size(1) == w.size(1))),
+                "offload cache: state must be fp32 CUDA [slots] or [slots, width]");
+    TORCH_CHECK(host[1 + k] != 0 && host[1 + k] % 16 == 0 &&
+                    reinterpret_cast<uintptr_t>(s.data_ptr()) % 16 == 0,
+                "offload cache: host state pointer is null or misaligned");
+    *cs[k] = s.data_ptr<float>();
+    *hs[k] = reinterpret_cast<float*>(host[1 + k]);
+    *sw[k] = static_cast<int32_t>(s.dim() == 1 ? 1 : s.size(1));
+  }
+  auto check_i = [&](const Tensor& t, at::ScalarType ty, int64_t n, const char* what) {
+    TORCH_CHECK(t.is_cuda() && t.scalar_type() == ty && t.is_contiguous() && t.numel() == n &&
+                    t.device() == w.device(),
+                "offload cache: ", what, " must be a contiguous CUDA tensor of ", n, " elements");
+  };
+  check_i(cache[3], at::kLong, slots, "tags (int64)");
+  check_i(cache[4], at::kInt, n_sets * 32, "ticks (int32)");
+  check_i(cache[5], at::kInt, slots, "dirty (int32)");
+  check_i(cache[6], at::kInt, 1, "tick_word (int32)");
+  check_i(cache[7], at::kLong, 4, "stats (int64)");
+  T.tags = cache[3].data_ptr<int64_t>();
+  T.ticks = cache[4].data_ptr<int32_t>();
+  T.dirty = cache[5].data_ptr<int32_t>();
+  T.tick_word = cache[6].data_ptr<int32_t>();
+  T.stats = cache[7].data_ptr<int64_t>();
+  T.n_sets = n_sets;
+  T.n_spill = n_spill;
+  T.rows = rows;
+  return T;
+}
+
+// One cache pass of one table (see offload_cache.cu).  descs / tables: the table's cached inputs
+// on their *host* rows (local_table 0, item_off rebased to [0, n_items)) and one TableDesc with
+// key_base 0; remap: their CacheRemap records (device bytes); out_ptr: the slot-id buffer.
+void offload_cache_pass(at::TensorList cache, at::IntArrayRef host, int64_t n_sets,
+                        int64_t n_spill, int64_t rows, const Tensor& descs, const Tensor& tables,
+                        int64_t n_inputs, int64_t batch, bool ids64, int64_t n_items,
+                        bool prefill_sentinel, const Tensor& remap, int64_t n_remap,
+                        int64_t max_remap_n, int64_t out_ptr, bool train) {
+  de::CacheTable T = to_cache(cache, host, n_sets, n_spill, rows);
+  TORCH_CHECK(n_items == n_spill && n_items >= 1,
+              "offload cache: the spill region must hold every id of the step (", n_items,
+              " ids, ", n_spill, " spill slots)");
+  TORCH_CHECK(n_items < (int64_t(1) << 31), "offload cache: too many ids per step");
+  TORCH_CHECK(descs.is_cuda() && tables.is_cuda() && remap.is_cuda() &&
+                  descs.device() == cache[0].device() && remap.device() == cache[0].device(),
+              "offload cache: descriptors must live on the cache's GPU");
+  TORCH_CHECK(descs.numel() == n_inputs * static_cast<int64_t>(sizeof(de::InputDesc)) &&
+                  tables.numel() == static_cast<int64_t>(sizeof(de::TableDesc)) &&
+                  remap.numel() == n_remap * static_cast<int64_t>(sizeof(de::CacheRemap)) &&
+                  n_inputs >= 1 && n_remap >= 1 && max_remap_n >= 0,
+              "offload cache: descriptor array sizes do not match their counts");
+  TORCH_CHECK(out_ptr != 0 && out_ptr % (ids64 ? 8 : 4) == 0, "offload cache: bad slot-id buffer");
+  TORCH_CHECK(n_sets * 32 + n_spill < (ids64 ? (int64_t(1) << 62) : (int64_t(1) << 31)),
+              "offload cache: slot ids do not fit the id type");
+  c10::cuda::CUDAGuard guard(cache[0].device());
+  auto stream = cur_stream();
+  auto dev = cache[0].device();
+  auto i64 = at::TensorOptions().device(dev).dtype(at::kLong);
+  auto i32 = at::TensorOptions().device(dev).dtype(at::kInt);
+  // nothing above launches: every argument is checked before the first kernel
+  de::launch_cache_spill_writeback(T, sm_count(), stream);
+  check_launch();
+  auto sorted = sort_items(descs, tables, 1, n_inputs, batch, batch, {}, ids64, n_items, rows,
+                           prefill_sentinel);
+  const Tensor& keys = std::get<0>(sorted);
+  const Tensor& seg_start = std::get<2>(sorted);
+  const Tensor& n_unique = std::get<3>(sorted);
+  Tensor uniq = at::empty({n_items}, i64), slot_of = at::empty({n_items}, i64);
+  Tensor move = at::empty({n_items}, i64);
+  Tensor set_a = at::empty({n_items}, i32), item_a = at::empty({n_items}, i32);
+  Tensor set_b = at::empty({n_items}, i32), item_b = at::empty({n_items}, i32);
+  Tensor set_sorted = at::empty({n_items}, i64);
+  Tensor seg = at::empty({n_items + 1}, i64), n_seg = at::zeros({1}, i64);
+  const size_t temp_bytes =
+      std::max(de::radix_sort_temp_bytes(n_items), de::head_segments_temp_bytes(n_items));
+  Tensor temp = at::empty({static_cast<int64_t>(temp_bytes)},
+                          at::TensorOptions().device(dev).dtype(at::kByte));
+  de::launch_cache_probe(T, keys.data_ptr<int64_t>(), seg_start.data_ptr<int64_t>(),
+                         n_unique.data_ptr<int64_t>(), n_items, train, uniq.data_ptr<int64_t>(),
+                         reinterpret_cast<uint32_t*>(set_a.data_ptr<int>()),
+                         reinterpret_cast<uint32_t*>(item_a.data_ptr<int>()),
+                         slot_of.data_ptr<int64_t>(), move.data_ptr<int64_t>(), sm_count(), stream);
+  check_launch();
+  // stable sort by set: a set's misses keep their ascending row order
+  int where = de::radix_sort_pairs32(
+      temp.data_ptr(), reinterpret_cast<uint32_t*>(set_a.data_ptr<int>()),
+      reinterpret_cast<uint32_t*>(item_a.data_ptr<int>()),
+      reinterpret_cast<uint32_t*>(set_b.data_ptr<int>()),
+      reinterpret_cast<uint32_t*>(item_b.data_ptr<int>()), set_sorted.data_ptr<int64_t>(), n_items,
+      bit_length(n_sets), stream);
+  const Tensor& u_sorted = where == 0 ? item_a : item_b;
+  de::head_segments(temp.data_ptr(), set_sorted.data_ptr<int64_t>(), n_items,
+                    seg.data_ptr<int64_t>(), n_seg.data_ptr<int64_t>(), stream);
+  check_launch();
+  de::launch_cache_assign(T, set_sorted.data_ptr<int64_t>(),
+                          reinterpret_cast<const uint32_t*>(u_sorted.data_ptr<int>()),
+                          seg.data_ptr<int64_t>(), n_seg.data_ptr<int64_t>(), n_items, train,
+                          uniq.data_ptr<int64_t>(), slot_of.data_ptr<int64_t>(),
+                          move.data_ptr<int64_t>(), sm_count(), stream);
+  check_launch();
+  de::launch_cache_fill(T, n_unique.data_ptr<int64_t>(), n_items, uniq.data_ptr<int64_t>(),
+                        slot_of.data_ptr<int64_t>(), move.data_ptr<int64_t>(), sm_count(), stream);
+  check_launch();
+  de::launch_cache_remap(reinterpret_cast<const de::CacheRemap*>(remap.data_ptr()),
+                         static_cast<int>(n_remap), max_remap_n, uniq.data_ptr<int64_t>(),
+                         n_unique.data_ptr<int64_t>(), slot_of.data_ptr<int64_t>(), rows, ids64,
+                         reinterpret_cast<void*>(out_ptr), sm_count(), stream);
+  check_launch();
+}
+
+void offload_cache_flush(at::TensorList cache, at::IntArrayRef host, int64_t n_sets,
+                         int64_t n_spill, int64_t rows) {
+  de::CacheTable T = to_cache(cache, host, n_sets, n_spill, rows);
+  c10::cuda::CUDAGuard guard(cache[0].device());
+  de::launch_cache_flush(T, sm_count(), cur_stream());
+  check_launch();
+}
+
 // Map a host tensor's storage for zero-copy GPU access (CPU-offloaded tables): returns the
 // device-visible pointer of pinned (cudaHostRegister'ed / pin_memory) memory.
 int64_t host_device_pointer(const Tensor& host) {
@@ -1396,4 +1549,12 @@ TORCH_LIBRARY(de_b200, m) {
   m.def("ipc_open(Tensor handle, int device_index) -> int", &ipc_open);
   m.def("ipc_close(int ptr, int device_index) -> ()", &ipc_close);
   m.def("host_device_pointer(Tensor host) -> int", &host_device_pointer);
+  m.def(
+      "offload_cache_pass(Tensor[] cache, int[] host, int n_sets, int n_spill, int rows, "
+      "Tensor descs, Tensor tables, int n_inputs, int batch, bool ids64, int n_items, "
+      "bool prefill_sentinel, Tensor remap, int n_remap, int max_remap_n, int out_ptr, "
+      "bool train) -> ()",
+      &offload_cache_pass);
+  m.def("offload_cache_flush(Tensor[] cache, int[] host, int n_sets, int n_spill, int rows) -> ()",
+        &offload_cache_flush);
 }

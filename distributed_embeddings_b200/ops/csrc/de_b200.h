@@ -166,6 +166,55 @@ bool launch_balanced_update(const InputDesc* descs, const TableDesc* tables, int
                             int max_width, int act_dtype, int sm_count, cudaStream_t stream,
                             int table_dtype = 0);
 
+// ---- HBM row cache of host-offloaded fp32 tables (offload_cache.cu) ------------------------
+// Slots [0, n_sets * 32) are the sets (32 ways each), [n_sets * 32, + n_spill) the spill region.
+struct CacheTable {
+  float* weight;        // [slots, width] HBM
+  float* state0;        // [slots, state0_width] HBM or nullptr
+  float* state1;        // [slots, state1_width] HBM or nullptr
+  float* host_weight;   // [rows, width] pinned host table (device-visible UVA pointer)
+  float* host_state0;   // its optimizer state, same layout as the cache's
+  float* host_state1;
+  int64_t* tags;        // [slots]: host row held by the slot, -1 = empty
+  int32_t* ticks;       // [n_sets * 32]: tick of the last use
+  int32_t* dirty;       // [slots]: the slot was updated since it was filled / flushed
+  int32_t* tick_word;   // last tick of a finished cache pass (device resident)
+  int64_t* stats;       // hits, misses, spills, write-backs (unique rows)
+  int64_t n_sets;
+  int64_t n_spill;
+  int64_t rows;         // host rows (= the sentinel key of the pass's sort)
+  int32_t width;
+  int32_t state0_width;  // width, 1 (row-wise Adagrad) or 0
+  int32_t state1_width;  // width (Adam v) or 0
+  int32_t pad;
+};
+// One cached input of the remap: ids[0, n) + id_shift valid below sub_rows are host rows
+// row_base + id; their slot ids go to out[out_off + i] (-1 for the others).
+struct alignas(16) CacheRemap {
+  const void* ids;
+  int64_t n;
+  int64_t id_shift;
+  int64_t sub_rows;
+  int64_t row_base;
+  int64_t out_off;
+};
+void launch_cache_spill_writeback(const CacheTable& T, int sm_count, cudaStream_t stream);
+void launch_cache_probe(const CacheTable& T, const int64_t* sorted_keys, const int64_t* seg_start,
+                        const int64_t* n_unique, int64_t cap, bool train, int64_t* uniq,
+                        uint32_t* miss_set, uint32_t* miss_item, int64_t* slot_of, int64_t* move,
+                        int sm_count, cudaStream_t stream);
+void launch_cache_assign(const CacheTable& T, const int64_t* set_sorted, const uint32_t* u_sorted,
+                         const int64_t* seg, const int64_t* n_seg, int64_t cap, bool train,
+                         const int64_t* uniq, int64_t* slot_of, int64_t* move, int sm_count,
+                         cudaStream_t stream);
+void launch_cache_fill(const CacheTable& T, const int64_t* n_unique, int64_t cap,
+                       const int64_t* uniq, const int64_t* slot_of, const int64_t* move,
+                       int sm_count, cudaStream_t stream);
+void launch_cache_remap(const CacheRemap* inputs, int n_inputs, int64_t max_n,
+                        const int64_t* uniq, const int64_t* n_unique, const int64_t* slot_of,
+                        int64_t rows, bool ids64, void* out, int sm_count, cudaStream_t stream);
+void launch_cache_flush(const CacheTable& T, int sm_count, cudaStream_t stream);
+
 // ---- misc ---------------------------------------------------------------------------------
 void launch_row_to_split(const int64_t* coo_indices, int64_t nnz, int64_t num_rows,
                          int64_t* row_splits, cudaStream_t stream);

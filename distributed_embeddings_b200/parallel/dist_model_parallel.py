@@ -232,6 +232,11 @@ class DistributedEmbedding(nn.Module):
       with stochastic rounding (``ops/stochastic_rounding.py``).  Replicated tables stay fp32.
       The ``dtype`` of a passed ``Embedding`` layer or config is ignored here, as it always was.
       Checkpoints (``get_weights`` / ``save_weights``) are fp32 whatever the table dtype.
+    offload_cache_size: per-rank HBM element budget (the unit of ``gpu_embedding_size``) for a
+      cache of the rows of this rank's offloaded tables (keyword only; fused back end, fp32
+      tables).  None (default) reads and updates offloaded rows zero-copy over PCIe on every
+      access.  The budget is split over the offloaded tables in proportion to their rows; each
+      also gets optimizer-state rows and a spill region (see ``parallel/offload_cache.py``).
   """
 
   def __init__(self,
@@ -251,8 +256,23 @@ class DistributedEmbedding(nn.Module):
                rank: Optional[int] = None,
                world_size: Optional[int] = None,
                input_hotness: Optional[Sequence[int]] = None,
-               table_dtype: torch.dtype = torch.float32):
+               table_dtype: torch.dtype = torch.float32,
+               offload_cache_size: Optional[int] = None):
     super().__init__()
+    if offload_cache_size is not None:
+      if gpu_embedding_size is None:
+        raise ValueError("offload_cache_size caches offloaded tables: it needs gpu_embedding_size")
+      if table_dtype != torch.float32:
+        raise ValueError("offload_cache_size supports fp32 tables only (16-bit tables key their "
+                         "stochastic rounding on the row, which a cache slot would change)")
+      if int(offload_cache_size) < 0:
+        raise ValueError("offload_cache_size must be >= 0")
+    self.offload_cache_size = None if offload_cache_size is None else int(offload_cache_size)
+    if self.offload_cache_size is not None:
+      # module checkpoints (state_dict / load_state_dict) see the host tables: flush the cache
+      # before they are read, and drop it before they are overwritten
+      self.register_state_dict_pre_hook(_flush_before_state_dict)
+      self._register_load_state_dict_pre_hook(_drop_before_load, with_module=True)
     if strategy not in STRATEGIES:
       raise ValueError(f"Unsupported shard strategy {strategy}")
     if table_dtype not in (torch.float32, torch.bfloat16, torch.float16):
@@ -273,6 +293,8 @@ class DistributedEmbedding(nn.Module):
     self.gpu_embedding_size = gpu_embedding_size
     # a single worker has nothing to replicate or row slice; mp input keeps everything
     # table-parallel for backward compatibility (reference dist_model_parallel.py:764-774)
+    if self.offload_cache_size is not None and self.world_size > 1:
+      raise ValueError("offload_cache_size is supported on one rank (world size 1) for now")
     if self.world_size > 1:
       self.row_slice_threshold = row_slice_threshold if dp_input else None
       self.data_parallel_threshold = data_parallel_threshold if dp_input else None
@@ -342,6 +364,9 @@ class DistributedEmbedding(nn.Module):
       raise ValueError(f"Unsupported backend {backend}")
     if backend == "fused" and not self._native_layers:
       raise ValueError("the fused backend needs native Embedding layers")
+    if self.offload_cache_size is not None and backend != "fused":
+      raise ValueError("offload_cache_size needs the fused back end (a CUDA device and native "
+                       "Embedding layers)")
     self.backend = backend
     self._engine = None
     # ids-per-sample capacity reserved for ragged inputs in the fused back end (None = inferred
@@ -631,6 +656,32 @@ class DistributedEmbedding(nn.Module):
       return group_rank
     return dist.get_global_rank(self.group, group_rank)
 
+  # ---------------------------------------------------------------------------- offload cache
+  def flush_offload_cache(self):
+    """Write every dirty row of the offload cache, and its optimizer state, back to the host
+    tables.  The checkpoint calls do this themselves."""
+    if self._engine is not None:
+      self._engine.flush_offload_cache()
+
+  def _drop_offload_cache(self):
+    """Flush and empty the cache: the host tables are about to be overwritten."""
+    if self._engine is not None:
+      self._engine.flush_offload_cache(invalidate=True)
+
+  def offload_cache_stats(self, reset: bool = True) -> List[Dict[str, int]]:
+    """Per cached table of this rank: ``{"table", "local_table", "hits", "misses", "spills",
+    "writebacks"}``, counted on the device in unique rows per step (a row a step looks up many
+    times counts once) since the last reset.  ``table`` is the global table index; ``misses``
+    include ``spills``.  Reading them synchronises the device."""
+    if self._engine is None:
+      return []
+    st = self.strategy
+    out = []
+    for m, v in sorted(self._engine.offload_cache_stats(reset).items()):
+      shard = next(s for s in st.shards[self.rank] if s.local_table == m)
+      out.append({"table": st.table_groups[1][shard.table], "local_table": m, **v})
+    return out
+
   def get_weights(self, all_ranks: bool = False, chunk: int = 1 << 26) -> List[np.ndarray]:
     """Return the *global, unsharded* tables as numpy arrays in original table order.
 
@@ -639,6 +690,7 @@ class DistributedEmbedding(nn.Module):
     empty list for the model-parallel tables they do not own).  Shards are read (and cast to
     fp32) in pieces of at most ``chunk`` elements.
     """
+    self.flush_offload_cache()
     weights = self.weights
     n_dp, n_col = len(self.dp_layers), len(self.local_embedding_layers)
     return self._gather_global(weights[:n_dp], weights[n_dp:n_dp + n_col],
@@ -721,6 +773,7 @@ class DistributedEmbedding(nn.Module):
       use_lock: load rank by rank in lock step (bounds host memory on shared nodes).
     """
     st = self.strategy
+    self._drop_offload_cache()
     if len(weights) != len(st.global_configs):
       raise ValueError(
           f"You called `set_weights(weights)` on layer DistributedEmbedding with a weight list of "
@@ -792,6 +845,7 @@ class DistributedEmbedding(nn.Module):
     st = self.strategy
     n_tables = len(st.global_configs)
     paths = [os.path.join(directory, f"{prefix}_{t}.npy") for t in range(n_tables)]
+    self.flush_offload_cache()
     if self.rank == 0:
       os.makedirs(directory, exist_ok=True)
       for t, path in enumerate(paths):
@@ -851,6 +905,7 @@ class DistributedEmbedding(nn.Module):
     every rank must call it; only rank 0 receives the arrays unless ``all_ranks``."""
     opt = self._fused_optimizer
     eng = self._engine
+    self.flush_offload_cache()
     if opt is None or eng is None or not eng.opt_state:
       return {"kind": opt["kind"] if opt else None, "step": eng.step_count() if eng else 0,
               "tables": None}
@@ -877,6 +932,7 @@ class DistributedEmbedding(nn.Module):
     if self._engine is None:
       raise RuntimeError("run a forward pass (or build the engine) before loading optimizer state")
     eng = self._engine
+    self._drop_offload_cache()
     if "tables" not in state:
       eng.load_optimizer_state_dict(state)
       return
@@ -916,6 +972,7 @@ class DistributedEmbedding(nn.Module):
     Collective; returns the path of ``optimizer.json`` (None when there is no state)."""
     import json  # pylint: disable=import-outside-toplevel
     opt, eng = self._fused_optimizer, self._engine
+    self.flush_offload_cache()
     if opt is None or eng is None or not eng.opt_state:
       return None
     st = self.strategy
@@ -993,6 +1050,14 @@ class DistributedEmbedding(nn.Module):
   def extra_repr(self):
     return (f"world_size={self.world_size}, rank={self.rank}, strategy={self.strategy.strategy}, "
             f"backend={self.backend}, dp_input={self.dp_input}")
+
+
+def _flush_before_state_dict(module, prefix, keep_vars):  # pylint: disable=unused-argument
+  module.flush_offload_cache()
+
+
+def _drop_before_load(module, *args, **kwargs):  # pylint: disable=unused-argument
+  module._drop_offload_cache()  # pylint: disable=protected-access
 
 
 # ------------------------------------------------------------------------- hybrid-parallel glue

@@ -46,6 +46,7 @@ from ..ops._native import DTYPE_CODE, GRAD_ROUTE, INPUT_DESC, TABLE_DESC
 from ..ops.ragged import RaggedIds
 from ..utils import nvtx
 from .comm import CH_BARRIER0, CH_CONSUMED, CH_GRAD, CH_IDS, CH_OUT, CommContext
+from .offload_cache import OffloadCache, split_budget
 
 _OPT_KIND = {"sgd": _native.OPT_SGD, "adagrad": _native.OPT_ADAGRAD,
              "rowwise_adagrad": _native.OPT_ROWWISE_ADAGRAD, "adam": _native.OPT_ADAM}
@@ -92,13 +93,13 @@ class ProducerUpdate(NamedTuple):
 class _FusedFn(torch.autograd.Function):
 
   @staticmethod
-  def forward(ctx, engine, token, *weights):  # pylint: disable=arguments-differ
+  def forward(ctx, engine, token, train, *weights):  # pylint: disable=arguments-differ
     ctx.engine = engine
     ctx.n_weights = len(weights)
     ctx.done = False
     engine._gen += 1
     ctx.gen = engine._gen
-    out = engine._run_forward()
+    out = engine._run_forward(train)
     # the backward of this call reads the engine's id / gradient buffers: remember the node so
     # that a second forward before this backward is routed elsewhere (see FusedEngine.busy)
     engine._pending = weakref.ref(ctx)
@@ -116,7 +117,7 @@ class _FusedFn(torch.autograd.Function):
           "or use backend='torch' for several forwards per backward.")
     ctx.done = True
     grads = engine._run_backward(grad_out)
-    return (None, None) + tuple(grads)
+    return (None, None, None) + tuple(grads)
 
 
 class FusedEngine:
@@ -172,6 +173,12 @@ class FusedEngine:
     self.n_col_tables = len(de.local_embedding_layers)
     # host-resident tables are read zero-copy over PCIe; their update must not use atomics
     self.has_offload = any(getattr(l, "cpu_offloaded", False) for l in self.mp_layers)
+    # HBM row cache of the offloaded table-parallel tables (offload_cache.py), local table -> cache
+    self.cache_size = getattr(de, "offload_cache_size", None)
+    self.caches: Dict[int, OffloadCache] = {}
+    self._cache_plan: List[tuple] = []
+    if self.cache_size is not None and (self.dry or self.W > 1):
+      raise NotImplementedError("the offload cache runs on one rank (world size 1) for now")
 
   def _ptr(self, t: torch.Tensor) -> int:
     return t.data_ptr() if self.dry else _dev_ptr(t)
@@ -392,15 +399,17 @@ class FusedEngine:
       return self.in_flat.data_ptr() + in_off[gi] * idsz
 
     # --- table descriptors (sorted-update path)
+    self._make_caches(B, hots, col_group, my_inputs, col_items)
     tdesc = np.zeros(len(self.mp_layers), dtype=TABLE_DESC)
     key = 0
     for m, layer in enumerate(self.mp_layers):
       w = _weight(layer)
+      rows = self.caches[m].slots if m in self.caches else w.shape[0]
       tdesc[m]["weight"] = self._ptr(w)
-      tdesc[m]["rows"] = w.shape[0]
+      tdesc[m]["rows"] = rows
       tdesc[m]["key_base"] = key
       tdesc[m]["width"] = w.shape[1]
-      key += w.shape[0]
+      key += rows
     self.total_rows = key
     self.tdesc_np = tdesc
     self.max_width = max([int(_weight(l).shape[1]) for l in self.mp_layers] + [1])
@@ -469,6 +478,7 @@ class FusedEngine:
         else:
           for s in range(W):
             segs.append([s, in_off[gi], col_items[li] + s * b * hots[gi], b * hots[gi]])
+    self._cache_descs(cdesc, col_items, B, hots, col_group, my_inputs, id_dtype)
     self.cdesc_np = cdesc
 
     # --- row-slice descriptors.  One-hot inputs: exactly one rank owns a sample's id, it stores
@@ -663,6 +673,105 @@ class FusedEngine:
     self._upload()
     self._key = (b, hots, ids64)
 
+  # ------------------------------------------------------------------ offload cache
+  def _make_caches(self, B, hots, col_group, my_inputs, col_items):
+    """(Re)create the caches of the offloaded tables for this batch layout; a cache whose spill
+    region no longer fits is flushed to the host first."""
+    if self.cache_size is None:
+      return
+    de = self.de
+    cached = [m for m in range(self.n_col_tables) if getattr(self.mp_layers[m], "cpu_offloaded",
+                                                             False)]
+    n_spill = {m: 0 for m in cached}
+    for li, k in enumerate(my_inputs):
+      m = next(s for s in self.st.shards[self.rank]
+               if s.table == self.st.map_groups[1][k]).local_table
+      if m in n_spill:
+        gi = col_group[k] if de.dp_input else li
+        n_spill[m] += B * abs(hots[gi])
+    cached = [m for m in cached if n_spill[m] > 0]
+    # a table no input of this layout reads keeps no cache: its rows go back to the host
+    for m in [m for m in self.caches if m not in cached]:
+      self.caches.pop(m).flush(self.ops)
+    sets = split_budget(int(self.cache_size),
+                        [tuple(_weight(self.mp_layers[m]).shape) for m in cached])
+    for m, n_sets in zip(cached, sets):
+      old = self.caches.get(m)
+      if old is not None and (old.n_sets, old.n_spill) == (n_sets, n_spill[m]):
+        continue
+      if old is not None:
+        # a new batch size or hotness changes the spill region: the cache starts over.  The old
+        # one is flushed and released before the new one is allocated (the flush is ordered
+        # before any reuse of its memory by the stream), so the peak stays one cache per table
+        self.caches.pop(m).flush(self.ops)
+        del old
+      c = OffloadCache(_weight(self.mp_layers[m]), n_sets, n_spill[m], self.device, self._ptr)
+      if self.opt_state.get(m):
+        c.set_state(self.opt_state[m])
+      self.caches[m] = c
+
+  def _cache_descs(self, cdesc, col_items, B, hots, col_group, my_inputs, id_dtype):
+    """Point the cached inputs at the cache: their ids become slot ids in ``ids_cache`` (laid out
+    like the owner's id buffer), their table the cache's weight rows.  Builds one pass plan per
+    cached table from the original (host-row) descriptors."""
+    self._cache_plan = []
+    self.ids_cache = None
+    if not self.caches:
+      return
+    dev = self.device
+    self.ids_cache = torch.full((max(self.n_items, 1),), -1, dtype=id_dtype, device=dev)
+    idsz = self.ids_cache.element_size()
+    tab = np.zeros(1, dtype=TABLE_DESC)
+    for m, c in self.caches.items():
+      lis = [li for li in range(len(cdesc)) if int(cdesc[li]["local_table"]) == m]
+      src = cdesc[lis].copy()
+      remap = np.zeros(len(lis), dtype=_native.CACHE_REMAP)
+      pos = 0
+      for j, li in enumerate(lis):
+        k = my_inputs[li]
+        n = B * abs(hots[col_group[k] if self.de.dp_input else li])
+        src[j]["local_table"] = 0
+        src[j]["item_off"] = pos
+        pos += n
+        r = remap[j]
+        r["ids"], r["n"] = cdesc[li]["ids"], n
+        r["id_shift"], r["sub_rows"] = cdesc[li]["id_shift"], cdesc[li]["sub_rows"]
+        r["row_base"], r["out_off"] = cdesc[li]["row_base"], col_items[li]
+        d = cdesc[li]
+        d["table"] = c.weight.data_ptr()
+        d["ids"] = self.ids_cache.data_ptr() + col_items[li] * idsz
+        d["id_shift"], d["row_base"], d["sub_rows"] = 0, 0, c.slots
+      t = tab.copy()
+      t[0]["rows"], t[0]["width"], t[0]["key_base"] = c.rows, c.width, 0
+      t[0]["weight"] = self._ptr(c.host_weight)
+      prefill = bool(src["offsets"].any())
+      self._cache_plan.append((m, _native.upload_struct_array(src, dev),
+                               _native.upload_struct_array(t, dev), len(src), pos, prefill,
+                               _native.upload_struct_array(remap, dev), len(remap),
+                               int(remap["n"].max())))
+
+  def _run_cache_pass(self, train: bool):
+    for m, descs, table, n_in, n_items, prefill, remap, n_remap, max_n in self._cache_plan:
+      c = self.caches[m]
+      self.ops.offload_cache_pass(c.tensors(), c.host_ptrs(), c.n_sets, c.n_spill, c.rows, descs,
+                                  table, n_in, self.B, self.ids64, n_items, prefill, remap,
+                                  n_remap, max_n, self.ids_cache.data_ptr(), bool(train))
+
+  def flush_offload_cache(self, invalidate: bool = False):
+    """Write every dirty cached row and its optimizer state back to the host tables (and, with
+    ``invalidate``, empty the caches).  Synchronises the device: the host tables are final when
+    this returns."""
+    if not self.caches:
+      return
+    for c in self.caches.values():
+      c.flush(self.ops)
+      if invalidate:
+        c.invalidate()
+    torch.cuda.synchronize(self.device)
+
+  def offload_cache_stats(self, reset: bool = True) -> Dict[int, Dict[str, int]]:
+    return {m: c.read_stats(reset) for m, c in self.caches.items()}
+
   def _upload(self):
     """(Re)upload descriptor arrays; table pointers / optimizer state may have changed."""
     dev = self.device
@@ -720,6 +829,13 @@ class FusedEngine:
     for m, layer in enumerate(self.mp_layers):
       t[m]["weight"] = self._ptr(_weight(layer))
       st = self.opt_state.get(m)
+      c = self.caches.get(m)
+      if c is not None:
+        if [s.data_ptr() for s in c.host_state] != [s.data_ptr() for s in st or []]:
+          c.invalidate()  # new host state (its old rows were flushed by reset_optimizer_state)
+          c.set_state(st or [])
+        t[m]["weight"] = c.weight.data_ptr()
+        st = c.state
       t[m]["state0"] = self._ptr(st[0]) if st else 0
       t[m]["state1"] = self._ptr(st[1]) if st and len(st) > 1 else 0
     self.tdesc = _native.upload_struct_array(t, self.device) if len(t) else None
@@ -731,6 +847,7 @@ class FusedEngine:
 
   # ------------------------------------------------------------------ optimizer state
   def reset_optimizer_state(self):
+    self.flush_offload_cache(invalidate=True)
     self.opt_state = {}
     opt = self.de._fused_optimizer
     if opt is None:
@@ -862,14 +979,16 @@ class FusedEngine:
     if self._tables_dirty:
       self._refresh_tables()
     weights = [_weight(l) for l in list(self.de.dp_layers) + self.mp_layers]
-    out = _FusedFn.apply(self, self._token, *weights)
+    # a forward that records a backward is a training pass: the cache marks its rows dirty
+    train = torch.is_grad_enabled() and any(w.requires_grad for w in weights)
+    out = _FusedFn.apply(self, self._token, train, *weights)
     if concat:
       return out
     return list(torch.split(out, self.out_widths, dim=1))
 
-  def _run_forward(self):
+  def _run_forward(self, train: bool = True):
     with nvtx.range("emb_forward"):
-      self.launch_forward()
+      self.launch_forward(train)
       self.wait_output()
       return self.out
 
@@ -883,8 +1002,9 @@ class FusedEngine:
     (``wait_output`` does it); a fused consumer can only fold the wait when this is False."""
     return self.rs_buf is not None
 
-  def launch_forward(self):
-    """Index exchange + lookups.  The pooled rows of this rank's tables are on their way to the
+  def launch_forward(self, train: bool = True):
+    """Index exchange + lookups.  ``train``: the step updates the tables after this forward (the
+    offload cache then marks the rows it serves dirty); False for a forward-only pass.  The pooled rows of this rank's tables are on their way to the
     requesters when this returns; the *consumer* of ``self.out`` must wait for the owners'
     "output ready" signals (:meth:`wait_output`, or ``sync_out_wait()`` folded into its kernel)."""
     ops, W, rank = self.ops, self.W, self.rank
@@ -907,6 +1027,14 @@ class FusedEngine:
         # requesters may only be overwritten once they are done with the previous step
         ops.sync_only(self._sync(signal=CH_IDS))
         wait_ids = CH_IDS
+    if self._cache_plan:
+      # the cache pass reads the arrived ids: it takes the "ids ready" wait, the lookups then
+      # run without one.  Its write-back of last step's rows is ordered behind last step's
+      # update by stream order (see DESIGN.md, offload cache)
+      if wait_ids >= 0:
+        ops.sync_only(self._sync(wait=wait_ids))
+        wait_ids = -1
+      self._run_cache_pass(train)
     if self.ddesc is not None:
       ops.lookup_fwd(self.ddesc, len(self.ddesc_np), lb, lb, lb, self.out_stride, [],
                      [self.out.data_ptr()], 0, self.ids64, self.act, self.vec4, [],
@@ -1095,6 +1223,9 @@ class FusedEngine:
         ops.sync_only(self._sync(wait=CH_GRAD, signal=CH_CONSUMED))
       return [None] * n_mp
     opt = de._fused_optimizer
+    if opt is None and self.caches:
+      raise RuntimeError("the offload cache updates its rows with the fused optimizer: call "
+                         "DistributedEmbedding.set_optimizer() before training a cached model")
     if opt is not None and opt["kind"] != "sgd" and not self.opt_state:
       self.reset_optimizer_state()
     if self._tables_dirty:

@@ -62,6 +62,11 @@ def parse():
   p.add_argument("--eval_batches", type=int, default=8,
                  help="eval batches per periodic evaluation (--eval_interval)")
   p.add_argument("--amp", action="store_true", default=True)
+  p.add_argument("--gpu_embedding_size", type=int, default=None,
+                 help="per-rank HBM element budget of the tables; the largest beyond it live in "
+                      "pinned host memory")
+  p.add_argument("--offload_cache_size", type=int, default=None,
+                 help="per-rank HBM element budget of the cache of the offloaded tables' rows")
   p.add_argument("--table_dtype", default="fp32", choices=sorted(TABLE_DTYPES),
                  help="storage of the model-parallel embedding tables (bf16 / fp16: half the "
                       "memory, stochastically rounded updates)")
@@ -108,6 +113,8 @@ def main():
                dist_strategy=args.dist_strategy, test_combiner=args.test_combiner, device=device,
                compute_dtype=torch.bfloat16 if (args.amp and cuda) else torch.float32,
                table_dtype=TABLE_DTYPES[args.table_dtype], interaction=args.interaction,
+               gpu_embedding_size=args.gpu_embedding_size,
+               offload_cache_size=args.offload_cache_size,
                dcn_num_layers=args.dcn_num_layers, dcn_low_rank_dim=args.dcn_low_rank_dim,
                multi_hot_sizes=hotness)
   table_ids = list(range(len(table_sizes))) if args.dp_input else \

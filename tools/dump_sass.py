@@ -54,6 +54,12 @@ HOT = [
     ("sgd_update", r"sgd_update_kernel"),
     ("dense_opt_adagrad", r"dense_opt_kernel<1>"),
     ("dense_opt_adam", r"dense_opt_kernel<3>"),
+    ("cache_spill_writeback", r"cache_spill_writeback_kernel"),
+    ("cache_probe", r"cache_probe_kernel"),
+    ("cache_assign", r"cache_assign_kernel"),
+    ("cache_fill", r"cache_fill_kernel"),
+    ("cache_remap_i32", r"cache_remap_kernel<int>"),
+    ("cache_flush", r"cache_flush_kernel"),
 ]
 
 

@@ -19,6 +19,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from distributed_embeddings_b200.models.configs import expand, synthetic_models_v3  # noqa: E402
 from distributed_embeddings_b200.models.dlrm import mlperf_table_sizes  # noqa: E402
+from distributed_embeddings_b200.parallel.offload_cache import cache_bytes, split_budget  # noqa: E402
 from distributed_embeddings_b200.parallel.strategy import (DistEmbeddingStrategy,  # noqa: E402
                                                            suggest_column_slice_threshold)
 
@@ -64,12 +65,23 @@ def main(argv=None):
                   help="storage of the model-parallel tables (DistributedEmbedding(table_dtype="
                        "...)): their table and gather bytes at its element size; optimizer slots "
                        "and replicated tables stay fp32")
+  ap.add_argument("--gpu-embedding-size", type=int, default=None,
+                  help="per-rank HBM element budget of the table-parallel tables; the largest "
+                       "beyond it go to pinned host memory")
+  ap.add_argument("--offload-cache-size", type=int, default=None,
+                  help="per-rank HBM element budget of the cache of the offloaded tables' rows "
+                       "(fp32 tables): its weight, optimizer-state and spill-region slots are "
+                       "reported as cache GiB and counted in HBM GiB")
   ap.add_argument("--json", action="store_true")
   args = ap.parse_args(argv)
 
   cfgs, imap, hots = model_tables(args)
+  if args.offload_cache_size is not None and (args.gpu_embedding_size is None or
+                                             args.table_dtype != "fp32"):
+    ap.error("--offload-cache-size needs --gpu-embedding-size and fp32 tables")
   kw = dict(input_table_map=imap, row_slice_threshold=_thr(args.row_slice_threshold),
-            data_parallel_threshold=_thr(args.data_parallel_threshold))
+            data_parallel_threshold=_thr(args.data_parallel_threshold),
+            gpu_embedding_size=args.gpu_embedding_size)
   cst = _thr(args.column_slice_threshold)
   if cst == "auto":
     cst = suggest_column_slice_threshold(cfgs, args.world, args.strategy, hotness=hots,
@@ -88,15 +100,35 @@ def main(argv=None):
     t = st.table_groups[0][st.map_groups[0][j]]
     dp_gather += args.global_batch // args.world * hot[gi] * int(st.global_configs[t]["output_dim"]) * 4
   ranks = []
+
+  def cache_gib(r):
+    """HBM of rank r's offload caches: the budget split like DistributedEmbedding splits it,
+    each table's spill region sized to its owner-side batch x hotness."""
+    if args.offload_cache_size is None or not st.table_groups[1]:
+      return 0.0
+    spill = {}
+    for li, g in enumerate(st.input_ids_list[r]):
+      m = st.local_maps[r][li]
+      if st.local_configs[r][m].get("cpu_offload"):
+        spill[m] = spill.get(m, 0) + args.global_batch * hot[st.input_groups[1][g]]
+    ms = sorted(spill)
+    shapes = [(int(st.local_configs[r][m]["input_dim"]), int(st.local_configs[r][m]["output_dim"]))
+              for m in ms]
+    sets = split_budget(args.offload_cache_size, shapes)
+    return sum(cache_bytes(n, spill[m], w, [w] * args.optimizer_slots)
+               for n, m, (_, w) in zip(sets, ms, shapes)) / 2**30
+
   for r in range(args.world):
     n_tab = len(st.local_configs[r]) if st.table_groups[1] else 0
     cols = sum(int(st.local_configs[r][m]["output_dim"]) for m in st.local_maps[r]) \
         if st.table_groups[1] else 0
-    gib = ((mem[r]["hbm_elements"] - dp_elems) * per_elem + dp_elems * per_elem_dp) / 2**30
+    cgib = cache_gib(r)
+    gib = ((mem[r]["hbm_elements"] - dp_elems) * per_elem + dp_elems * per_elem_dp) / 2**30 + cgib
     gather = (tr["ranks"][r]["gather_bytes"] - dp_gather) * esz / 4 + dp_gather
     ranks.append({"rank": r, "fused_tables": n_tab, "inputs": len(st.input_ids_list[r]),
                   "exchanged_columns": cols, "hbm_gib": round(gib, 2),
                   "host_gib": round(mem[r]["host_elements"] * per_elem / 2**30, 2),
+                  "cache_gib": round(cgib, 6),
                   "gather_mb": round(gather / 1e6, 1),
                   "nvlink_out_mb": round(tr["ranks"][r]["nvlink_out_bytes"] / 1e6, 1),
                   "lookups": int(tr["ranks"][r]["lookups"]),
@@ -114,11 +146,11 @@ def main(argv=None):
         f"column_slice_threshold {cst}, {args.table_dtype} tables: {rep['replicated']} replicated, "
         f"{rep['table_parallel']} table-parallel, {rep['row_sliced']} row-sliced")
   print(f"{'rank':>4} {'tables':>7} {'inputs':>7} {'columns':>8} {'HBM GiB':>9} {'host GiB':>9} "
-        f"{'gather MB':>10} {'NVLink out MB':>14} {'lookups':>12}")
+        f"{'cache GiB':>10} {'gather MB':>10} {'NVLink out MB':>14} {'lookups':>12}")
   for x in ranks:
     flag = "" if x["fits"] else f"   > {args.hbm_gib:g} GiB!"
     print(f"{x['rank']:>4} {x['fused_tables']:>7} {x['inputs']:>7} {x['exchanged_columns']:>8} "
-          f"{x['hbm_gib']:>9.2f} {x['host_gib']:>9.2f} {x['gather_mb']:>10.1f} "
+          f"{x['hbm_gib']:>9.2f} {x['host_gib']:>9.2f} {x['cache_gib']:>10.3f} {x['gather_mb']:>10.1f} "
           f"{x['nvlink_out_mb']:>14.1f} {x['lookups']:>12}{flag}")
   print(f"imbalance (max / mean): gather {rep['gather_imbalance']}, "
         f"NVLink {rep['nvlink_imbalance']}  (per step, global batch {args.global_batch})")
