@@ -356,9 +356,10 @@ void segment_update(const Tensor& descs, const Tensor& tables, int64_t n_tables,
                     double weight_decay, int64_t lr_ptr, const c10::optional<Tensor>& emit_keys,
                     const c10::optional<Tensor>& emit_rows, int64_t max_width, int64_t act_dtype,
                     bool vec4, const c10::optional<Tensor>& scratch, int64_t step_ptr,
-                    int64_t table_dtype) {
+                    int64_t table_dtype, int64_t state_dtype) {
   c10::cuda::CUDAGuard guard(descs.device());
   TORCH_CHECK(table_dtype >= 0 && table_dtype <= 2, "table_dtype: 0 fp32, 1 bf16, 2 fp16");
+  TORCH_CHECK(state_dtype == 0 || state_dtype == 1, "state_dtype: 0 fp32, 1 bf16");
   de::OptimizerArgs opt;
   opt.kind = static_cast<int32_t>(opt_kind);
   opt.lr = static_cast<float>(lr);
@@ -386,7 +387,8 @@ void segment_update(const Tensor& descs, const Tensor& tables, int64_t n_tables,
         reinterpret_cast<const uint32_t*>(sorted_items.data_ptr<int>()), n_items,
         seg_start.data_ptr<int64_t>(), n_unique.data_ptr<int64_t>(), opt,
         scratch->data_ptr<float>(), static_cast<int>(sw), static_cast<int>(max_width),
-        static_cast<int>(act_dtype), sm_count(), cur_stream(), static_cast<int>(table_dtype));
+        static_cast<int>(act_dtype), sm_count(), cur_stream(), static_cast<int>(table_dtype),
+        static_cast<int>(state_dtype));
     TORCH_CHECK(ok, "balanced update launch failed");
     check_launch();
     return;
@@ -399,7 +401,8 @@ void segment_update(const Tensor& descs, const Tensor& tables, int64_t n_tables,
       seg_start.data_ptr<int64_t>(), n_unique.data_ptr<int64_t>(), sorted_keys.numel(), opt,
       emit_keys.has_value() ? emit_keys->data_ptr<int64_t>() : nullptr,
       emit_rows.has_value() ? emit_rows->data_ptr<float>() : nullptr, static_cast<int>(max_width),
-      static_cast<int>(act_dtype), vec4, sm_count(), cur_stream(), static_cast<int>(table_dtype));
+      static_cast<int>(act_dtype), vec4, sm_count(), cur_stream(), static_cast<int>(table_dtype),
+      static_cast<int>(state_dtype));
   check_launch();
 }
 
@@ -535,7 +538,7 @@ std::tuple<Tensor, Tensor> embedding_lookup_grad(const Tensor& values,
   std::vector<int64_t> gp = {reinterpret_cast<int64_t>(grad.data_ptr())};
   segment_update(dd, td, 1, batch, batch, gstride, gp, std::get<0>(sorted), std::get<1>(sorted),
                  std::get<2>(sorted), std::get<3>(sorted), de::kOptEmit, 0, 0, 0, 0, 1, 1, 1.0, 0, 0,
-                 emit_keys, emit_rows, width, gdt, vec4, c10::nullopt, 0, 0);
+                 emit_keys, emit_rows, width, gdt, vec4, c10::nullopt, 0, 0, 0);
   // sizing the IndexedSlices-style result needs the unique count on the host (compat path only)
   int64_t n_unique = std::get<3>(sorted).item<int64_t>();
   if (n_unique > 0) {
@@ -1439,7 +1442,7 @@ TORCH_LIBRARY(de_b200, m) {
       "Tensor seg_start, Tensor n_unique, int opt_kind, float lr, float eps, float beta1, "
       "float beta2, float bias1, float bias2, float grad_scale, float weight_decay, int lr_ptr, "
       "Tensor? emit_keys, Tensor? emit_rows, int max_width, int act_dtype, bool vec4, "
-      "Tensor? scratch, int step_ptr, int table_dtype=0) -> ()",
+      "Tensor? scratch, int step_ptr, int table_dtype=0, int state_dtype=0) -> ()",
       &segment_update);
   m.def(
       "embedding_lookup_fwd(Tensor param, Tensor values, Tensor? offsets, int hotness, int batch, "

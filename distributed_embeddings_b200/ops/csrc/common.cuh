@@ -214,8 +214,10 @@ __device__ __forceinline__ FVec<VEC> ld_tab(const TabT* p) {
 //   u = (r >> 8) * 2^-24;  result = u * (hi - lo) < x - lo ? hi : lo
 // with every fp32 operation exact, so E[result] = x.  NaN / inf and values beyond the finite
 // range convert as round-to-nearest does.  r is a 32-bit hash of (optimizer step, row key,
-// column): the result does not depend on which thread stores the element, and the step counter
-// is device resident, so CUDA-graph replays draw fresh bits.
+// column, stream): the result does not depend on which thread stores the element, and the step
+// counter is device resident, so CUDA-graph replays draw fresh bits.  The stream separates the
+// stored quantities: 0 the weight, 1 state0 (Adagrad accumulator / Adam m), 2 state1 (Adam v);
+// it is folded into the step seed (step + 0x9e3779b9 + stream * 0x632be5ab).
 __device__ __forceinline__ uint32_t sr_mix(uint32_t h) {
   h ^= h >> 16;
   h *= 0x7feb352du;
@@ -224,8 +226,10 @@ __device__ __forceinline__ uint32_t sr_mix(uint32_t h) {
   h ^= h >> 16;
   return h;
 }
-__device__ __forceinline__ uint32_t sr_row_seed(uint32_t step, int64_t key) {
-  uint32_t h = sr_mix(step + 0x9e3779b9u);
+constexpr uint32_t kStreamWeight = 0, kStreamState0 = 1, kStreamState1 = 2;
+__device__ __forceinline__ uint32_t sr_row_seed(uint32_t step, int64_t key,
+                                                uint32_t stream = kStreamWeight) {
+  uint32_t h = sr_mix(step + 0x9e3779b9u + stream * 0x632be5abu);
   h = sr_mix(h ^ static_cast<uint32_t>(key));
   return sr_mix(h ^ static_cast<uint32_t>(static_cast<uint64_t>(key) >> 32));
 }
@@ -272,15 +276,15 @@ __device__ __forceinline__ FVec<VEC> ld_tab_rw(const TabT* p) {
   return ld_act<TabT, VEC>(p);
 }
 
-// Write-back of an updated row fragment: fp32 as is, 16-bit with stochastic rounding keyed by
-// (step, row key, column).
+// Write-back of an updated row fragment (weights and optimizer state): fp32 as is, 16-bit with
+// stochastic rounding keyed by (step, row key, column, stream).
 template <typename TabT, int VEC>
 __device__ __forceinline__ void st_tab(TabT* p, const FVec<VEC>& x, uint32_t step, int64_t key,
-                                       int col) {
+                                       int col, uint32_t stream = kStreamWeight) {
   if constexpr (sizeof(TabT) == 4) {
     st_f32<VEC>(reinterpret_cast<float*>(p), x);
   } else {
-    const uint32_t seed = sr_row_seed(step, key);
+    const uint32_t seed = sr_row_seed(step, key, stream);
     unsigned short b[VEC];
 #pragma unroll
     for (int i = 0; i < VEC; ++i) b[i] = round_stochastic<TabT>(x.v[i], sr_bits(seed, col + i));

@@ -82,7 +82,8 @@ enum OptimizerKind : int32_t { kOptSGD = 0, kOptAdagrad = 1, kOptRowwiseAdagrad 
 struct alignas(16) TableDesc {
   void* weight;       // [rows, width]; fp32, bf16 or fp16 (`table_dtype` of the launch)
   void* state0;       // Adagrad accumulator [rows,width] / row-wise [rows] / Adam m
-  void* state1;       // Adam v
+  void* state1;       // Adam v  (element-wise state: fp32 or bf16, `state_dtype` of the launch;
+                      // row-wise state is always fp32)
   int64_t rows;
   int64_t key_base;   // first global row key of this table (prefix sum of rows)
   int32_t width;
@@ -155,7 +156,10 @@ void launch_segment_update(const InputDesc* descs, const TableDesc* tables, int 
                            const uint32_t* sorted_items, const int64_t* seg_start,
                            const int64_t* n_unique, int64_t n_items, const OptimizerArgs& opt,
                            int64_t* emit_keys, float* emit_rows, int max_width, int act_dtype,
-                           bool vec4, int sm_count, cudaStream_t stream, int table_dtype = 0);
+                           bool vec4, int sm_count, cudaStream_t stream, int table_dtype = 0,
+                           int state_dtype = 0);
+// state_dtype: storage of the Adagrad accumulator / Adam moments, 0 = fp32, 1 = bf16 (widened
+// to fp32 for the update, stored with stochastic rounding; other optimizers ignore it).
 
 bool launch_balanced_update(const InputDesc* descs, const TableDesc* tables, int n_tables,
                             int64_t batch, int64_t grad_batch, int64_t grad_stride,
@@ -164,7 +168,7 @@ bool launch_balanced_update(const InputDesc* descs, const TableDesc* tables, int
                             const int64_t* seg_start, const int64_t* n_unique,
                             const OptimizerArgs& opt, float* scratch, int scratch_width,
                             int max_width, int act_dtype, int sm_count, cudaStream_t stream,
-                            int table_dtype = 0);
+                            int table_dtype = 0, int state_dtype = 0);
 
 // ---- HBM row cache of host-offloaded fp32 tables (offload_cache.cu) ------------------------
 // Slots [0, n_sets * 32) are the sets (32 ways each), [n_sets * 32, + n_spill) the spill region.

@@ -92,14 +92,14 @@ __device__ __forceinline__ void resolve_step(OptimizerArgs& opt) {
   }
 }
 
-// The step that keys the stochastic rounding of 16-bit tables: the same device-resident count
-// (fp32 tables do not use it, and their kernels never read it).  The count is an fp32 word that
-// advances by 1.0 per step, exact up to 2^24 = 16.7 M steps; beyond that it stops changing and
-// every later step would draw the same bits for a given (row, column), which biases the rounding.
-// Runs that long need an integer counter here.
-template <typename TabT>
+// The step that keys the stochastic rounding of 16-bit tables and 16-bit optimizer state: the
+// same device-resident count (kernels with fp32 tables and fp32 state do not use it and never
+// read it).  The count is an fp32 word that advances by 1.0 per step, exact up to 2^24 = 16.7 M
+// steps; beyond that it stops changing and every later step would draw the same bits for a given
+// (row, column), which biases the rounding.  Runs that long need an integer counter here.
+template <typename TabT, typename StateT>
 __device__ __forceinline__ uint32_t rounding_step(const OptimizerArgs& opt) {
-  if constexpr (sizeof(TabT) == 2) {
+  if constexpr (sizeof(TabT) == 2 || sizeof(StateT) == 2) {
     return opt.step_ptr != nullptr ? static_cast<uint32_t>(*opt.step_ptr) : 0u;
   } else {
     return 0u;
@@ -107,10 +107,12 @@ __device__ __forceinline__ uint32_t rounding_step(const OptimizerArgs& opt) {
 }
 
 // ------------------------------------------------------------------ per-row optimizer apply
-// The weight is read in its storage type (TabT: fp32, bf16 or fp16), the optimizer runs in fp32
-// on fp32 state, and a 16-bit weight is written back with stochastic rounding (st_tab).  Every
-// row has exactly one writer per step, so each element is rounded once.
-template <typename TabT, int VEC>
+// The weight is read in its storage type (TabT: fp32, bf16 or fp16) and the Adagrad / Adam state
+// in its own (StateT: fp32 or bf16), both widened to fp32; the optimizer runs in fp32, the weight
+// update uses the unrounded new state, and 16-bit weights and state are written back with
+// stochastic rounding (st_tab), each from its own random stream.  Every row has exactly one
+// writer per step, so each element is rounded once.  Row-wise Adagrad state is always fp32.
+template <typename TabT, int VEC, typename StateT = float>
 __device__ __forceinline__ void apply_update(const TableDesc& T, const OptimizerArgs& opt,
                                              int64_t row, int col, const FVec<VEC>& g,
                                              float row_sumsq_mean, uint32_t step) {
@@ -121,23 +123,23 @@ __device__ __forceinline__ void apply_update(const TableDesc& T, const Optimizer
   if (opt.kind == kOptSGD) {
     wv.fma(-opt.lr, gv);
   } else if (opt.kind == kOptAdagrad) {
-    float* a = reinterpret_cast<float*>(T.state0) + row * T.width + col;
-    FVec<VEC> av = ld_f32_rw<VEC>(a);
+    StateT* a = reinterpret_cast<StateT*>(T.state0) + row * T.width + col;
+    FVec<VEC> av = ld_tab_rw<StateT, VEC>(a);
 #pragma unroll
     for (int i = 0; i < VEC; ++i) {
       av.v[i] = fmaf(gv.v[i], gv.v[i], av.v[i]);
       wv.v[i] -= opt.lr * gv.v[i] / (sqrtf(av.v[i]) + opt.eps);
     }
-    st_f32<VEC>(a, av);
+    st_tab<StateT, VEC>(a, av, step, T.key_base + row, col, kStreamState0);
   } else if (opt.kind == kOptRowwiseAdagrad) {
     // state0[row] was already advanced by the caller; row_sumsq_mean carries the new value
     const float denom = sqrtf(row_sumsq_mean) + opt.eps;
 #pragma unroll
     for (int i = 0; i < VEC; ++i) wv.v[i] -= opt.lr * gv.v[i] / denom;
   } else if (opt.kind == kOptAdam) {
-    float* m = reinterpret_cast<float*>(T.state0) + row * T.width + col;
-    float* v = reinterpret_cast<float*>(T.state1) + row * T.width + col;
-    FVec<VEC> mv = ld_f32_rw<VEC>(m), vv = ld_f32_rw<VEC>(v);
+    StateT* m = reinterpret_cast<StateT*>(T.state0) + row * T.width + col;
+    StateT* v = reinterpret_cast<StateT*>(T.state1) + row * T.width + col;
+    FVec<VEC> mv = ld_tab_rw<StateT, VEC>(m), vv = ld_tab_rw<StateT, VEC>(v);
 #pragma unroll
     for (int i = 0; i < VEC; ++i) {
       mv.v[i] = opt.beta1 * mv.v[i] + (1.f - opt.beta1) * gv.v[i];
@@ -146,8 +148,8 @@ __device__ __forceinline__ void apply_update(const TableDesc& T, const Optimizer
       const float vh = vv.v[i] / opt.bias2;
       wv.v[i] -= opt.lr * mh / (sqrtf(vh) + opt.eps);
     }
-    st_f32<VEC>(m, mv);
-    st_f32<VEC>(v, vv);
+    st_tab<StateT, VEC>(m, mv, step, T.key_base + row, col, kStreamState0);
+    st_tab<StateT, VEC>(v, vv, step, T.key_base + row, col, kStreamState1);
   }
   st_tab<TabT, VEC>(w, wv, step, T.key_base + row, col);
 }
@@ -202,7 +204,7 @@ __device__ __forceinline__ FVec<VEC> reduce_segment(const InputDesc* __restrict_
   return acc;
 }
 
-template <typename GradT, int VEC, typename TabT>
+template <typename GradT, int VEC, typename TabT, typename StateT>
 __device__ __forceinline__ void segment_update_body(
     const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables, int n_tables,
     int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride, const PeerPtrs& grad,
@@ -213,7 +215,7 @@ __device__ __forceinline__ void segment_update_body(
   OptimizerArgs opt = opt_in;
   if (opt.lr_ptr != nullptr) opt.lr = *opt.lr_ptr;
   resolve_step(opt);
-  const uint32_t sr_step = rounding_step<TabT>(opt);
+  const uint32_t sr_step = rounding_step<TabT, StateT>(opt);
   const int64_t n_unique = *n_unique_p;
   const int64_t sentinel = tables[n_tables - 1].key_base + tables[n_tables - 1].rows;
   const int lane = threadIdx.x & 31;
@@ -283,7 +285,7 @@ __device__ __forceinline__ void segment_update_body(
       if (opt.kind == kOptEmit) {
         st_f32<VEC>(emit_rows + u * emit_width + col, g);
       } else {
-        apply_update<TabT, VEC>(T, opt, row, col, g, row_state, sr_step);
+        apply_update<TabT, VEC, StateT>(T, opt, row, col, g, row_state, sr_step);
       }
     }
   }
@@ -297,7 +299,7 @@ __global__ void __launch_bounds__(kThreads) segment_update_kernel(const InputDes
     const uint32_t* __restrict__ sorted_items, const int64_t* __restrict__ seg_start,
     const int64_t* __restrict__ n_unique_p, const __grid_constant__ OptimizerArgs opt_in,
     int64_t* __restrict__ emit_keys, float* __restrict__ emit_rows, int emit_width) {
-  segment_update_body<GradT, VEC, float>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
+  segment_update_body<GradT, VEC, float, float>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
                                      sorted_keys, sorted_items, seg_start, n_unique_p, opt_in,
                                      emit_keys, emit_rows, emit_width);
 }
@@ -310,7 +312,20 @@ __global__ void __launch_bounds__(kThreads) segment_update_tab16_kernel(const In
     const uint32_t* __restrict__ sorted_items, const int64_t* __restrict__ seg_start,
     const int64_t* __restrict__ n_unique_p, const __grid_constant__ OptimizerArgs opt_in,
     int64_t* __restrict__ emit_keys, float* __restrict__ emit_rows, int emit_width) {
-  segment_update_body<GradT, VEC, TabT>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
+  segment_update_body<GradT, VEC, TabT, float>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
+                                     sorted_keys, sorted_items, seg_start, n_unique_p, opt_in,
+                                     emit_keys, emit_rows, emit_width);
+}
+
+// fp32, bf16 or fp16 tables (TabT) with bf16 Adagrad / Adam state
+template <typename GradT, int VEC, typename TabT>
+__global__ void __launch_bounds__(kThreads) segment_update_bf16state_kernel(const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables,
+    int n_tables, int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
+    const __grid_constant__ PeerPtrs grad, const int64_t* __restrict__ sorted_keys,
+    const uint32_t* __restrict__ sorted_items, const int64_t* __restrict__ seg_start,
+    const int64_t* __restrict__ n_unique_p, const __grid_constant__ OptimizerArgs opt_in,
+    int64_t* __restrict__ emit_keys, float* __restrict__ emit_rows, int emit_width) {
+  segment_update_body<GradT, VEC, TabT, __nv_bfloat16>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
                                      sorted_keys, sorted_items, seg_start, n_unique_p, opt_in,
                                      emit_keys, emit_rows, emit_width);
 }
@@ -370,7 +385,7 @@ __device__ __forceinline__ int find_table(const TableDesc* __restrict__ tables, 
 }
 
 // Apply the optimizer to one row given the complete (scaled) gradient fragment of this lane.
-template <typename TabT>
+template <typename TabT, typename StateT>
 __device__ __forceinline__ void apply_row(const TableDesc& T, const OptimizerArgs& opt,
                                           int64_t row, int col, FVec<4> g, int lpr,
                                           unsigned group_mask, uint32_t step) {
@@ -388,10 +403,10 @@ __device__ __forceinline__ void apply_row(const TableDesc& T, const OptimizerArg
     __syncwarp(group_mask);
     if (col == 0) *st = row_state;
   }
-  if (col_ok) apply_update<TabT, 4>(T, opt, row, col, g, row_state, step);
+  if (col_ok) apply_update<TabT, 4, StateT>(T, opt, row, col, g, row_state, step);
 }
 
-template <typename GradT, typename TabT>
+template <typename GradT, typename TabT, typename StateT>
 __device__ __forceinline__ void balanced_update_body(
     const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables, int n_tables,
     int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride, const PeerPtrs& grad,
@@ -401,7 +416,7 @@ __device__ __forceinline__ void balanced_update_body(
   OptimizerArgs opt = opt_in;
   if (opt.lr_ptr != nullptr) opt.lr = *opt.lr_ptr;
   resolve_step(opt);
-  const uint32_t sr_step = rounding_step<TabT>(opt);
+  const uint32_t sr_step = rounding_step<TabT, StateT>(opt);
   const int64_t n_unique = *n_unique_p;
   const int64_t sentinel = tables[n_tables - 1].key_base + tables[n_tables - 1].rows;
   const int lane = threadIdx.x & 31;
@@ -453,7 +468,7 @@ __device__ __forceinline__ void balanced_update_body(
             FVec<4> g = acc;
             g.scale(opt.grad_scale);
             if (start_done) {
-              apply_row<TabT>(T, opt, run_key - T.key_base, col, g, lpr, group_mask, sr_step);
+              apply_row<TabT, StateT>(T, opt, run_key - T.key_base, col, g, lpr, group_mask, sr_step);
             } else if (col < T.width) {
               // continues a segment that started in an earlier chunk: that chunk owns the slot
               const int64_t s = segment_start_of(seg_start, n_unique, k0);
@@ -476,7 +491,7 @@ __device__ __forceinline__ void balanced_update_body(
       FVec<4> g = acc;
       g.scale(opt.grad_scale);
       if (start_done && end_done) {
-        apply_row<TabT>(T, opt, run_key - T.key_base, col, g, lpr, group_mask, sr_step);
+        apply_row<TabT, StateT>(T, opt, run_key - T.key_base, col, g, lpr, group_mask, sr_step);
       } else if (col < T.width) {
         const int64_t s = start_done ? run_start : segment_start_of(seg_start, n_unique, k0);
         red_add_f32<4>(scratch + (s / kChunk) * scratch_width + col, g);
@@ -494,7 +509,7 @@ __global__ void __launch_bounds__(kThreads) balanced_update_kernel(const InputDe
     const uint32_t* __restrict__ sorted_items, int64_t n_items,
     const int64_t* __restrict__ seg_start, const int64_t* __restrict__ n_unique_p,
     const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch, int scratch_width) {
-  balanced_update_body<GradT, float>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
+  balanced_update_body<GradT, float, float>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
                                     sorted_keys, sorted_items, n_items, seg_start, n_unique_p,
                                     opt_in, scratch, scratch_width);
 }
@@ -506,12 +521,24 @@ __global__ void __launch_bounds__(kThreads) balanced_update_tab16_kernel(const I
     const uint32_t* __restrict__ sorted_items, int64_t n_items,
     const int64_t* __restrict__ seg_start, const int64_t* __restrict__ n_unique_p,
     const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch, int scratch_width) {
-  balanced_update_body<GradT, TabT>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
+  balanced_update_body<GradT, TabT, float>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
                                     sorted_keys, sorted_items, n_items, seg_start, n_unique_p,
                                     opt_in, scratch, scratch_width);
 }
 
-template <typename TabT>
+template <typename GradT, typename TabT>
+__global__ void __launch_bounds__(kThreads) balanced_update_bf16state_kernel(const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables,
+    int n_tables, int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
+    const __grid_constant__ PeerPtrs grad, const int64_t* __restrict__ sorted_keys,
+    const uint32_t* __restrict__ sorted_items, int64_t n_items,
+    const int64_t* __restrict__ seg_start, const int64_t* __restrict__ n_unique_p,
+    const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch, int scratch_width) {
+  balanced_update_body<GradT, TabT, __nv_bfloat16>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
+                                    sorted_keys, sorted_items, n_items, seg_start, n_unique_p,
+                                    opt_in, scratch, scratch_width);
+}
+
+template <typename TabT, typename StateT>
 __device__ __forceinline__ void finalize_crossing_body(
     const TableDesc* __restrict__ tables, int n_tables, int lpr,
     const int64_t* __restrict__ sorted_keys, int64_t n_items, const OptimizerArgs& opt_in,
@@ -519,7 +546,7 @@ __device__ __forceinline__ void finalize_crossing_body(
   OptimizerArgs opt = opt_in;
   if (opt.lr_ptr != nullptr) opt.lr = *opt.lr_ptr;
   resolve_step(opt);
-  const uint32_t sr_step = rounding_step<TabT>(opt);
+  const uint32_t sr_step = rounding_step<TabT, StateT>(opt);
   const int64_t sentinel = tables[n_tables - 1].key_base + tables[n_tables - 1].rows;
   const int lane = threadIdx.x & 31;
   const int rpw = 32 / lpr;
@@ -549,7 +576,7 @@ __device__ __forceinline__ void finalize_crossing_body(
       z.zero();
       st_f32<4>(sp, z);
     }
-    apply_row<TabT>(T, opt, key - T.key_base, col, g, lpr, group_mask, sr_step);
+    apply_row<TabT, StateT>(T, opt, key - T.key_base, col, g, lpr, group_mask, sr_step);
   }
 }
 
@@ -558,7 +585,7 @@ finalize_crossing_kernel(const TableDesc* __restrict__ tables, int n_tables, int
                          const int64_t* __restrict__ sorted_keys, int64_t n_items,
                          const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch,
                          int scratch_width) {
-  finalize_crossing_body<float>(tables, n_tables, lpr, sorted_keys, n_items, opt_in, scratch, scratch_width);
+  finalize_crossing_body<float, float>(tables, n_tables, lpr, sorted_keys, n_items, opt_in, scratch, scratch_width);
 }
 
 template <typename TabT>
@@ -567,7 +594,16 @@ finalize_crossing_tab16_kernel(const TableDesc* __restrict__ tables, int n_table
                          const int64_t* __restrict__ sorted_keys, int64_t n_items,
                          const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch,
                          int scratch_width) {
-  finalize_crossing_body<TabT>(tables, n_tables, lpr, sorted_keys, n_items, opt_in, scratch, scratch_width);
+  finalize_crossing_body<TabT, float>(tables, n_tables, lpr, sorted_keys, n_items, opt_in, scratch, scratch_width);
+}
+
+template <typename TabT>
+__global__ void __launch_bounds__(kThreads)
+finalize_crossing_bf16state_kernel(const TableDesc* __restrict__ tables, int n_tables, int lpr,
+                         const int64_t* __restrict__ sorted_keys, int64_t n_items,
+                         const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch,
+                         int scratch_width) {
+  finalize_crossing_body<TabT, __nv_bfloat16>(tables, n_tables, lpr, sorted_keys, n_items, opt_in, scratch, scratch_width);
 }
 
 int grid_cap(int64_t work_warps, int sm_count, int per_sm) {
@@ -639,7 +675,7 @@ void unique_segments(void* temp, size_t temp_bytes, const int64_t* sorted_keys, 
   finish_segments_kernel<<<1, 32, 0, stream>>>(seg_start, n_unique, n);
 }
 
-template <typename GradT, int VEC, typename TabT>
+template <typename GradT, int VEC, typename TabT, typename StateT>
 static void launch_seg(int grid, cudaStream_t stream, const InputDesc* descs,
                        const TableDesc* tables, int n_tables, int lpr, int64_t batch,
                        int64_t grad_batch, int64_t grad_stride, const PeerPtrs& grad,
@@ -647,7 +683,11 @@ static void launch_seg(int grid, cudaStream_t stream, const InputDesc* descs,
                        const int64_t* seg_start, const int64_t* n_unique,
                        const OptimizerArgs& opt, int64_t* emit_keys, float* emit_rows,
                        int emit_width) {
-  if constexpr (std::is_same<TabT, float>::value)
+  if constexpr (!std::is_same<StateT, float>::value)
+    segment_update_bf16state_kernel<GradT, VEC, TabT><<<grid, kThreads, 0, stream>>>(
+        descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
+        sorted_items, seg_start, n_unique, opt, emit_keys, emit_rows, emit_width);
+  else if constexpr (std::is_same<TabT, float>::value)
     segment_update_kernel<GradT, VEC><<<grid, kThreads, 0, stream>>>(
         descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
         sorted_items, seg_start, n_unique, opt, emit_keys, emit_rows, emit_width);
@@ -656,20 +696,20 @@ static void launch_seg(int grid, cudaStream_t stream, const InputDesc* descs,
         descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
         sorted_items, seg_start, n_unique, opt, emit_keys, emit_rows, emit_width);
 }
-#define DE_DISPATCH_SEG(GradT, VEC, TabT)                                                      \
-  launch_seg<GradT, VEC, TabT>(grid, stream, descs, tables, n_tables, lpr, batch, grad_batch,  \
+#define DE_DISPATCH_SEG(GradT, VEC, TabT, StateT)                                              \
+  launch_seg<GradT, VEC, TabT, StateT>(grid, stream, descs, tables, n_tables, lpr, batch, grad_batch,  \
                                grad_stride, grad, sorted_keys, sorted_items, seg_start,        \
                                n_unique, opt, emit_keys, emit_rows, emit_width)
-#define DE_DISPATCH_SEG_G(VEC, TabT)                                                           \
+#define DE_DISPATCH_SEG_G(VEC, TabT, StateT)                                                   \
   do {                                                                                         \
-    if (act_dtype == 1) DE_DISPATCH_SEG(__nv_bfloat16, VEC, TabT);                             \
-    else if (act_dtype == 2) DE_DISPATCH_SEG(__half, VEC, TabT);                               \
-    else DE_DISPATCH_SEG(float, VEC, TabT);                                                    \
+    if (act_dtype == 1) DE_DISPATCH_SEG(__nv_bfloat16, VEC, TabT, StateT);                     \
+    else if (act_dtype == 2) DE_DISPATCH_SEG(__half, VEC, TabT, StateT);                       \
+    else DE_DISPATCH_SEG(float, VEC, TabT, StateT);                                            \
   } while (0)
-#define DE_DISPATCH_SEG_V(TabT)                                                                \
+#define DE_DISPATCH_SEG_V(TabT, StateT)                                                        \
   do {                                                                                         \
-    if (vec4) DE_DISPATCH_SEG_G(4, TabT);                                                      \
-    else DE_DISPATCH_SEG_G(1, TabT);                                                           \
+    if (vec4) DE_DISPATCH_SEG_G(4, TabT, StateT);                                              \
+    else DE_DISPATCH_SEG_G(1, TabT, StateT);                                                   \
   } while (0)
 
 void launch_segment_update(const InputDesc* descs, const TableDesc* tables, int n_tables,
@@ -678,7 +718,8 @@ void launch_segment_update(const InputDesc* descs, const TableDesc* tables, int 
                            const uint32_t* sorted_items, const int64_t* seg_start,
                            const int64_t* n_unique, int64_t n_items, const OptimizerArgs& opt,
                            int64_t* emit_keys, float* emit_rows, int max_width, int act_dtype,
-                           bool vec4, int sm_count, cudaStream_t stream, int table_dtype) {
+                           bool vec4, int sm_count, cudaStream_t stream, int table_dtype,
+                           int state_dtype) {
   const int emit_width = max_width;
   if (n_items <= 0 || n_tables <= 0) return;
   // lanes per row from the widest table of this launch (narrower tables leave lanes idle)
@@ -692,13 +733,18 @@ void launch_segment_update(const InputDesc* descs, const TableDesc* tables, int 
   const int rpw = 32 / lpr;
   const int64_t warps = (n_items + rpw - 1) / rpw;
   const int grid = grid_cap(warps, sm_count, 8);
-  // the emit path never touches the table: one instantiation serves every storage type
-  if (table_dtype == 1 && opt.kind != kOptEmit) DE_DISPATCH_SEG_V(__nv_bfloat16);
-  else if (table_dtype == 2 && opt.kind != kOptEmit) DE_DISPATCH_SEG_V(__half);
-  else DE_DISPATCH_SEG_V(float);
+  // the emit path never touches the table: one instantiation serves every storage type; only
+  // Adagrad and Adam read element-wise state, every other optimizer takes the fp32-state kernels
+  if (state_dtype == 1 && (opt.kind == kOptAdagrad || opt.kind == kOptAdam)) {
+    if (table_dtype == 1) DE_DISPATCH_SEG_V(__nv_bfloat16, __nv_bfloat16);
+    else if (table_dtype == 2) DE_DISPATCH_SEG_V(__half, __nv_bfloat16);
+    else DE_DISPATCH_SEG_V(float, __nv_bfloat16);
+  } else if (table_dtype == 1 && opt.kind != kOptEmit) DE_DISPATCH_SEG_V(__nv_bfloat16, float);
+  else if (table_dtype == 2 && opt.kind != kOptEmit) DE_DISPATCH_SEG_V(__half, float);
+  else DE_DISPATCH_SEG_V(float, float);
 }
 
-template <typename GradT, typename TabT>
+template <typename GradT, typename TabT, typename StateT>
 static void launch_balanced_g(const InputDesc* descs, const TableDesc* tables, int n_tables,
                               int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
                               const PeerPtrs& grad, const int64_t* sorted_keys,
@@ -706,7 +752,11 @@ static void launch_balanced_g(const InputDesc* descs, const TableDesc* tables, i
                               const int64_t* seg_start, const int64_t* n_unique,
                               const OptimizerArgs& opt, float* scratch, int scratch_width,
                               int grid, cudaStream_t stream) {
-  if constexpr (std::is_same<TabT, float>::value)
+  if constexpr (!std::is_same<StateT, float>::value)
+    balanced_update_bf16state_kernel<GradT, TabT><<<grid, kThreads, 0, stream>>>(
+        descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
+        sorted_items, n_items, seg_start, n_unique, opt, scratch, scratch_width);
+  else if constexpr (std::is_same<TabT, float>::value)
     balanced_update_kernel<GradT><<<grid, kThreads, 0, stream>>>(
         descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
         sorted_items, n_items, seg_start, n_unique, opt, scratch, scratch_width);
@@ -716,7 +766,7 @@ static void launch_balanced_g(const InputDesc* descs, const TableDesc* tables, i
         sorted_items, n_items, seg_start, n_unique, opt, scratch, scratch_width);
 }
 
-template <typename TabT>
+template <typename TabT, typename StateT>
 static void launch_balanced(const InputDesc* descs, const TableDesc* tables, int n_tables, int lpr,
                             int64_t batch, int64_t grad_batch, int64_t grad_stride,
                             const PeerPtrs& grad, const int64_t* sorted_keys,
@@ -725,19 +775,22 @@ static void launch_balanced(const InputDesc* descs, const TableDesc* tables, int
                             const OptimizerArgs& opt, float* scratch, int scratch_width,
                             int act_dtype, int grid, cudaStream_t stream) {
   if (act_dtype == 1)
-    launch_balanced_g<__nv_bfloat16, TabT>(descs, tables, n_tables, lpr, batch, grad_batch,
+    launch_balanced_g<__nv_bfloat16, TabT, StateT>(descs, tables, n_tables, lpr, batch, grad_batch,
                                            grad_stride, grad, sorted_keys, sorted_items, n_items,
                                            seg_start, n_unique, opt, scratch, scratch_width, grid,
                                            stream);
   else if (act_dtype == 2)
-    launch_balanced_g<__half, TabT>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride,
+    launch_balanced_g<__half, TabT, StateT>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride,
                                     grad, sorted_keys, sorted_items, n_items, seg_start, n_unique,
                                     opt, scratch, scratch_width, grid, stream);
   else
-    launch_balanced_g<float, TabT>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride,
+    launch_balanced_g<float, TabT, StateT>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride,
                                    grad, sorted_keys, sorted_items, n_items, seg_start, n_unique,
                                    opt, scratch, scratch_width, grid, stream);
-  if constexpr (std::is_same<TabT, float>::value)
+  if constexpr (!std::is_same<StateT, float>::value)
+    finalize_crossing_bf16state_kernel<TabT><<<grid, kThreads, 0, stream>>>(
+        tables, n_tables, lpr, sorted_keys, n_items, opt, scratch, scratch_width);
+  else if constexpr (std::is_same<TabT, float>::value)
     finalize_crossing_kernel<<<grid, kThreads, 0, stream>>>(tables, n_tables, lpr, sorted_keys,
                                                             n_items, opt, scratch, scratch_width);
   else
@@ -755,7 +808,7 @@ bool launch_balanced_update(const InputDesc* descs, const TableDesc* tables, int
                             const int64_t* seg_start, const int64_t* n_unique,
                             const OptimizerArgs& opt, float* scratch, int scratch_width,
                             int max_width, int act_dtype, int sm_count, cudaStream_t stream,
-                            int table_dtype) {
+                            int table_dtype, int state_dtype) {
   if (n_items <= 0 || n_tables <= 0) return true;
   if (max_width > 128 || max_width % 4 || scratch_width % 4 || opt.kind == kOptEmit) return false;
   int lpr = 1;
@@ -763,18 +816,22 @@ bool launch_balanced_update(const InputDesc* descs, const TableDesc* tables, int
   const int rpw = 32 / lpr;
   const int64_t n_chunks = (n_items + kChunk - 1) / kChunk;
   const int grid = grid_cap((n_chunks + rpw - 1) / rpw, sm_count, 8);
-  if (table_dtype == 1)
-    launch_balanced<__nv_bfloat16>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride,
-                                   grad, sorted_keys, sorted_items, n_items, seg_start, n_unique,
-                                   opt, scratch, scratch_width, act_dtype, grid, stream);
-  else if (table_dtype == 2)
-    launch_balanced<__half>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
-                            sorted_keys, sorted_items, n_items, seg_start, n_unique, opt, scratch,
-                            scratch_width, act_dtype, grid, stream);
-  else
-    launch_balanced<float>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
-                           sorted_keys, sorted_items, n_items, seg_start, n_unique, opt, scratch,
-                           scratch_width, act_dtype, grid, stream);
+#define DE_BAL(TabT, StateT)                                                                   \
+  launch_balanced<TabT, StateT>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, \
+                                grad, sorted_keys, sorted_items, n_items, seg_start, n_unique, \
+                                opt, scratch, scratch_width, act_dtype, grid, stream)
+  if (state_dtype == 1 && (opt.kind == kOptAdagrad || opt.kind == kOptAdam)) {
+    if (table_dtype == 1) DE_BAL(__nv_bfloat16, __nv_bfloat16);
+    else if (table_dtype == 2) DE_BAL(__half, __nv_bfloat16);
+    else DE_BAL(float, __nv_bfloat16);
+  } else if (table_dtype == 1) {
+    DE_BAL(__nv_bfloat16, float);
+  } else if (table_dtype == 2) {
+    DE_BAL(__half, float);
+  } else {
+    DE_BAL(float, float);
+  }
+#undef DE_BAL
   return cudaGetLastError() == cudaSuccess;
 }
 

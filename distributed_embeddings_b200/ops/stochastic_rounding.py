@@ -13,9 +13,22 @@ The rule is defined once and implemented twice, here and in ``ops/csrc/common.cu
 * otherwise ``u = (r >> 8) * 2**-24`` and the result is ``hi`` if ``u * (hi - lo) < x - lo``,
   else ``lo``.  Every fp32 operation of that comparison is exact.
 * NaN, +-inf and values beyond the finite range of the target convert as round-to-nearest does.
-* ``r`` is a 32-bit hash of (optimizer step, row key, column), see :func:`random_bits`.  The row
-  key of the fused back end is the row's position in the rank's sorted-update key space (the
-  fused local table's ``key_base`` plus the row), of :class:`SparseRowOptimizer` the row index.
+* ``r`` is a 32-bit hash of (optimizer step, row key, column, stream), see :func:`random_bits`.
+  The row key of the fused back end is the row's position in the rank's sorted-update key space
+  (the fused local table's ``key_base`` plus the row), of :class:`SparseRowOptimizer` the row
+  index.
+
+Half-precision optimizer state (``set_optimizer(..., state_dtype=torch.bfloat16)``) is stored
+with the same rule.  Each stored quantity draws from its own stream of the hash, so the rounding
+decisions of a weight and of its state are independent:
+
+* stream 0: the weight (the bits of half-precision tables, unchanged by the streams);
+* stream 1: ``state0`` (the Adagrad accumulator, Adam's ``m``);
+* stream 2: ``state1`` (Adam's ``v``).
+
+The stream is folded into the step seed: ``mix((step + 0x9E3779B9 + stream * 0x632BE5AB) mod
+2**32)``.  Two streams draw the same bits only at step offsets of about 1.7e9, far beyond the
+2**24 steps the fp32 step counter counts exactly.
 """
 from __future__ import annotations
 
@@ -37,14 +50,33 @@ def _mix(h: np.ndarray) -> np.ndarray:
   return h ^ (h >> np.uint64(16))
 
 
-def random_bits(step: int, keys, cols) -> np.ndarray:
-  """``r`` of every (row key, column): ``keys`` and ``cols`` broadcast against each other."""
+STREAM_WEIGHT, STREAM_STATE0, STREAM_STATE1 = 0, 1, 2
+
+
+def random_bits(step: int, keys, cols, stream: int = STREAM_WEIGHT) -> np.ndarray:
+  """``r`` of every (row key, column) of ``stream``: ``keys`` and ``cols`` broadcast against each
+  other."""
   keys = np.asarray(keys, dtype=np.int64).view(np.uint64)
   cols = np.asarray(cols, dtype=np.int64).astype(np.uint64) & _M32
-  h = _mix(np.asarray((int(step) + 0x9E3779B9) & 0xFFFFFFFF, dtype=np.uint64))
+  seed = (int(step) + 0x9E3779B9 + int(stream) * 0x632BE5AB) & 0xFFFFFFFF
+  h = _mix(np.asarray(seed, dtype=np.uint64))
   h = _mix(h ^ (keys & _M32))
   h = _mix(h ^ (keys >> np.uint64(32)))
   return _mix(h ^ cols).astype(np.uint32)
+
+
+def check_state_dtype(kind: str, state_dtype: torch.dtype) -> torch.dtype:
+  """Validate the storage dtype of an optimizer's per-element state; returns it."""
+  if state_dtype not in (torch.float32, torch.bfloat16):
+    raise ValueError(
+        f"optimizer state_dtype must be torch.float32 or torch.bfloat16, not {state_dtype} "
+        "(fp16 cannot hold it: an Adagrad accumulator can pass 65504 and Adam's v underflows)")
+  if state_dtype == torch.bfloat16 and kind == "sgd":
+    raise ValueError("state_dtype=torch.bfloat16 needs an optimizer with state: sgd has none")
+  if state_dtype == torch.bfloat16 and kind == "rowwise_adagrad":
+    raise ValueError("state_dtype=torch.bfloat16 does not apply to rowwise_adagrad: its one "
+                     "fp32 word per row stays fp32")
+  return state_dtype
 
 
 def _ordered(bits: np.ndarray) -> np.ndarray:
@@ -81,9 +113,11 @@ def stochastic_round_bits(x: np.ndarray, dtype: torch.dtype, r: np.ndarray) -> n
 
 
 def stochastic_round(x: torch.Tensor, dtype: torch.dtype, step: int,
-                     keys: Union[torch.Tensor, np.ndarray, int], col0: int = 0) -> torch.Tensor:
+                     keys: Union[torch.Tensor, np.ndarray, int], col0: int = 0,
+                     stream: int = STREAM_WEIGHT) -> torch.Tensor:
   """Round fp32 rows ``x`` (``[..., width]``) into ``dtype``; ``keys`` (``[...]``) are the row
-  keys, columns count from ``col0``.  Returns a CPU tensor of ``dtype`` and ``x``'s shape."""
+  keys, columns count from ``col0``, ``stream`` selects the random stream (see the module
+  docstring).  Returns a CPU tensor of ``dtype`` and ``x``'s shape."""
   if dtype not in HALF_DTYPES:
     raise ValueError(f"stochastic rounding targets bf16 or fp16, not {dtype}")
   xs = x.detach().to("cpu", torch.float32).contiguous().numpy()
@@ -91,7 +125,7 @@ def stochastic_round(x: torch.Tensor, dtype: torch.dtype, step: int,
     keys = keys.detach().cpu().numpy()
   width = xs.shape[-1] if xs.ndim else 1
   cols = np.arange(col0, col0 + width, dtype=np.int64)
-  r = random_bits(step, np.asarray(keys, dtype=np.int64)[..., None], cols)
+  r = random_bits(step, np.asarray(keys, dtype=np.int64)[..., None], cols, stream)
   r = np.broadcast_to(r, xs.shape)
   bits = stochastic_round_bits(xs, dtype, r)
   return torch.from_numpy(bits.view(np.int16).copy()).view(dtype)

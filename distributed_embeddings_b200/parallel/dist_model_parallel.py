@@ -27,6 +27,7 @@ from torch import nn
 from ..layers.embedding import Embedding, config_from_layer
 from ..ops import embedding_lookup_ops as elo
 from ..ops.ragged import RaggedIds, SparseIds
+from ..ops.stochastic_rounding import check_state_dtype
 from ..utils import initializers
 from .comm import dist_ready
 from .strategy import DistEmbeddingStrategy, STRATEGIES, suggest_column_slice_threshold
@@ -595,13 +596,21 @@ class DistributedEmbedding(nn.Module):
   def set_optimizer(self, kind: str = "sgd", lr: float = 0.01, **kwargs):
     """Attach an optimizer that is applied to the model-parallel tables *inside* the backward
     kernels (no sparse gradient is materialised).  ``kind``: ``sgd`` | ``adagrad`` |
-    ``rowwise_adagrad`` | ``adam``.  Only the fused back end consumes it."""
+    ``rowwise_adagrad`` | ``adam``.  Only the fused back end consumes it.
+
+    ``state_dtype``: storage of the Adagrad accumulator / Adam moments, ``torch.float32``
+    (default) or ``torch.bfloat16`` (half the bytes; the update runs in fp32 and stores the state
+    with stochastic rounding, see the user guide, "Half-precision optimizer state")."""
     kind = kind.lower()
     if kind not in ("sgd", "adagrad", "rowwise_adagrad", "adam"):
       raise ValueError(f"Unsupported fused optimizer {kind}")
+    state_dtype = check_state_dtype(kind, kwargs.pop("state_dtype", torch.float32))
+    if state_dtype != torch.float32 and self.offload_cache_size is not None:
+      raise ValueError("state_dtype=torch.bfloat16 is not supported with offload_cache_size: the "
+                       "HBM row cache keeps optimizer state rows as fp32 words")
     cfg = {"kind": kind, "lr": float(lr), "eps": 1e-7 if kind != "adam" else 1e-8,
            "beta1": 0.9, "beta2": 0.999, "weight_decay": 0.0, "initial_accumulator_value": 0.1,
-           "deterministic": kind != "sgd", "step": 0}
+           "deterministic": kind != "sgd", "step": 0, "state_dtype": state_dtype}
     cfg.update(kwargs)
     self._fused_optimizer = cfg
     if self._engine is not None:
@@ -925,10 +934,12 @@ class DistributedEmbedding(nn.Module):
                 for t in range(len(self.strategy.global_configs))]
     return {"kind": kind, "step": eng.step_count(), "tables": tables}
 
-  def set_optimizer_state(self, state: Dict[str, Any]):
+  def set_optimizer_state(self, state: Dict[str, Any], chunk: int = 134217728):
     """Load a state produced by :meth:`get_optimizer_state` (any sharding) - every rank passes
     the same global arrays and keeps its slices, like :meth:`set_weights`.  The older per-rank
-    format of ``FusedEngine.optimizer_state_dict`` is still accepted."""
+    format of ``FusedEngine.optimizer_state_dict`` is still accepted.  Element-wise state is
+    copied in pieces of at most ``chunk`` elements and converted to the state's storage dtype
+    (bf16 state: round to nearest)."""
     if self._engine is None:
       raise RuntimeError("run a forward pass (or build the engine) before loading optimizer state")
     eng = self._engine
@@ -950,14 +961,21 @@ class DistributedEmbedding(nn.Module):
         for s in st.shards[self.rank] if st.table_groups[1] else []:
           t = st.table_groups[1][s.table]
           for k, arr in enumerate(tables[t]):
-            dst = eng.opt_state[s.local_table][k][s.row_offset:s.row_offset + s.rows]
-            src = np.asarray(arr)[:, 0] if per_row else np.asarray(arr)[:, s.col_start:s.col_end]
-            dst.copy_(torch.from_numpy(np.array(src, dtype=np.float32)))
+            dst = eng.opt_state[s.local_table][k]
+            if per_row:
+              dst[s.row_offset:s.row_offset + s.rows].copy_(
+                  torch.from_numpy(np.array(np.asarray(arr)[:, 0], dtype=np.float32)))
+            else:
+              self._assign_chunked(dst, s.row_offset, np.asarray(arr)[:, s.col_start:s.col_end],
+                                   chunk)
         for gt, t in enumerate(st.table_groups[2]):
           lo, hi = st.row_ranges[gt][self.rank]
           for k, arr in enumerate(tables[t]):
-            src = np.asarray(arr)[lo:hi, 0] if per_row else np.asarray(arr)[lo:hi]
-            eng.opt_state[n_col + gt][k].copy_(torch.from_numpy(np.array(src, dtype=np.float32)))
+            dst = eng.opt_state[n_col + gt][k]
+            if per_row:
+              dst.copy_(torch.from_numpy(np.array(np.asarray(arr)[lo:hi, 0], dtype=np.float32)))
+            else:
+              self._assign_chunked(dst, 0, np.asarray(arr)[lo:hi], chunk)
     step = int(state.get("step", 0))
     eng.step_t.fill_(float(step))
     self._fused_optimizer["step"] = step
@@ -1028,9 +1046,9 @@ class DistributedEmbedding(nn.Module):
     self._barrier()
     return meta_path
 
-  def load_optimizer_state(self, directory: str):
+  def load_optimizer_state(self, directory: str, chunk: int = 134217728):
     """Load what :meth:`save_optimizer_state` wrote (any world size / sharding); the arrays stay
-    memory mapped, every rank reads only its slices."""
+    memory mapped, every rank reads only its slices, ``chunk`` elements at a time."""
     import json  # pylint: disable=import-outside-toplevel
     with open(os.path.join(directory, "optimizer.json"), encoding="utf-8") as f:
       meta = json.load(f)
@@ -1038,7 +1056,8 @@ class DistributedEmbedding(nn.Module):
     for t, has in enumerate(meta["tables"]):
       tables.append([np.load(os.path.join(directory, f"opt_{t}_slot{k}.npy"), mmap_mode="r")
                      for k in range(int(meta["slots"]))] if has else None)
-    self.set_optimizer_state({"kind": meta["kind"], "step": int(meta["step"]), "tables": tables})
+    self.set_optimizer_state({"kind": meta["kind"], "step": int(meta["step"]), "tables": tables},
+                             chunk=chunk)
 
   def close(self):
     """Release the fused engine's peer-mapped buffers (collective over the process group).

@@ -32,7 +32,7 @@ import numpy as np
 import torch
 
 from ..ops._native import GRAD_ROUTE, INPUT_DESC, MAX_PEERS, TABLE_DESC
-from ..ops.stochastic_rounding import stochastic_round
+from ..ops.stochastic_rounding import STREAM_STATE0, STREAM_STATE1, stochastic_round
 from . import fused as _fused
 
 
@@ -502,10 +502,18 @@ class DryOps:
   def segment_update(self, descs, tables, n_tables, batch, grad_batch, grad_stride, grad_ptrs,
                      keys, items, seg, n_unique, kind, lr, eps, beta1, beta2, bias1, bias2,
                      grad_scale, weight_decay, lr_ptr, emit_keys, emit_rows, max_width, act_dtype,
-                     vec4, scratch, step_ptr, table_dtype=0):
+                     vec4, scratch, step_ptr, table_dtype=0, state_dtype=0):
     self._count("segment_update")
     tdt = self._ADT[int(table_dtype)]
     tsz = 4 if int(table_dtype) == 0 else 2
+    # Adagrad / Adam state in bf16: widened to fp32 for the update, stored with stochastic
+    # rounding (streams 1 and 2); the other optimizers ignore the code, like the kernels
+    half_state = int(state_dtype) == 1 and kind in (1, 3)
+    sdt, ssz = (torch.bfloat16, 2) if half_state else (torch.float32, 4)
+
+    def state(ptr, row, width, what):
+      t = self.world.tensor(int(ptr) + row * width * ssz, sdt, width, what)
+      return (t, t.float()) if half_state else (t, t)
     step = 0
     # the kernels take the optimizer constants in fp32 and form 1 - beta and the bias
     # corrections in fp32 from them
@@ -566,19 +574,24 @@ class DryOps:
       if kind == 0:
         wt -= lr * g
       elif kind == 1:
-        a = self.world.tensor(int(t["state0"]) + row * width * 4, torch.float32, width, "state0")
+        a16, a = state(t["state0"], row, width, "state0")
         a += g * g
         wt -= lr * g / (a.sqrt() + eps)
+        if half_state:
+          a16.copy_(stochastic_round(a, sdt, step, key, stream=STREAM_STATE0))
       elif kind == 2:
         a = self.world.tensor(int(t["state0"]) + row * 4, torch.float32, 1, "row state")
         a += (g * g).sum() / width
         wt -= lr * g / (a.sqrt() + eps)
       elif kind == 3:
-        mm = self.world.tensor(int(t["state0"]) + row * width * 4, torch.float32, width, "adam m")
-        vv = self.world.tensor(int(t["state1"]) + row * width * 4, torch.float32, width, "adam v")
+        m16, mm = state(t["state0"], row, width, "adam m")
+        v16, vv = state(t["state1"], row, width, "adam v")
         mm.mul_(beta1).add_(float(np.float32(1) - np.float32(beta1)) * g)
         vv.mul_(beta2).add_(float(np.float32(1) - np.float32(beta2)) * g * g)
         wt -= lr * (mm / bias1) / ((vv / bias2).sqrt() + eps)
+        if half_state:
+          m16.copy_(stochastic_round(mm, sdt, step, key, stream=STREAM_STATE0))
+          v16.copy_(stochastic_round(vv, sdt, step, key, stream=STREAM_STATE1))
       else:
         raise ValueError(f"optimizer kind {kind}")
       if tsz == 2:

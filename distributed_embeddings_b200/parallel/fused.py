@@ -855,20 +855,29 @@ class FusedEngine:
     kind = opt["kind"]
     self.step_t.fill_(float(opt.get("step", 0)))
 
-    def like(w, value, shape=None):
-      t = torch.full(shape or tuple(w.shape), value, dtype=torch.float32, device=w.device)
+    sdt = self.state_dtype
+
+    def like(w, value, shape=None, dtype=torch.float32):
+      # (a bf16 initial value is the round-to-nearest of ``value``)
+      t = torch.full(shape or tuple(w.shape), value, dtype=dtype, device=w.device)
       # state of offloaded tables stays on the host (pinned, read zero-copy by the kernels)
       return t.pin_memory() if not (w.is_cuda or self.dry) else t
 
     for m, layer in enumerate(self.mp_layers):
       w = _weight(layer)
       if kind == "adagrad":
-        self.opt_state[m] = [like(w, opt["initial_accumulator_value"])]
+        self.opt_state[m] = [like(w, opt["initial_accumulator_value"], dtype=sdt)]
       elif kind == "rowwise_adagrad":
         self.opt_state[m] = [like(w, opt["initial_accumulator_value"], (w.shape[0],))]
       elif kind == "adam":
-        self.opt_state[m] = [like(w, 0.0), like(w, 0.0)]
+        self.opt_state[m] = [like(w, 0.0, dtype=sdt), like(w, 0.0, dtype=sdt)]
     self._tables_dirty = True
+
+  @property
+  def state_dtype(self) -> torch.dtype:
+    """Storage of the element-wise optimizer state (Adagrad accumulator, Adam moments)."""
+    opt = self.de._fused_optimizer
+    return opt.get("state_dtype", torch.float32) if opt is not None else torch.float32
 
   def update_lr(self, lr: float):
     self.lr_t.fill_(lr)
@@ -1264,7 +1273,7 @@ class FusedEngine:
                          opt["eps"], opt["beta1"], opt["beta2"], 1.0, 1.0, gscale,
                          opt["weight_decay"], self.lr_t.data_ptr(), None, None, self.max_width,
                          self.act, self.vec4, self._balanced_scratch(), self.step_t.data_ptr(),
-                         self.tab)
+                         self.tab, DTYPE_CODE[self.state_dtype])
       if multi:
         ops.sync_only(self._sync(signal=CH_CONSUMED))
       return [None] * n_mp

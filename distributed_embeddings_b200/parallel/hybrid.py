@@ -18,7 +18,8 @@ import torch
 import torch.distributed as dist
 from torch import nn
 
-from ..ops.stochastic_rounding import HALF_DTYPES, stochastic_round
+from ..ops.stochastic_rounding import (HALF_DTYPES, STREAM_STATE0, STREAM_STATE1,
+                                       check_state_dtype, stochastic_round)
 from .comm import CommContext, dist_ready
 from .dist_model_parallel import _is_mp, broadcast_variables
 
@@ -262,14 +263,20 @@ class SparseRowOptimizer:
 
   bf16 / fp16 parameters keep fp32 state; their touched rows are updated in fp32 and written
   back with stochastic rounding keyed by (step, row, column), the rule of the fused kernels
-  (``ops/stochastic_rounding.py``)."""
+  (``ops/stochastic_rounding.py``).
+
+  ``state_dtype=torch.bfloat16`` stores the Adagrad accumulator / Adam moments in bf16 like the
+  fused back end: the touched rows' state is widened to fp32, the update runs in fp32 with the
+  unrounded new state, and the state is stored with stochastic rounding (streams 1 and 2)."""
 
   def __init__(self, params: Sequence[nn.Parameter], kind: str = "sgd", lr: float = 0.01,
                eps: Optional[float] = None, beta1: float = 0.9, beta2: float = 0.999,
-               initial_accumulator_value: float = 0.1, weight_decay: float = 0.0):
+               initial_accumulator_value: float = 0.1, weight_decay: float = 0.0,
+               state_dtype: torch.dtype = torch.float32):
     kind = kind.lower()
     if kind not in ("sgd", "adagrad", "rowwise_adagrad", "adam"):
       raise ValueError(f"Unsupported optimizer {kind}")
+    self.state_dtype = check_state_dtype(kind, state_dtype)
     self.params = [p for p in params if p.requires_grad]
     self.kind, self.lr = kind, float(lr)
     self.eps = (1e-8 if kind == "adam" else 1e-7) if eps is None else eps
@@ -278,13 +285,14 @@ class SparseRowOptimizer:
     self.state = []
     for p in self.params:
       sdt = torch.float32 if p.dtype in HALF_DTYPES else p.dtype  # half tables: fp32 state
+      esdt = torch.bfloat16 if self.state_dtype == torch.bfloat16 else sdt  # element-wise state
       if kind == "adagrad":
-        self.state.append([torch.full_like(p, initial_accumulator_value, dtype=sdt)])
+        self.state.append([torch.full_like(p, initial_accumulator_value, dtype=esdt)])
       elif kind == "rowwise_adagrad":
         self.state.append([torch.full((p.shape[0],), initial_accumulator_value, dtype=sdt,
                                       device=p.device)])
       elif kind == "adam":
-        self.state.append([torch.zeros_like(p, dtype=sdt), torch.zeros_like(p, dtype=sdt)])
+        self.state.append([torch.zeros_like(p, dtype=esdt), torch.zeros_like(p, dtype=esdt)])
       else:
         self.state.append([])
 
@@ -304,7 +312,7 @@ class SparseRowOptimizer:
       else:
         idx = torch.arange(p.shape[0], device=p.device)
         val = g.to(p.dtype)
-      if p.dtype in HALF_DTYPES:
+      if p.dtype in HALF_DTYPES or self.state_dtype != torch.float32:
         self._step_half(p, st, idx, val.float())
         p.grad = None
         continue
@@ -330,25 +338,37 @@ class SparseRowOptimizer:
       p.grad = None
 
   def _step_half(self, p, st, idx, val):
-    """fp32 update of the rows ``idx`` of a bf16 / fp16 table, stochastically rounded back."""
+    """fp32 update of the rows ``idx`` of a bf16 / fp16 table or of a table with bf16 state;
+    16-bit values are stochastically rounded back."""
     w = p[idx].float()
     if self.weight_decay:
       val = val + self.weight_decay * w
     if self.kind == "sgd":
       w = w - self.lr * val
     elif self.kind == "adagrad":
-      acc = st[0][idx] + val * val
-      st[0][idx] = acc
+      acc = st[0][idx].float() + val * val
+      self._store_state(st[0], idx, acc, STREAM_STATE0)
       w = w - self.lr * val / (acc.sqrt() + self.eps)
     elif self.kind == "rowwise_adagrad":
       acc = st[0][idx] + (val * val).mean(dim=1)
       st[0][idx] = acc
       w = w - self.lr * val / (acc.sqrt().unsqueeze(1) + self.eps)
     else:
-      m = self.beta1 * st[0][idx] + (1 - self.beta1) * val
-      v = self.beta2 * st[1][idx] + (1 - self.beta2) * val * val
-      st[0][idx], st[1][idx] = m, v
+      m = self.beta1 * st[0][idx].float() + (1 - self.beta1) * val
+      v = self.beta2 * st[1][idx].float() + (1 - self.beta2) * val * val
+      self._store_state(st[0], idx, m, STREAM_STATE0)
+      self._store_state(st[1], idx, v, STREAM_STATE1)
       b1 = 1 - self.beta1**self.step_count
       b2 = 1 - self.beta2**self.step_count
       w = w - self.lr * (m / b1) / ((v / b2).sqrt() + self.eps)
-    p[idx] = stochastic_round(w, p.dtype, self.step_count, idx).to(p.device)
+    if p.dtype in HALF_DTYPES:
+      p[idx] = stochastic_round(w, p.dtype, self.step_count, idx).to(p.device)
+    else:
+      p[idx] = w
+
+  def _store_state(self, s, idx, x, stream):
+    """Store fp32 state rows ``x`` at ``idx``: as is, or stochastically rounded into bf16."""
+    if s.dtype in HALF_DTYPES:
+      s[idx] = stochastic_round(x, s.dtype, self.step_count, idx, stream=stream).to(s.device)
+    else:
+      s[idx] = x

@@ -51,6 +51,9 @@ def main():
   p.add_argument("--amp", action="store_true", help="bf16 activations / MLP")
   p.add_argument("--table_dtype", default="fp32", choices=["bf16", "fp16", "fp32"],
                  help="storage of the model-parallel embedding tables (--embedding_api de)")
+  p.add_argument("--optimizer_state_dtype", default="fp32", choices=["fp32", "bf16"],
+                 help="storage of the Adagrad / Adam state of the model-parallel tables "
+                      "(--embedding_api de; bf16: half the memory, stochastically rounded)")
   p.add_argument("--backend", default="auto", choices=["auto", "fused", "torch"])
   p.add_argument("--row_scale", type=float, default=1.0, help="shrink tables (smoke runs)")
   p.add_argument("--device", default=None)
@@ -99,6 +102,8 @@ def main():
 
   if args.embedding_api == "de":
     lr = {"sgd": 0.03, "adagrad": 0.001, "rowwise_adagrad": 0.001, "adam": 0.001}[args.optimizer]
+    opt_kwargs = {"state_dtype": {"fp32": torch.float32,
+                                  "bf16": torch.bfloat16}[args.optimizer_state_dtype]}
     from distributed_embeddings_b200.models.synthetic_fast import SyntheticTrainStep
     why = SyntheticTrainStep.unsupported_reason(model) if use_cuda else "needs CUDA"
     if args.trainer == "fast" and why:
@@ -106,12 +111,14 @@ def main():
     if args.trainer != "autograd" and not why:
       trainer = SyntheticTrainStep(model, lr=lr, embedding_optimizer=args.optimizer,
                                    use_cuda_graph=bool(args.cuda_graph),
-                                   dense_optimizer=args.dense_optimizer)
+                                   dense_optimizer=args.dense_optimizer,
+                                   embedding_optimizer_kwargs=opt_kwargs)
       trainer_kind = "fast"
     else:
       trainer = HybridTrainer(model, lr=lr, embedding_optimizer=args.optimizer,
                               use_cuda_graph=bool(args.cuda_graph) and use_cuda,
-                              dense_optimizer=args.dense_optimizer)
+                              dense_optimizer=args.dense_optimizer,
+                              embedding_optimizer_kwargs=opt_kwargs)
       trainer_kind = "autograd"
     step = lambda num, cat, lab: trainer.step(num, cat, lab)
   else:

@@ -31,6 +31,7 @@ from distributed_embeddings_b200.utils.metrics import binary_auc
 
 
 TABLE_DTYPES = {"fp32": torch.float32, "bf16": torch.bfloat16, "fp16": torch.float16}
+STATE_DTYPES = {"fp32": torch.float32, "bf16": torch.bfloat16}
 
 
 def parse():
@@ -70,6 +71,11 @@ def parse():
   p.add_argument("--table_dtype", default="fp32", choices=sorted(TABLE_DTYPES),
                  help="storage of the model-parallel embedding tables (bf16 / fp16: half the "
                       "memory, stochastically rounded updates)")
+  p.add_argument("--embedding_optimizer", default="sgd", choices=["sgd", "adagrad", "adam"],
+                 help="fused optimizer of the model-parallel tables")
+  p.add_argument("--optimizer_state_dtype", default="fp32", choices=["fp32", "bf16"],
+                 help="storage of the Adagrad / Adam state of the model-parallel tables (bf16: "
+                      "half the memory, stochastically rounded)")
   p.add_argument("--warmup_steps", type=int, default=8000)
   p.add_argument("--decay_start_step", type=int, default=48000)
   p.add_argument("--decay_steps", type=int, default=24000)
@@ -139,18 +145,23 @@ def main():
                                 decay_steps=args.decay_steps)
   de.broadcast_variables(model)
   fast = args.fast and cuda and args.dp_input
+  opt_kwargs = {"state_dtype": STATE_DTYPES[args.optimizer_state_dtype]}
   if args.eval_interval > 0 and not fast:
     raise SystemExit("--eval_interval needs the hand-scheduled step: --fast with --dp_input on "
                      "a GPU")
   if fast:
     from distributed_embeddings_b200.models.dlrm_fast import DLRMTrainStep
-    trainer = DLRMTrainStep(model, lr=args.learning_rate, scheduler=sched)
+    trainer = DLRMTrainStep(model, lr=args.learning_rate, scheduler=sched,
+                            embedding_optimizer=args.embedding_optimizer,
+                            embedding_optimizer_kwargs=opt_kwargs)
     if args.interaction == "dcnv2":  # list of [b, h_f] ids
       step = lambda n, c, l: trainer.step(n, [x.to(torch.int32) for x in c], l)
     else:
       step = lambda n, c, l: trainer.step(n, torch.stack([x.to(torch.int32) for x in c]), l)
   else:
-    trainer = HybridTrainer(model, lr=args.learning_rate, scheduler=sched)
+    trainer = HybridTrainer(model, lr=args.learning_rate, scheduler=sched,
+                            embedding_optimizer=args.embedding_optimizer,
+                            embedding_optimizer_kwargs=opt_kwargs)
     step = trainer.step
 
   def batches():

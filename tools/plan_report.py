@@ -60,7 +60,10 @@ def main(argv=None):
   ap.add_argument("--global-batch", type=int, default=65536)
   ap.add_argument("--hbm-gib", type=float, default=79.0, help="per-GPU memory to check against")
   ap.add_argument("--optimizer-slots", type=int, default=0,
-                  help="fp32 state copies per table element (adagrad 1, adam 2)")
+                  help="state copies per table element (adagrad 1, adam 2)")
+  ap.add_argument("--state-dtype", default="fp32", choices=["fp32", "bf16"],
+                  help="storage of the Adagrad / Adam state of the model-parallel tables "
+                       "(set_optimizer(state_dtype=...)); replicated tables stay fp32")
   ap.add_argument("--table-dtype", default="fp32", choices=["fp32", "bf16", "fp16"],
                   help="storage of the model-parallel tables (DistributedEmbedding(table_dtype="
                        "...)): their table and gather bytes at its element size; optimizer slots "
@@ -79,6 +82,8 @@ def main(argv=None):
   if args.offload_cache_size is not None and (args.gpu_embedding_size is None or
                                              args.table_dtype != "fp32"):
     ap.error("--offload-cache-size needs --gpu-embedding-size and fp32 tables")
+  if args.offload_cache_size is not None and args.state_dtype != "fp32":
+    ap.error("--offload-cache-size needs fp32 optimizer state")
   kw = dict(input_table_map=imap, row_slice_threshold=_thr(args.row_slice_threshold),
             data_parallel_threshold=_thr(args.data_parallel_threshold),
             gpu_embedding_size=args.gpu_embedding_size)
@@ -91,7 +96,8 @@ def main(argv=None):
   mem = st.memory_report()
   tr = st.traffic_report(args.global_batch, hots)
   esz = 4 if args.table_dtype == "fp32" else 2
-  per_elem = esz + 4 * args.optimizer_slots       # model-parallel tables
+  ssz = 4 if args.state_dtype == "fp32" else 2
+  per_elem = esz + ssz * args.optimizer_slots     # model-parallel tables
   per_elem_dp = 4 * (1 + args.optimizer_slots)    # replicated tables are always fp32
   dp_elems = sum(int(c["input_dim"]) * int(c["output_dim"]) for c in st.dp_configs)
   hot = hots or [1] * len(st.input_table_map)
@@ -134,7 +140,7 @@ def main(argv=None):
                   "lookups": int(tr["ranks"][r]["lookups"]),
                   "fits": gib <= args.hbm_gib})
   rep = {"world": args.world, "strategy": args.strategy, "column_slice_threshold": cst,
-         "table_dtype": args.table_dtype,
+         "table_dtype": args.table_dtype, "state_dtype": args.state_dtype,
          "tables": len(cfgs), "replicated": len(st.table_groups[0]),
          "table_parallel": len(st.table_groups[1]), "row_sliced": len(st.table_groups[2]),
          "gather_imbalance": round(tr["gather_imbalance"], 3),
@@ -143,7 +149,8 @@ def main(argv=None):
     print(json.dumps(rep))
     return rep
   print(f"{len(cfgs)} tables on {args.world} ranks, strategy {args.strategy}, "
-        f"column_slice_threshold {cst}, {args.table_dtype} tables: {rep['replicated']} replicated, "
+        f"column_slice_threshold {cst}, {args.table_dtype} tables, {args.state_dtype} state: "
+        f"{rep['replicated']} replicated, "
         f"{rep['table_parallel']} table-parallel, {rep['row_sliced']} row-sliced")
   print(f"{'rank':>4} {'tables':>7} {'inputs':>7} {'columns':>8} {'HBM GiB':>9} {'host GiB':>9} "
         f"{'cache GiB':>10} {'gather MB':>10} {'NVLink out MB':>14} {'lookups':>12}")
