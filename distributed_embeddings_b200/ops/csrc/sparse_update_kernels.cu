@@ -204,7 +204,11 @@ __device__ __forceinline__ FVec<VEC> reduce_segment(const InputDesc* __restrict_
   return acc;
 }
 
-template <typename GradT, int VEC, typename TabT, typename StateT>
+// kRowDecay: row-wise Adagrad with weight decay.  Its accumulator takes the row mean of the
+// squared decayed gradient (s * g + weight_decay * w), the gradient apply_update applies, so pass 1
+// reads the weights.  Those launches get kernels of their own: the other kernels keep their code
+// and registers.
+template <typename GradT, int VEC, typename TabT, typename StateT, bool kRowDecay = false>
 __device__ __forceinline__ void segment_update_body(
     const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables, int n_tables,
     int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride, const PeerPtrs& grad,
@@ -254,10 +258,20 @@ __device__ __forceinline__ void segment_update_body(
           if (cv < nvec) {
             FVec<VEC> g = reduce_segment<GradT, VEC>(descs, sorted_items, k0, k1, batch,
                                                      grad_batch, grad_stride, grad, cv * VEC);
+            if constexpr (kRowDecay) {
+              // the same fp32 operations as apply_update, so the same values
+              g.scale(opt.grad_scale);
+              g.fma(opt.weight_decay,
+                    ld_tab_rw<TabT, VEC>(reinterpret_cast<const TabT*>(T.weight) + row * W +
+                                         cv * VEC));
 #pragma unroll
-            for (int i = 0; i < VEC; ++i) {
-              const float x = g.v[i] * opt.grad_scale;
-              ss = fmaf(x, x, ss);
+              for (int i = 0; i < VEC; ++i) ss = fmaf(g.v[i], g.v[i], ss);
+            } else {
+#pragma unroll
+              for (int i = 0; i < VEC; ++i) {
+                const float x = g.v[i] * opt.grad_scale;
+                ss = fmaf(x, x, ss);
+              }
             }
           }
         }
@@ -313,6 +327,19 @@ __global__ void __launch_bounds__(kThreads) segment_update_tab16_kernel(const In
     const int64_t* __restrict__ n_unique_p, const __grid_constant__ OptimizerArgs opt_in,
     int64_t* __restrict__ emit_keys, float* __restrict__ emit_rows, int emit_width) {
   segment_update_body<GradT, VEC, TabT, float>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
+                                     sorted_keys, sorted_items, seg_start, n_unique_p, opt_in,
+                                     emit_keys, emit_rows, emit_width);
+}
+
+// row-wise Adagrad with weight decay on fp32, bf16 or fp16 tables (TabT)
+template <typename GradT, int VEC, typename TabT>
+__global__ void __launch_bounds__(kThreads) segment_update_rowwise_decay_kernel(const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables,
+    int n_tables, int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
+    const __grid_constant__ PeerPtrs grad, const int64_t* __restrict__ sorted_keys,
+    const uint32_t* __restrict__ sorted_items, const int64_t* __restrict__ seg_start,
+    const int64_t* __restrict__ n_unique_p, const __grid_constant__ OptimizerArgs opt_in,
+    int64_t* __restrict__ emit_keys, float* __restrict__ emit_rows, int emit_width) {
+  segment_update_body<GradT, VEC, TabT, float, true>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
                                      sorted_keys, sorted_items, seg_start, n_unique_p, opt_in,
                                      emit_keys, emit_rows, emit_width);
 }
@@ -385,7 +412,8 @@ __device__ __forceinline__ int find_table(const TableDesc* __restrict__ tables, 
 }
 
 // Apply the optimizer to one row given the complete (scaled) gradient fragment of this lane.
-template <typename TabT, typename StateT>
+// kRowDecay: row-wise Adagrad with weight decay (see segment_update_body).
+template <typename TabT, typename StateT, bool kRowDecay = false>
 __device__ __forceinline__ void apply_row(const TableDesc& T, const OptimizerArgs& opt,
                                           int64_t row, int col, FVec<4> g, int lpr,
                                           unsigned group_mask, uint32_t step) {
@@ -394,8 +422,17 @@ __device__ __forceinline__ void apply_row(const TableDesc& T, const OptimizerArg
   if (opt.kind == kOptRowwiseAdagrad) {
     float ss = 0.f;
     if (col_ok) {
+      if constexpr (kRowDecay) {
+        // the accumulator takes the gradient apply_update applies: g + weight_decay * w
+        FVec<4> gd = g;
+        gd.fma(opt.weight_decay,
+               ld_tab_rw<TabT, 4>(reinterpret_cast<const TabT*>(T.weight) + row * T.width + col));
 #pragma unroll
-      for (int i = 0; i < 4; ++i) ss = fmaf(g.v[i], g.v[i], ss);
+        for (int i = 0; i < 4; ++i) ss = fmaf(gd.v[i], gd.v[i], ss);
+      } else {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) ss = fmaf(g.v[i], g.v[i], ss);
+      }
     }
     for (int off = lpr >> 1; off > 0; off >>= 1) ss += __shfl_xor_sync(group_mask, ss, off);
     float* st = reinterpret_cast<float*>(T.state0) + row;
@@ -406,7 +443,7 @@ __device__ __forceinline__ void apply_row(const TableDesc& T, const OptimizerArg
   if (col_ok) apply_update<TabT, 4, StateT>(T, opt, row, col, g, row_state, step);
 }
 
-template <typename GradT, typename TabT, typename StateT>
+template <typename GradT, typename TabT, typename StateT, bool kRowDecay = false>
 __device__ __forceinline__ void balanced_update_body(
     const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables, int n_tables,
     int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride, const PeerPtrs& grad,
@@ -468,7 +505,7 @@ __device__ __forceinline__ void balanced_update_body(
             FVec<4> g = acc;
             g.scale(opt.grad_scale);
             if (start_done) {
-              apply_row<TabT, StateT>(T, opt, run_key - T.key_base, col, g, lpr, group_mask, sr_step);
+              apply_row<TabT, StateT, kRowDecay>(T, opt, run_key - T.key_base, col, g, lpr, group_mask, sr_step);
             } else if (col < T.width) {
               // continues a segment that started in an earlier chunk: that chunk owns the slot
               const int64_t s = segment_start_of(seg_start, n_unique, k0);
@@ -491,7 +528,7 @@ __device__ __forceinline__ void balanced_update_body(
       FVec<4> g = acc;
       g.scale(opt.grad_scale);
       if (start_done && end_done) {
-        apply_row<TabT, StateT>(T, opt, run_key - T.key_base, col, g, lpr, group_mask, sr_step);
+        apply_row<TabT, StateT, kRowDecay>(T, opt, run_key - T.key_base, col, g, lpr, group_mask, sr_step);
       } else if (col < T.width) {
         const int64_t s = start_done ? run_start : segment_start_of(seg_start, n_unique, k0);
         red_add_f32<4>(scratch + (s / kChunk) * scratch_width + col, g);
@@ -526,6 +563,19 @@ __global__ void __launch_bounds__(kThreads) balanced_update_tab16_kernel(const I
                                     opt_in, scratch, scratch_width);
 }
 
+// row-wise Adagrad with weight decay on fp32, bf16 or fp16 tables (TabT)
+template <typename GradT, typename TabT>
+__global__ void __launch_bounds__(kThreads) balanced_update_rowwise_decay_kernel(const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables,
+    int n_tables, int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
+    const __grid_constant__ PeerPtrs grad, const int64_t* __restrict__ sorted_keys,
+    const uint32_t* __restrict__ sorted_items, int64_t n_items,
+    const int64_t* __restrict__ seg_start, const int64_t* __restrict__ n_unique_p,
+    const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch, int scratch_width) {
+  balanced_update_body<GradT, TabT, float, true>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
+                                    sorted_keys, sorted_items, n_items, seg_start, n_unique_p,
+                                    opt_in, scratch, scratch_width);
+}
+
 template <typename GradT, typename TabT>
 __global__ void __launch_bounds__(kThreads) balanced_update_bf16state_kernel(const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables,
     int n_tables, int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
@@ -538,7 +588,7 @@ __global__ void __launch_bounds__(kThreads) balanced_update_bf16state_kernel(con
                                     opt_in, scratch, scratch_width);
 }
 
-template <typename TabT, typename StateT>
+template <typename TabT, typename StateT, bool kRowDecay = false>
 __device__ __forceinline__ void finalize_crossing_body(
     const TableDesc* __restrict__ tables, int n_tables, int lpr,
     const int64_t* __restrict__ sorted_keys, int64_t n_items, const OptimizerArgs& opt_in,
@@ -576,7 +626,7 @@ __device__ __forceinline__ void finalize_crossing_body(
       z.zero();
       st_f32<4>(sp, z);
     }
-    apply_row<TabT, StateT>(T, opt, key - T.key_base, col, g, lpr, group_mask, sr_step);
+    apply_row<TabT, StateT, kRowDecay>(T, opt, key - T.key_base, col, g, lpr, group_mask, sr_step);
   }
 }
 
@@ -595,6 +645,15 @@ finalize_crossing_tab16_kernel(const TableDesc* __restrict__ tables, int n_table
                          const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch,
                          int scratch_width) {
   finalize_crossing_body<TabT, float>(tables, n_tables, lpr, sorted_keys, n_items, opt_in, scratch, scratch_width);
+}
+
+template <typename TabT>
+__global__ void __launch_bounds__(kThreads)
+finalize_crossing_rowwise_decay_kernel(const TableDesc* __restrict__ tables, int n_tables, int lpr,
+                         const int64_t* __restrict__ sorted_keys, int64_t n_items,
+                         const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch,
+                         int scratch_width) {
+  finalize_crossing_body<TabT, float, true>(tables, n_tables, lpr, sorted_keys, n_items, opt_in, scratch, scratch_width);
 }
 
 template <typename TabT>
@@ -682,9 +741,13 @@ static void launch_seg(int grid, cudaStream_t stream, const InputDesc* descs,
                        const int64_t* sorted_keys, const uint32_t* sorted_items,
                        const int64_t* seg_start, const int64_t* n_unique,
                        const OptimizerArgs& opt, int64_t* emit_keys, float* emit_rows,
-                       int emit_width) {
+                       int emit_width, bool row_decay) {
   if constexpr (!std::is_same<StateT, float>::value)
     segment_update_bf16state_kernel<GradT, VEC, TabT><<<grid, kThreads, 0, stream>>>(
+        descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
+        sorted_items, seg_start, n_unique, opt, emit_keys, emit_rows, emit_width);
+  else if (row_decay)
+    segment_update_rowwise_decay_kernel<GradT, VEC, TabT><<<grid, kThreads, 0, stream>>>(
         descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
         sorted_items, seg_start, n_unique, opt, emit_keys, emit_rows, emit_width);
   else if constexpr (std::is_same<TabT, float>::value)
@@ -699,7 +762,7 @@ static void launch_seg(int grid, cudaStream_t stream, const InputDesc* descs,
 #define DE_DISPATCH_SEG(GradT, VEC, TabT, StateT)                                              \
   launch_seg<GradT, VEC, TabT, StateT>(grid, stream, descs, tables, n_tables, lpr, batch, grad_batch,  \
                                grad_stride, grad, sorted_keys, sorted_items, seg_start,        \
-                               n_unique, opt, emit_keys, emit_rows, emit_width)
+                               n_unique, opt, emit_keys, emit_rows, emit_width, row_decay)
 #define DE_DISPATCH_SEG_G(VEC, TabT, StateT)                                                   \
   do {                                                                                         \
     if (act_dtype == 1) DE_DISPATCH_SEG(__nv_bfloat16, VEC, TabT, StateT);                     \
@@ -733,6 +796,7 @@ void launch_segment_update(const InputDesc* descs, const TableDesc* tables, int 
   const int rpw = 32 / lpr;
   const int64_t warps = (n_items + rpw - 1) / rpw;
   const int grid = grid_cap(warps, sm_count, 8);
+  const bool row_decay = opt.kind == kOptRowwiseAdagrad && opt.weight_decay != 0.f;
   // the emit path never touches the table: one instantiation serves every storage type; only
   // Adagrad and Adam read element-wise state, every other optimizer takes the fp32-state kernels
   if (state_dtype == 1 && (opt.kind == kOptAdagrad || opt.kind == kOptAdam)) {
@@ -751,9 +815,13 @@ static void launch_balanced_g(const InputDesc* descs, const TableDesc* tables, i
                               const uint32_t* sorted_items, int64_t n_items,
                               const int64_t* seg_start, const int64_t* n_unique,
                               const OptimizerArgs& opt, float* scratch, int scratch_width,
-                              int grid, cudaStream_t stream) {
+                              int grid, cudaStream_t stream, bool row_decay) {
   if constexpr (!std::is_same<StateT, float>::value)
     balanced_update_bf16state_kernel<GradT, TabT><<<grid, kThreads, 0, stream>>>(
+        descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
+        sorted_items, n_items, seg_start, n_unique, opt, scratch, scratch_width);
+  else if (row_decay)
+    balanced_update_rowwise_decay_kernel<GradT, TabT><<<grid, kThreads, 0, stream>>>(
         descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
         sorted_items, n_items, seg_start, n_unique, opt, scratch, scratch_width);
   else if constexpr (std::is_same<TabT, float>::value)
@@ -774,21 +842,25 @@ static void launch_balanced(const InputDesc* descs, const TableDesc* tables, int
                             const int64_t* seg_start, const int64_t* n_unique,
                             const OptimizerArgs& opt, float* scratch, int scratch_width,
                             int act_dtype, int grid, cudaStream_t stream) {
+  const bool row_decay = opt.kind == kOptRowwiseAdagrad && opt.weight_decay != 0.f;
   if (act_dtype == 1)
     launch_balanced_g<__nv_bfloat16, TabT, StateT>(descs, tables, n_tables, lpr, batch, grad_batch,
                                            grad_stride, grad, sorted_keys, sorted_items, n_items,
                                            seg_start, n_unique, opt, scratch, scratch_width, grid,
-                                           stream);
+                                           stream, row_decay);
   else if (act_dtype == 2)
     launch_balanced_g<__half, TabT, StateT>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride,
                                     grad, sorted_keys, sorted_items, n_items, seg_start, n_unique,
-                                    opt, scratch, scratch_width, grid, stream);
+                                    opt, scratch, scratch_width, grid, stream, row_decay);
   else
     launch_balanced_g<float, TabT, StateT>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride,
                                    grad, sorted_keys, sorted_items, n_items, seg_start, n_unique,
-                                   opt, scratch, scratch_width, grid, stream);
+                                   opt, scratch, scratch_width, grid, stream, row_decay);
   if constexpr (!std::is_same<StateT, float>::value)
     finalize_crossing_bf16state_kernel<TabT><<<grid, kThreads, 0, stream>>>(
+        tables, n_tables, lpr, sorted_keys, n_items, opt, scratch, scratch_width);
+  else if (row_decay)
+    finalize_crossing_rowwise_decay_kernel<TabT><<<grid, kThreads, 0, stream>>>(
         tables, n_tables, lpr, sorted_keys, n_items, opt, scratch, scratch_width);
   else if constexpr (std::is_same<TabT, float>::value)
     finalize_crossing_kernel<<<grid, kThreads, 0, stream>>>(tables, n_tables, lpr, sorted_keys,

@@ -598,9 +598,24 @@ class DistributedEmbedding(nn.Module):
     kernels (no sparse gradient is materialised).  ``kind``: ``sgd`` | ``adagrad`` |
     ``rowwise_adagrad`` | ``adam``.  Only the fused back end consumes it.
 
-    ``state_dtype``: storage of the Adagrad accumulator / Adam moments, ``torch.float32``
-    (default) or ``torch.bfloat16`` (half the bytes; the update runs in fp32 and stores the state
-    with stochastic rounding, see the user guide, "Half-precision optimizer state")."""
+    Keyword arguments (any other raises ``ValueError``):
+
+    - ``eps``: added to the square root in the denominator (default 1e-7, Adam 1e-8).
+    - ``beta1``, ``beta2``: Adam's moment decay rates (0.9, 0.999).
+    - ``initial_accumulator_value``: start value of the Adagrad / row-wise Adagrad accumulator
+      (0.1).
+    - ``weight_decay``: L2 decay (default 0).  ``weight_decay * w`` is added to the summed,
+      scaled gradient of a row before the optimizer sees it, once per step for every row that at
+      least one id of the step touched (a row whose ids carry only zero gradients included).  The
+      optimizers are lazy: rows no id touched, and their state, do not move.  Row-wise Adagrad
+      accumulates the mean square of this decayed gradient.
+    - ``deterministic``: SGD only (default False).  False sends SGD without weight decay through
+      one atomic scatter of the gradient rows into the tables; True, or any weight decay, takes
+      the sorted update, which sums each row's gradient before it applies it.
+    - ``step``: Adam's step count to resume from (0).
+    - ``state_dtype``: storage of the Adagrad accumulator / Adam moments, ``torch.float32``
+      (default) or ``torch.bfloat16`` (half the bytes; the update runs in fp32 and stores the
+      state with stochastic rounding, see the user guide, "Half-precision optimizer state")."""
     kind = kind.lower()
     if kind not in ("sgd", "adagrad", "rowwise_adagrad", "adam"):
       raise ValueError(f"Unsupported fused optimizer {kind}")
@@ -611,6 +626,10 @@ class DistributedEmbedding(nn.Module):
     cfg = {"kind": kind, "lr": float(lr), "eps": 1e-7 if kind != "adam" else 1e-8,
            "beta1": 0.9, "beta2": 0.999, "weight_decay": 0.0, "initial_accumulator_value": 0.1,
            "deterministic": kind != "sgd", "step": 0, "state_dtype": state_dtype}
+    unknown = sorted(set(kwargs) - set(cfg))
+    if unknown:
+      raise ValueError(f"unknown fused optimizer argument(s) {unknown}; the known ones are "
+                       f"{sorted(set(cfg) - {'kind', 'lr'})}")
     cfg.update(kwargs)
     self._fused_optimizer = cfg
     if self._engine is not None:

@@ -187,8 +187,8 @@ class FusedEngine:
     return self.ctx.sync(wait=wait, wait_abs=wait_abs, signal=signal) if self.W > 1 else []
 
   def dry_updates(self, on: bool):
-    """While on, the update kernels run on a zero gradient (scale 0) and the optimizer step
-    counter is left alone: the warm-up passes a trainer runs before capturing its CUDA graph
+    """While on, the update kernels run on a zero gradient (scale 0) without weight decay and the
+    optimizer step counter is left alone: the warm-up passes a trainer runs before capturing its CUDA graph
     exercise every kernel (lazy module loading, workspaces) without touching the tables or the
     optimizer state (Adagrad accumulators would otherwise absorb the warm-up gradients)."""
     self._dry_updates = bool(on)
@@ -1167,10 +1167,12 @@ class FusedEngine:
     self._backward_mp(producer)
 
   def _atomic_sgd(self) -> bool:
-    """The SGD update is one atomic scatter of the gradient rows into the tables."""
+    """The SGD update is one atomic scatter of the gradient rows into the tables.  Not with
+    weight decay: the scatter adds each id's gradient on its own, so with duplicate ids it could
+    not apply the decay exactly once per row; SGD with decay takes the sorted update."""
     opt = self.de._fused_optimizer
     return opt is not None and opt["kind"] == "sgd" and not opt.get("deterministic", False) and \
-        not self.has_offload and self.tab == 0
+        opt.get("weight_decay", 0.0) == 0.0 and not self.has_offload and self.tab == 0
 
   def producer_update(self, dim: int, min_rows: int) -> Optional["ProducerUpdate"]:
     """The SGD table update a single-GPU gradient producer can apply itself.
@@ -1268,10 +1270,13 @@ class FusedEngine:
       kind = _OPT_KIND[opt["kind"]]
       if self._dry_updates and opt["kind"] == "adam":
         kind = _OPT_KIND["sgd"]  # a zero gradient would still decay Adam's moments
+      # a dry update has no decay either: weight_decay * w would move the weights and feed the
+      # Adagrad accumulators on every warm-up pass
+      wd = 0.0 if self._dry_updates else opt["weight_decay"]
       ops.segment_update(self.mpdesc, self.tdesc, n_mp, B, B, self.recv_width, self.recv_ptr,
                          keys, items, seg, n_unique, kind, opt["lr"],
                          opt["eps"], opt["beta1"], opt["beta2"], 1.0, 1.0, gscale,
-                         opt["weight_decay"], self.lr_t.data_ptr(), None, None, self.max_width,
+                         wd, self.lr_t.data_ptr(), None, None, self.max_width,
                          self.act, self.vec4, self._balanced_scratch(), self.step_t.data_ptr(),
                          self.tab, DTYPE_CODE[self.state_dtype])
       if multi:

@@ -51,66 +51,13 @@ import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
+from optim_reference import reference  # pylint: disable=wrong-import-order
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-U = 2.0**-24  # fp32 unit roundoff
-TINY = 1e-37
 
 
-# ------------------------------------------------------------------ float64 model + bounds
-def _ulp32(x):
-  """ulp of fp32 numbers of magnitude |x| (float64 tensor), subnormal floor included."""
-  e = torch.floor(torch.log2(x.abs().clamp_min(2.0**-126)))
-  return torch.pow(2.0, e - 23)
-
-
-def reference(kind, p, g, s0, s1, lr, t, cfg, defect=None):
-  """float64 result of one update on fp32 inputs, with its error bounds.  ``defect`` models a
-  wrong kernel: 'bias_t_minus_1', 'eps_in_sqrt', 'no_state_writeback', 'no_grad_zero'."""
-  f = lambda x: x.double()
-  p, g, s0 = f(p), f(g), f(s0)
-  f32 = lambda v: float(torch.tensor(v, dtype=torch.float32))
-  lr, eps = f32(lr), f32(cfg["eps"])
-  out, bound = {}, {}
-  if kind == "adagrad":
-    a = s0 + g * g
-    den = (a + eps).sqrt() if defect == "eps_in_sqrt" else a.sqrt() + eps
-    d = lr * g / den
-    out["s0"] = s0 if defect == "no_state_writeback" else a
-    bound["s0"] = _ulp32(a) + TINY  # one fma: exactly rounded
-    e_d = 6 * U * d.abs()
-  else:
-    s1 = f(s1)
-    b1, b2 = f32(cfg["beta1"]), f32(cfg["beta2"])
-    c1, c2 = 1.0 - b1, 1.0 - b2  # exact in fp32 (Sterbenz)
-    tt = t - 1 if defect == "bias_t_minus_1" else t
-    m = b1 * s0 + c1 * g
-    v = b2 * s1 + c2 * g * g
-    pw1, pw2 = b1**tt, b2**tt
-    bias1, bias2 = 1.0 - pw1, 1.0 - pw2
-    mh, vh = m / bias1, v / bias2
-    sq = (vh + eps).sqrt() if defect == "eps_in_sqrt" else vh.sqrt()
-    den = sq if defect == "eps_in_sqrt" else sq + eps
-    d = lr * mh / den
-    out["s0"] = s0 if defect == "no_state_writeback" else m
-    out["s1"] = s1 if defect == "no_state_writeback" else v
-    # moments: two or three roundings of the terms (fma contraction only removes some)
-    e_m = 2.5 * U * ((b1 * s0).abs() + (c1 * g).abs())
-    e_v = 3.5 * U * ((b2 * s1).abs() + c2 * g * g)
-    bound["s0"], bound["s1"] = e_m + TINY, e_v + TINY
-    # bias corrections: powf within 4 ulps, then one rounding of 1 - x
-    rb1 = 4 * float(_ulp32(torch.tensor(pw1))) / bias1 + U
-    rb2 = 4 * float(_ulp32(torch.tensor(pw2))) / bias2 + U
-    e_mh = e_m / bias1 + mh.abs() * (rb1 + U)
-    rv = torch.where(v > 0, e_v / v.clamp_min(1e-300), torch.zeros_like(v)) + rb2 + U
-    e_sq = sq * (rv / 2 + U)
-    e_den = e_sq + U * den
-    e_d = (lr * e_mh + U * lr * mh.abs()) / den + d.abs() * (e_den / den + U)
-  out["p"] = p - d
-  bound["p"] = 1.05 * e_d + U * out["p"].abs() + TINY
-  out["g"] = g if defect == "no_grad_zero" else torch.zeros_like(g)
-  return out, bound
-
-
+# ------------------------------------------------------------------ bounds (float64 model and
+# operation-count bounds: optim_reference.py)
 def worst_ratio(kind, inputs, got, cfg, t=1):
   """max |got - ref| / bound over p32 and the state; inf when p16 / g32 are not exact."""
   ref, bound = reference(kind, *inputs, t, cfg)

@@ -47,11 +47,15 @@ def assemble(des, get=lambda p: p.detach().float()):
   return out
 
 
-def reference_step(tables, imap, glob_ids, combiners, grads, lr, world, kind, state):
+def reference_step(tables, imap, glob_ids, combiners, grads, lr, world, kind, state,
+                   weight_decay=0.0):
   """Unsharded model: returns outputs [global batch, width] per input and updates ``tables``
-  in place with the mean-of-ranks gradient contract (sum over the global batch / world)."""
+  in place with the mean-of-ranks gradient contract (sum over the global batch / world).  The
+  optimizers are lazy: a row is touched when at least one id hits it (zero gradients included),
+  and only touched rows get the decay and advance their state."""
   outs = []
   dense = [np.zeros_like(t) for t in tables]
+  touched_rows = [np.zeros(t.shape[0], dtype=bool) for t in tables]
   for i, t in enumerate(imap):
     ids = glob_ids[i]
     if isinstance(ids, list):  # ragged: one id list per sample
@@ -63,6 +67,7 @@ def reference_step(tables, imap, glob_ids, combiners, grads, lr, world, kind, st
         scale = 1.0 / n if combiners[t] == "mean" else 1.0
         out[b] = tables[t][row].sum(0) * scale
         np.add.at(dense[t], np.asarray(row, dtype=np.int64), grads[i][b] * scale)
+        touched_rows[t][np.asarray(row, dtype=np.int64)] = True
       outs.append(out)
       continue
     # ids outside the table (fed to row-sliced tables) pool to zero and get no gradient
@@ -74,13 +79,15 @@ def reference_step(tables, imap, glob_ids, combiners, grads, lr, world, kind, st
     per_id = np.repeat(g, n, axis=0)
     flat_ok = ok.reshape(-1)
     np.add.at(dense[t], ids.reshape(-1)[flat_ok], per_id[flat_ok])
+    touched_rows[t][ids.reshape(-1)[flat_ok]] = True
   if kind == "none":
     return outs, [g / world for g in dense]
   for t, g in enumerate(dense):
+    touched = touched_rows[t]
     g = g / world
-    touched = np.abs(g).sum(1) != 0
+    g[touched] += weight_decay * tables[t][touched]
     if kind == "sgd":
-      tables[t] -= lr * g
+      tables[t][touched] -= lr * g[touched]
     elif kind == "adagrad":
       acc = state.setdefault(t, np.full_like(tables[t], 0.1))
       acc[touched] += g[touched]**2
@@ -89,7 +96,7 @@ def reference_step(tables, imap, glob_ids, combiners, grads, lr, world, kind, st
       acc = state.setdefault(t, np.full(tables[t].shape[0], 0.1, dtype=np.float32))
       acc[touched] += (g[touched]**2).mean(1)
       tables[t][touched] -= lr * g[touched] / (np.sqrt(acc[touched])[:, None] + 1e-7)
-    elif kind == "adam":  # first step of lazy Adam: m/bias1 = g, v/bias2 = g^2
+    elif kind == "adam":  # first step of lazy Adam: m/bias1 = g, v/bias2 = g^2 (0/eps = 0)
       tables[t][touched] -= lr * g[touched] / (np.abs(g[touched]) + 1e-8)
   return outs
 
@@ -131,7 +138,7 @@ def _draw_grads(nrng, shapes, dyadic):
 
 
 def run_plan(seed, world, kind="sgd", dtype=torch.float32, ragged=False, profile=None,
-             world_cls=dry_run.DryWorld):
+             world_cls=dry_run.DryWorld, weight_decay=0.0):
   prof = dict(SMALL_PROFILE, **(profile or {}))
   rng = random.Random(seed)
   nrng = np.random.default_rng(seed)
@@ -178,7 +185,7 @@ def run_plan(seed, world, kind="sgd", dtype=torch.float32, ragged=False, profile
   for de in des:
     de.set_weights(tables)
     if kind != "none":
-      de.set_optimizer(kind, lr=0.5)
+      de.set_optimizer(kind, lr=0.5, weight_decay=weight_decay)
   lb = rng.choice(prof["local_batch"])
   B = lb * world
   glob = [_draw_ids(nrng, sizes[t][0], (B, hots[t]), prof["power_law"]) for t in imap]
@@ -232,7 +239,8 @@ def run_plan(seed, world, kind="sgd", dtype=torch.float32, ragged=False, profile
   results = dry_run.run_ranks(sim, rank_fn)
   ref_tables = [t.copy() for t in tables]
   # replicated tables are not updated by the engine (their dense gradient goes to the all-reduce)
-  ref_outs = reference_step(ref_tables, imap, glob, combiners, grads, 0.5, world, kind, {})
+  ref_outs = reference_step(ref_tables, imap, glob, combiners, grads, 0.5, world, kind, {},
+                            weight_decay)
   ref_grads = None
   if kind == "none":
     ref_outs, ref_grads = ref_outs
@@ -277,12 +285,18 @@ def test_random_plans_sgd(world):
   n = 8 if world < 8 else 4
   outcomes = [run_plan(1000 * world + s, world, "sgd") for s in range(n)]
   assert outcomes.count("ok") >= n // 2 + 1, outcomes
+  # SGD with weight decay leaves the atomic scatter for the sorted update
+  outcomes = [run_plan(1000 * world + s, world, "sgd", weight_decay=0.25) for s in range(2)]
+  assert outcomes.count("ok") >= 1, outcomes
 
 
 @pytest.mark.parametrize("world", [1, 2, 4])
 @pytest.mark.parametrize("kind", ["adagrad", "rowwise_adagrad", "adam"])
 def test_random_plans_stateful_optimizers(world, kind):
   outcomes = [run_plan(5000 * world + s, world, kind) for s in range(5)]
+  assert outcomes.count("ok") >= 3, outcomes
+  # weight decay (dyadic, so exact on the dyadic grid of the GPU conformance profile as well)
+  outcomes = [run_plan(5000 * world + s, world, kind, weight_decay=0.25) for s in range(5)]
   assert outcomes.count("ok") >= 3, outcomes
 
 
@@ -402,7 +416,12 @@ def _run_steps(seed, world, kind, n_steps=3):
     t_step = step + 1
     for t, g in enumerate(dense):
       g = g / world
-      touched = np.abs(g).sum(1) != 0
+      # lazy: the rows an id hit, whatever their gradient (Adam decays the moments of a row hit
+      # by zero gradients)
+      touched = np.zeros(ref[t].shape[0], dtype=bool)
+      for i, ti in enumerate(imap):
+        if ti == t:
+          touched[glob[i].reshape(-1)] = True
       if kind == "sgd":
         ref[t] -= lr * g
       elif kind == "adagrad":
@@ -937,7 +956,13 @@ def test_shared_learning_rate_word_is_owned_by_the_trainer(kind):
 def test_dry_updates_leave_tables_and_optimizer_state_untouched(kind):
   """Graph warm-up passes of the hand-scheduled trainers run with ``dry_updates(True)``: every
   kernel is launched, but tables, optimizer state and the step counter must come out exactly as
-  they went in - then a real step must equal a step taken without any warm-up."""
+  they went in - then a real step must equal a step taken without any warm-up.  With weight decay
+  as well: a dry pass applies none."""
+  for weight_decay in (0.0, 0.5):
+    _dry_updates_case(kind, weight_decay)
+
+
+def _dry_updates_case(kind, weight_decay):
   rng = np.random.default_rng(4)
   sizes = [(30, 8), (12, 16), (50, 8), (21, 16)]
   embs = [{"input_dim": r, "output_dim": w, "combiner": "sum"} for r, w in sizes]
@@ -950,7 +975,7 @@ def test_dry_updates_leave_tables_and_optimizer_state_untouched(kind):
     sim, des = dry_run.build_engines(embs, world, strategy="memory_balanced")
     for de in des:
       de.set_weights(tables)
-      de.set_optimizer(kind, lr=0.3)
+      de.set_optimizer(kind, lr=0.3, weight_decay=weight_decay)
     return sim, des
 
   def step(sim, des):
@@ -979,8 +1004,9 @@ def test_dry_updates_leave_tables_and_optimizer_state_untouched(kind):
   step(sim_b, des_b)
   for a, b in zip(assemble(des_a), assemble(des_b)):
     np.testing.assert_array_equal(a, b)
+  # SGD counts steps on the sorted update only, which it takes with weight decay
   assert des_a[0]._engine.step_count() == des_b[0]._engine.step_count() == \
-      (0 if kind == "sgd" else 1)
+      (0 if kind == "sgd" and not weight_decay else 1)
 
 
 @pytest.mark.parametrize("world", [1, 3])

@@ -8,7 +8,8 @@ GPU:
     table row is within the fp32 accumulation bound of the float64 update, untouched rows are bit
     identical;
   * the zero-rate warm-up passes leave every table bit identical;
-  * ineligible configurations (Adagrad, bf16 tables) run the schedule of ``fused_table_update=False``;
+  * ineligible configurations (Adagrad, bf16 tables, SGD with weight decay) run the schedule of
+    ``fused_table_update=False``; with weight decay the tables match the float64 SGD step;
   * ``interact_bwd`` rejects malformed apply records before any launch.
 CPU (plan interpreter): the descriptor split at world 1, the configurations that get none, and a
 step whose producer applies the large tables against the unsharded SGD reference.
@@ -204,7 +205,8 @@ def test_zero_rate_warmup_leaves_tables():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("kw", [{"embedding_optimizer": "adagrad"}, {"table_dtype": "bf16"}])
+@pytest.mark.parametrize("kw", [{"embedding_optimizer": "adagrad"}, {"table_dtype": "bf16"},
+                                {"embedding_optimizer_kwargs": {"weight_decay": 0.5}}])
 def test_ineligible_steps_run_todays_schedule(kw):
   from distributed_embeddings_b200.models.dlrm import DLRM
   from distributed_embeddings_b200.models.dlrm_fast import DLRMTrainStep
@@ -216,8 +218,10 @@ def test_ineligible_steps_run_todays_schedule(kw):
     mkw = {"table_dtype": torch.bfloat16} if "table_dtype" in kw else {}
     model = DLRM(sizes, device=dev, compute_dtype=torch.bfloat16, backend="fused", **mkw)
     step = DLRMTrainStep(model, lr=0.1, use_cuda_graph=False, fused_table_update=fused,
-                         embedding_optimizer=kw.get("embedding_optimizer", "sgd"))
+                         embedding_optimizer=kw.get("embedding_optimizer", "sgd"),
+                         embedding_optimizer_kwargs=kw.get("embedding_optimizer_kwargs"))
     proxy = _watch(step)
+    old = _tables(model)
     g = torch.Generator().manual_seed(2)
     cat = torch.stack([torch.randint(0, s, (256,), generator=g, dtype=torch.int32)
                        for s in sizes]).to(dev)
@@ -226,6 +230,21 @@ def test_ineligible_steps_run_todays_schedule(kw):
     torch.cuda.synchronize()
     assert step.engine.producer_update(step.dim, 1) is None
     runs.append(proxy.calls)
+    if "embedding_optimizer_kwargs" in kw:
+      # SGD with decay on the sorted update: every table against the float64 step from the
+      # gradient rows of the receive buffer (the producer applied none), hit rows within the
+      # operation-count bound, rows no id hit bit identical
+      from optim_reference import table_step, worst_table_ratio
+      grads = _grad_rows(step)
+      new = _tables(model)
+      for t in range(len(sizes)):
+        out, bound, _ = table_step("sgd", old[t].cpu().numpy(), [], cat[t].long().cpu().numpy(),
+                                   grads[:, t].cpu().numpy(), 1.0, 0.1, 1,
+                                   kw["embedding_optimizer_kwargs"])
+        r = worst_table_ratio(out, bound, {"p": new[t].cpu().numpy()})
+        assert r <= 1.0, (t, r)
+  if "embedding_optimizer_kwargs" in kw:
+    assert all(op != "scatter_add_bwd" for op, _ in runs[0]), runs[0]
   assert runs[0] == runs[1]
   assert ("interact_bwd", False) in runs[0]
 

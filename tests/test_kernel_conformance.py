@@ -528,6 +528,9 @@ def test_gpu_random_plans(world, kind):
   before = REPLAYED.copy()
   _ok([run_plan(31000 * world + 7 * s + len(kind), world, kind, profile=DYADIC,
                 world_cls=_gpu_world()) for s in range(n)], 1)
+  if kind != "none":  # weight decay (dyadic: exact on the grid) at grad_scale = 1 / world
+    _ok([run_plan(32000 * world + 7 * s + len(kind), world, kind, profile=DYADIC,
+                  world_cls=_gpu_world(), weight_decay=0.25) for s in range(2)], 1)
   d = _delta(before)
   assert d.get("lookup_fwd, several destinations", 0) > 0, d
   if kind == "none":
