@@ -647,21 +647,15 @@ void launch_copy_cast_2d(const void* src, int64_t src_stride, void* dst, int64_t
   const int threads = 256;
   int64_t blocks = (rows * cols + threads - 1) / threads;
   if (blocks > kGridCapSms * 8) blocks = kGridCapSms * 8;
-#define DE_CC(S, D)                                                                              \
-  copy_cast_2d_kernel<S, D><<<static_cast<unsigned>(blocks), threads, 0, stream>>>(              \
-      reinterpret_cast<const S*>(src), src_stride, reinterpret_cast<D*>(dst), dst_stride, rows,  \
-      cols, scale)
-#define DE_CC_D(S)                                                                               \
-  do {                                                                                           \
-    if (dst_dtype == 1) DE_CC(S, __nv_bfloat16);                                                 \
-    else if (dst_dtype == 2) DE_CC(S, __half);                                                   \
-    else DE_CC(S, float);                                                                        \
-  } while (0)
-  if (src_dtype == 1) DE_CC_D(__nv_bfloat16);
-  else if (src_dtype == 2) DE_CC_D(__half);
-  else DE_CC_D(float);
-#undef DE_CC_D
-#undef DE_CC
+  with_dtype(src_dtype, [&](auto src_t) {
+    using S = typename decltype(src_t)::type;
+    with_dtype(dst_dtype, [&](auto dst_t) {
+      using D = typename decltype(dst_t)::type;
+      copy_cast_2d_kernel<S, D><<<static_cast<unsigned>(blocks), threads, 0, stream>>>(
+          reinterpret_cast<const S*>(src), src_stride, reinterpret_cast<D*>(dst), dst_stride, rows,
+          cols, scale);
+    });
+  });
 }
 
 void launch_p2p_store_bench(const void* src, void* dst, int64_t n_rows, int row_bytes,
@@ -730,20 +724,14 @@ void launch_push_grad(const GradRoute* routes, int n_routes, const void* src, in
   const int64_t total = ((rows + 7) / 8) * n_routes;
   int64_t blocks = total;
   if (blocks > static_cast<int64_t>(sm_count) * 8) blocks = static_cast<int64_t>(sm_count) * 8;
-#define DE_PG(S, D)                                                                               \
-  push_grad_kernel<S, D><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(                      \
-      routes, n_routes, reinterpret_cast<const S*>(src), src_stride, rows, scale, sync)
-#define DE_PG_D(S)                                                                                \
-  do {                                                                                            \
-    if (dst_dtype == 1) DE_PG(S, __nv_bfloat16);                                                  \
-    else if (dst_dtype == 2) DE_PG(S, __half);                                                    \
-    else DE_PG(S, float);                                                                         \
-  } while (0)
-  if (src_dtype == 1) DE_PG_D(__nv_bfloat16);
-  else if (src_dtype == 2) DE_PG_D(__half);
-  else DE_PG_D(float);
-#undef DE_PG_D
-#undef DE_PG
+  with_dtype(src_dtype, [&](auto src_t) {
+    using S = typename decltype(src_t)::type;
+    with_dtype(dst_dtype, [&](auto dst_t) {
+      using D = typename decltype(dst_t)::type;
+      push_grad_kernel<S, D><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
+          routes, n_routes, reinterpret_cast<const S*>(src), src_stride, rows, scale, sync);
+    });
+  });
 }
 
 void launch_rowslice_reduce(const float* partial, int world, int64_t rows, int64_t part_stride,
@@ -756,18 +744,12 @@ void launch_rowslice_reduce(const float* partial, int world, int64_t rows, int64
   const int64_t n = rows * total_width;
   int64_t blocks = (n + 255) / 256;
   if (blocks > kGridCapSms * 8) blocks = kGridCapSms * 8;
-  if (out_dtype == 1)
-    rowslice_reduce_kernel<__nv_bfloat16><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
-        partial, world, rows, part_stride, reinterpret_cast<__nv_bfloat16*>(out), out_stride, cols,
-        n_cols, total_width);
-  else if (out_dtype == 2)
-    rowslice_reduce_kernel<__half><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
-        partial, world, rows, part_stride, reinterpret_cast<__half*>(out), out_stride, cols,
-        n_cols, total_width);
-  else
-    rowslice_reduce_kernel<float><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
-        partial, world, rows, part_stride, reinterpret_cast<float*>(out), out_stride, cols, n_cols,
+  with_dtype(out_dtype, [&](auto out_t) {
+    using OutT = typename decltype(out_t)::type;
+    rowslice_reduce_kernel<OutT><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
+        partial, world, rows, part_stride, reinterpret_cast<OutT*>(out), out_stride, cols, n_cols,
         total_width);
+  });
 }
 
 }  // namespace de

@@ -19,6 +19,29 @@ __host__ __device__ __forceinline__ int pow2_ceil(int x) {
   return p;
 }
 
+// ---- host-side dispatch of launch codes to template arguments -------------------------------
+// The launchers call a generic lambda with a tag and recover the type as
+// `typename decltype(tag)::type`, so each launch site is written once for every type.
+template <typename T>
+struct type_tag {
+  using type = T;
+};
+
+// dtype code of activations, gradients and tables: 0 fp32, 1 bf16, 2 fp16
+template <typename F>
+void with_dtype(int code, F&& f) {
+  if (code == 1) f(type_tag<__nv_bfloat16>{});
+  else if (code == 2) f(type_tag<__half>{});
+  else f(type_tag<float>{});
+}
+
+// one of two types by a flag (64- or 32-bit ids, 32- or 64-bit sort keys)
+template <typename IfTrue, typename IfFalse, typename F>
+void with_type_if(bool flag, F&& f) {
+  if (flag) f(type_tag<IfTrue>{});
+  else f(type_tag<IfFalse>{});
+}
+
 // ---- small fixed-size vectors of fp32 ---------------------------------------------------
 template <int VEC>
 struct FVec {

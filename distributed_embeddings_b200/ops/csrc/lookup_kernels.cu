@@ -97,11 +97,11 @@ __device__ __forceinline__ IdReader<IdT> make_reader(const InputDesc& D, const P
 
 // =============================================================================== forward
 template <typename IdT, typename OutT, int VEC, typename TabT>
-__device__ __forceinline__ void lookup_fwd_body(const InputDesc* __restrict__ descs, int n_inputs,
-                                                int64_t batch, int64_t src_batch,
-                                                int64_t dst_batch, int64_t dst_stride,
-                                                const PeerPtrs& src, const PeerPtrs& dst, int rot,
-                                                const SyncArgs& sync, int ts) {
+__global__ void __launch_bounds__(kThreads, fwd_blocks_per_sm(VEC))
+lookup_fwd_kernel(const InputDesc* __restrict__ descs, int n_inputs, int64_t batch,
+                  int64_t src_batch, int64_t dst_batch, int64_t dst_stride,
+                  const __grid_constant__ PeerPtrs src, const __grid_constant__ PeerPtrs dst,
+                  int rot, const __grid_constant__ SyncArgs sync, int ts) {
   // ts = samples per warp tile (power of two <= 32): 32 for one-hot inputs; multi-hot inputs
   // get smaller tiles so that a launch still has enough warps when every sample pools tens or
   // hundreds of rows (the reference splits long reductions over blockDim.y, CU:195-226)
@@ -216,28 +216,6 @@ __device__ __forceinline__ void lookup_fwd_body(const InputDesc* __restrict__ de
     }
   }
   sync_tail(sync);  // every pooled row of this rank is on its way: tell the requesters
-}
-
-// fp32 tables
-template <typename IdT, typename OutT, int VEC>
-__global__ void __launch_bounds__(kThreads, kBlocksPerSM)
-lookup_fwd_kernel(const InputDesc* __restrict__ descs, int n_inputs, int64_t batch,
-                  int64_t src_batch, int64_t dst_batch, int64_t dst_stride,
-                  const __grid_constant__ PeerPtrs src, const __grid_constant__ PeerPtrs dst,
-                  int rot, const __grid_constant__ SyncArgs sync, int ts) {
-  lookup_fwd_body<IdT, OutT, VEC, float>(descs, n_inputs, batch, src_batch, dst_batch,
-                                         dst_stride, src, dst, rot, sync, ts);
-}
-
-// bf16 / fp16 tables (TabT)
-template <typename IdT, typename OutT, int VEC, typename TabT>
-__global__ void __launch_bounds__(kThreads, fwd_blocks_per_sm(VEC))
-lookup_fwd_tab16_kernel(const InputDesc* __restrict__ descs, int n_inputs, int64_t batch,
-                        int64_t src_batch, int64_t dst_batch, int64_t dst_stride,
-                        const __grid_constant__ PeerPtrs src, const __grid_constant__ PeerPtrs dst,
-                        int rot, const __grid_constant__ SyncArgs sync, int ts) {
-  lookup_fwd_body<IdT, OutT, VEC, TabT>(descs, n_inputs, batch, src_batch, dst_batch, dst_stride,
-                                        src, dst, rot, sync, ts);
 }
 
 // =============================================================================== backward
@@ -546,46 +524,6 @@ int64_t count_tiles(int n_inputs, int64_t batch, int64_t dst_batch, int ts = kTi
 
 }  // namespace
 
-// fp32 tables keep their own kernel; 16-bit tables take lookup_fwd_tab16_kernel
-template <typename IdT, typename OutT, int VEC, typename TabT>
-static void launch_fwd(int grid, cudaStream_t stream, const InputDesc* descs, int n_inputs,
-                       int64_t batch, int64_t src_batch, int64_t dst_batch, int64_t dst_stride,
-                       const PeerPtrs& src, const PeerPtrs& dst, int rot, const SyncArgs& sync,
-                       int ts) {
-  if constexpr (std::is_same<TabT, float>::value)
-    lookup_fwd_kernel<IdT, OutT, VEC><<<grid, kThreads, 0, stream>>>(
-        descs, n_inputs, batch, src_batch, dst_batch, dst_stride, src, dst, rot, sync, ts);
-  else
-    lookup_fwd_tab16_kernel<IdT, OutT, VEC, TabT><<<grid, kThreads, 0, stream>>>(
-        descs, n_inputs, batch, src_batch, dst_batch, dst_stride, src, dst, rot, sync, ts);
-}
-#define DE_DISPATCH_FWD(IdT, OutT, VEC, TabT)                                                  \
-  launch_fwd<IdT, OutT, VEC, TabT>(grid, stream, descs, n_inputs, batch, src_batch, dst_batch, \
-                                   dst_stride, src, dst, rot, sync, ts)
-#define DE_DISPATCH_FWD_T(IdT, VEC, TabT)                                                      \
-  do {                                                                                         \
-    if (act_dtype == 1) DE_DISPATCH_FWD(IdT, __nv_bfloat16, VEC, TabT);                        \
-    else if (act_dtype == 2) DE_DISPATCH_FWD(IdT, __half, VEC, TabT);                          \
-    else DE_DISPATCH_FWD(IdT, float, VEC, TabT);                                               \
-  } while (0)
-#define DE_DISPATCH_FWD_ID(VEC, TabT)                                                          \
-  do {                                                                                         \
-    if (ids64) DE_DISPATCH_FWD_T(int64_t, VEC, TabT);                                          \
-    else DE_DISPATCH_FWD_T(int32_t, VEC, TabT);                                                \
-  } while (0)
-
-template <typename TabT>
-static void dispatch_fwd_half(int vec, const InputDesc* descs, int n_inputs, int64_t batch,
-                              int64_t src_batch, int64_t dst_batch, int64_t dst_stride,
-                              const PeerPtrs& src, const PeerPtrs& dst, int rot, bool ids64,
-                              int act_dtype, int grid, cudaStream_t stream, const SyncArgs& sync,
-                              int ts) {
-  // 16-bit rows: 8 columns (one 16-byte load) per lane where the widths allow it
-  if (vec == 8) DE_DISPATCH_FWD_ID(8, TabT);
-  else if (vec == 4) DE_DISPATCH_FWD_ID(4, TabT);
-  else DE_DISPATCH_FWD_ID(1, TabT);
-}
-
 void launch_lookup_fwd(const InputDesc* descs, int n_inputs, int64_t batch, int64_t src_batch,
                        int64_t dst_batch, int64_t dst_stride, const PeerPtrs& src,
                        const PeerPtrs& dst, int rot, bool ids64, int act_dtype, bool vec4,
@@ -597,34 +535,32 @@ void launch_lookup_fwd(const InputDesc* descs, int n_inputs, int64_t batch, int6
   }
   int ts = 1;
   while (ts * 2 <= tile_samples && ts < kTile) ts *= 2;  // power of two in [1, 32]
-  if (table_dtype != 0) {
-    const int vec = vec4 ? (vec8 ? 8 : 4) : 1;
-    const int grid = grid_for(count_tiles(n_inputs, batch, dst_batch, ts), sm_count,
-                              fwd_blocks_per_sm(vec));
-    if (table_dtype == 1)
-      dispatch_fwd_half<__nv_bfloat16>(vec, descs, n_inputs, batch, src_batch, dst_batch,
-                                       dst_stride, src, dst, rot, ids64, act_dtype, grid, stream,
-                                       sync, ts);
-    else
-      dispatch_fwd_half<__half>(vec, descs, n_inputs, batch, src_batch, dst_batch, dst_stride,
-                                src, dst, rot, ids64, act_dtype, grid, stream, sync, ts);
-    return;
-  }
-  const int grid = grid_for(count_tiles(n_inputs, batch, dst_batch, ts), sm_count, kBlocksPerSM);
-  if (vec4) DE_DISPATCH_FWD_ID(4, float);
-  else DE_DISPATCH_FWD_ID(1, float);
+  // 16-bit rows: 8 columns (one 16-byte load) per lane where the widths allow it
+  const int vec = !vec4 ? 1 : (vec8 && table_dtype != 0) ? 8 : 4;
+  const int grid = grid_for(count_tiles(n_inputs, batch, dst_batch, ts), sm_count,
+                            fwd_blocks_per_sm(vec));
+  with_dtype(table_dtype, [&](auto tab) {
+    using TabT = typename decltype(tab)::type;
+    with_type_if<int64_t, int32_t>(ids64, [&](auto id) {
+      using IdT = typename decltype(id)::type;
+      with_dtype(act_dtype, [&](auto out) {
+        using OutT = typename decltype(out)::type;
+        auto launch = [&](auto kernel) {
+          kernel<<<grid, kThreads, 0, stream>>>(descs, n_inputs, batch, src_batch, dst_batch,
+                                                dst_stride, src, dst, rot, sync, ts);
+        };
+        if constexpr (sizeof(TabT) == 2) {
+          if (vec == 8) {
+            launch(lookup_fwd_kernel<IdT, OutT, 8, TabT>);
+            return;
+          }
+        }
+        if (vec == 4) launch(lookup_fwd_kernel<IdT, OutT, 4, TabT>);
+        else launch(lookup_fwd_kernel<IdT, OutT, 1, TabT>);
+      });
+    });
+  });
 }
-
-#define DE_DISPATCH_BWD(IdT, GradT, VEC)                                                       \
-  scatter_add_bwd_kernel<IdT, GradT, VEC><<<grid, kThreads, 0, stream>>>(                      \
-      descs, n_inputs, batch, src_batch, grad_batch, grad_stride, src, grad, rot, scale,       \
-      scale_ptr, sync)
-#define DE_DISPATCH_BWD_T(IdT, VEC)                                                            \
-  do {                                                                                         \
-    if (act_dtype == 1) DE_DISPATCH_BWD(IdT, __nv_bfloat16, VEC);                              \
-    else if (act_dtype == 2) DE_DISPATCH_BWD(IdT, __half, VEC);                                \
-    else DE_DISPATCH_BWD(IdT, float, VEC);                                                     \
-  } while (0)
 
 void launch_scatter_add_bwd(const InputDesc* descs, int n_inputs, int64_t batch, int64_t src_batch,
                             int64_t grad_batch, int64_t grad_stride, const PeerPtrs& src,
@@ -635,51 +571,41 @@ void launch_scatter_add_bwd(const InputDesc* descs, int n_inputs, int64_t batch,
     launch_sync_only(sync, stream);
     return;
   }
-  if (staged && vec4) {
-    // caller guarantees: every gradient row is a 16-byte multiple of at most 256 bytes, 16-byte
-    // aligned in the source (column offsets, row stride, base pointers)
-    const int64_t tiles = count_tiles(n_inputs, batch, grad_batch);
-    int64_t blocks = (tiles + kStagedWarps - 1) / kStagedWarps;
-    if (blocks > static_cast<int64_t>(sm_count) * 2) blocks = static_cast<int64_t>(sm_count) * 2;
-    const size_t smem = static_cast<size_t>(kStagedWarps) * 2 * kStageBytes;
-#define DE_STAGED(IdT, GradT)                                                                     \
-  {                                                                                               \
-    cudaFuncSetAttribute(scatter_add_staged_kernel<IdT, GradT>,                                   \
-                         cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));    \
-    scatter_add_staged_kernel<IdT, GradT><<<static_cast<unsigned>(blocks), kStagedThreads, smem,  \
-                                           stream>>>(descs, n_inputs, batch, src_batch,           \
-                                                     grad_batch, grad_stride, src, grad, rot,     \
-                                                     scale, scale_ptr, sync);                     \
-  }
-    if (act_dtype == 1) {
-      if (ids64) DE_STAGED(int64_t, __nv_bfloat16) else DE_STAGED(int32_t, __nv_bfloat16)
-    } else if (act_dtype == 2) {
-      if (ids64) DE_STAGED(int64_t, __half) else DE_STAGED(int32_t, __half)
-    } else {
-      if (ids64) DE_STAGED(int64_t, float) else DE_STAGED(int32_t, float)
-    }
-#undef DE_STAGED
-    return;
-  }
-  const int grid = grid_for(count_tiles(n_inputs, batch, grad_batch), sm_count, kBlocksPerSM);
-  if (vec8 && act_dtype != 0) {
-    // 16-byte gradient loads: 8 columns per lane, two rows per warp instruction
-    if (act_dtype == 1) {
-      if (ids64) DE_DISPATCH_BWD(int64_t, __nv_bfloat16, 8);
-      else DE_DISPATCH_BWD(int32_t, __nv_bfloat16, 8);
-    } else {
-      if (ids64) DE_DISPATCH_BWD(int64_t, __half, 8);
-      else DE_DISPATCH_BWD(int32_t, __half, 8);
-    }
-    return;
-  }
-  if (vec4) {
-    if (ids64) DE_DISPATCH_BWD_T(int64_t, 4);
-    else DE_DISPATCH_BWD_T(int32_t, 4);
-  } else {
-    if (ids64) DE_DISPATCH_BWD_T(int64_t, 1);
-    else DE_DISPATCH_BWD_T(int32_t, 1);
-  }
+  with_type_if<int64_t, int32_t>(ids64, [&](auto id) {
+    using IdT = typename decltype(id)::type;
+    with_dtype(act_dtype, [&](auto grad_t) {
+      using GradT = typename decltype(grad_t)::type;
+      if (staged && vec4) {
+        // caller guarantees: every gradient row is a 16-byte multiple of at most 256 bytes,
+        // 16-byte aligned in the source (column offsets, row stride, base pointers)
+        const int64_t tiles = count_tiles(n_inputs, batch, grad_batch);
+        int64_t blocks = (tiles + kStagedWarps - 1) / kStagedWarps;
+        if (blocks > static_cast<int64_t>(sm_count) * 2) blocks = static_cast<int64_t>(sm_count) * 2;
+        const size_t smem = static_cast<size_t>(kStagedWarps) * 2 * kStageBytes;
+        cudaFuncSetAttribute(scatter_add_staged_kernel<IdT, GradT>,
+                             cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+        scatter_add_staged_kernel<IdT, GradT>
+            <<<static_cast<unsigned>(blocks), kStagedThreads, smem, stream>>>(
+                descs, n_inputs, batch, src_batch, grad_batch, grad_stride, src, grad, rot, scale,
+                scale_ptr, sync);
+        return;
+      }
+      const int grid = grid_for(count_tiles(n_inputs, batch, grad_batch), sm_count, kBlocksPerSM);
+      auto launch = [&](auto kernel) {
+        kernel<<<grid, kThreads, 0, stream>>>(descs, n_inputs, batch, src_batch, grad_batch,
+                                              grad_stride, src, grad, rot, scale, scale_ptr, sync);
+      };
+      if constexpr (sizeof(GradT) == 2) {
+        // 16-byte gradient loads: 8 columns per lane, two rows per warp instruction
+        if (vec8) {
+          launch(scatter_add_bwd_kernel<IdT, GradT, 8>);
+          return;
+        }
+      }
+      if (vec4) launch(scatter_add_bwd_kernel<IdT, GradT, 4>);
+      else launch(scatter_add_bwd_kernel<IdT, GradT, 1>);
+    });
+  });
 }
 
 }  // namespace de

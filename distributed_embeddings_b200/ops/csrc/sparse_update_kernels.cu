@@ -204,11 +204,13 @@ __device__ __forceinline__ FVec<VEC> reduce_segment(const InputDesc* __restrict_
   return acc;
 }
 
+// One lane group per unique row.  TabT is the table's storage type, StateT that of the Adagrad /
+// Adam state; with_update_types() below says which combinations a launch takes.
 // kRowDecay: row-wise Adagrad with weight decay.  Its accumulator takes the row mean of the
 // squared decayed gradient (s * g + weight_decay * w), the gradient apply_update applies, so pass 1
-// reads the weights.  Those launches get kernels of their own: the other kernels keep their code
+// reads the weights.  Those launches get instantiations of their own: the others keep their code
 // and registers.
-template <typename GradT, int VEC, typename TabT, typename StateT, bool kRowDecay = false>
+template <typename GradT, int VEC, typename TabT, typename StateT, bool kRowDecay>
 __device__ __forceinline__ void segment_update_body(
     const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables, int n_tables,
     int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride, const PeerPtrs& grad,
@@ -305,56 +307,19 @@ __device__ __forceinline__ void segment_update_body(
   }
 }
 
-// fp32 tables
-template <typename GradT, int VEC>
-__global__ void __launch_bounds__(kThreads) segment_update_kernel(const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables,
-    int n_tables, int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
+// The bodies of the three update kernels stay separate inlined functions: folded into the kernels,
+// they get a different register allocation from ptxas.
+template <typename GradT, int VEC, typename TabT, typename StateT, bool kRowDecay>
+__global__ void __launch_bounds__(kThreads) segment_update_kernel(
+    const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables, int n_tables,
+    int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
     const __grid_constant__ PeerPtrs grad, const int64_t* __restrict__ sorted_keys,
     const uint32_t* __restrict__ sorted_items, const int64_t* __restrict__ seg_start,
     const int64_t* __restrict__ n_unique_p, const __grid_constant__ OptimizerArgs opt_in,
     int64_t* __restrict__ emit_keys, float* __restrict__ emit_rows, int emit_width) {
-  segment_update_body<GradT, VEC, float, float>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
-                                     sorted_keys, sorted_items, seg_start, n_unique_p, opt_in,
-                                     emit_keys, emit_rows, emit_width);
-}
-
-// bf16 / fp16 tables (TabT)
-template <typename GradT, int VEC, typename TabT>
-__global__ void __launch_bounds__(kThreads) segment_update_tab16_kernel(const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables,
-    int n_tables, int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
-    const __grid_constant__ PeerPtrs grad, const int64_t* __restrict__ sorted_keys,
-    const uint32_t* __restrict__ sorted_items, const int64_t* __restrict__ seg_start,
-    const int64_t* __restrict__ n_unique_p, const __grid_constant__ OptimizerArgs opt_in,
-    int64_t* __restrict__ emit_keys, float* __restrict__ emit_rows, int emit_width) {
-  segment_update_body<GradT, VEC, TabT, float>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
-                                     sorted_keys, sorted_items, seg_start, n_unique_p, opt_in,
-                                     emit_keys, emit_rows, emit_width);
-}
-
-// row-wise Adagrad with weight decay on fp32, bf16 or fp16 tables (TabT)
-template <typename GradT, int VEC, typename TabT>
-__global__ void __launch_bounds__(kThreads) segment_update_rowwise_decay_kernel(const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables,
-    int n_tables, int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
-    const __grid_constant__ PeerPtrs grad, const int64_t* __restrict__ sorted_keys,
-    const uint32_t* __restrict__ sorted_items, const int64_t* __restrict__ seg_start,
-    const int64_t* __restrict__ n_unique_p, const __grid_constant__ OptimizerArgs opt_in,
-    int64_t* __restrict__ emit_keys, float* __restrict__ emit_rows, int emit_width) {
-  segment_update_body<GradT, VEC, TabT, float, true>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
-                                     sorted_keys, sorted_items, seg_start, n_unique_p, opt_in,
-                                     emit_keys, emit_rows, emit_width);
-}
-
-// fp32, bf16 or fp16 tables (TabT) with bf16 Adagrad / Adam state
-template <typename GradT, int VEC, typename TabT>
-__global__ void __launch_bounds__(kThreads) segment_update_bf16state_kernel(const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables,
-    int n_tables, int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
-    const __grid_constant__ PeerPtrs grad, const int64_t* __restrict__ sorted_keys,
-    const uint32_t* __restrict__ sorted_items, const int64_t* __restrict__ seg_start,
-    const int64_t* __restrict__ n_unique_p, const __grid_constant__ OptimizerArgs opt_in,
-    int64_t* __restrict__ emit_keys, float* __restrict__ emit_rows, int emit_width) {
-  segment_update_body<GradT, VEC, TabT, __nv_bfloat16>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
-                                     sorted_keys, sorted_items, seg_start, n_unique_p, opt_in,
-                                     emit_keys, emit_rows, emit_width);
+  segment_update_body<GradT, VEC, TabT, StateT, kRowDecay>(
+      descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
+      sorted_items, seg_start, n_unique_p, opt_in, emit_keys, emit_rows, emit_width);
 }
 
 // ------------------------------------------------------------------ occurrence-balanced update
@@ -412,7 +377,7 @@ __device__ __forceinline__ int find_table(const TableDesc* __restrict__ tables, 
 }
 
 // Apply the optimizer to one row given the complete (scaled) gradient fragment of this lane.
-// kRowDecay: row-wise Adagrad with weight decay (see segment_update_body).
+// kRowDecay: row-wise Adagrad with weight decay (see segment_update_kernel).
 template <typename TabT, typename StateT, bool kRowDecay = false>
 __device__ __forceinline__ void apply_row(const TableDesc& T, const OptimizerArgs& opt,
                                           int64_t row, int col, FVec<4> g, int lpr,
@@ -443,7 +408,7 @@ __device__ __forceinline__ void apply_row(const TableDesc& T, const OptimizerArg
   if (col_ok) apply_update<TabT, 4, StateT>(T, opt, row, col, g, row_state, step);
 }
 
-template <typename GradT, typename TabT, typename StateT, bool kRowDecay = false>
+template <typename GradT, typename TabT, typename StateT, bool kRowDecay>
 __device__ __forceinline__ void balanced_update_body(
     const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables, int n_tables,
     int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride, const PeerPtrs& grad,
@@ -537,58 +502,22 @@ __device__ __forceinline__ void balanced_update_body(
   }
 }
 
+template <typename GradT, typename TabT, typename StateT, bool kRowDecay>
+__global__ void __launch_bounds__(kThreads) balanced_update_kernel(
+    const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables, int n_tables,
+    int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
+    const __grid_constant__ PeerPtrs grad, const int64_t* __restrict__ sorted_keys,
+    const uint32_t* __restrict__ sorted_items, int64_t n_items,
+    const int64_t* __restrict__ seg_start, const int64_t* __restrict__ n_unique_p,
+    const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch, int scratch_width) {
+  balanced_update_body<GradT, TabT, StateT, kRowDecay>(
+      descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
+      sorted_items, n_items, seg_start, n_unique_p, opt_in, scratch, scratch_width);
+}
+
 // One lane group per chunk: if a segment that crosses the chunk's end border starts in this chunk,
 // its complete gradient sits in the chunk's scratch row: apply it, then clear the row.
-template <typename GradT>
-__global__ void __launch_bounds__(kThreads) balanced_update_kernel(const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables,
-    int n_tables, int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
-    const __grid_constant__ PeerPtrs grad, const int64_t* __restrict__ sorted_keys,
-    const uint32_t* __restrict__ sorted_items, int64_t n_items,
-    const int64_t* __restrict__ seg_start, const int64_t* __restrict__ n_unique_p,
-    const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch, int scratch_width) {
-  balanced_update_body<GradT, float, float>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
-                                    sorted_keys, sorted_items, n_items, seg_start, n_unique_p,
-                                    opt_in, scratch, scratch_width);
-}
-
-template <typename GradT, typename TabT>
-__global__ void __launch_bounds__(kThreads) balanced_update_tab16_kernel(const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables,
-    int n_tables, int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
-    const __grid_constant__ PeerPtrs grad, const int64_t* __restrict__ sorted_keys,
-    const uint32_t* __restrict__ sorted_items, int64_t n_items,
-    const int64_t* __restrict__ seg_start, const int64_t* __restrict__ n_unique_p,
-    const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch, int scratch_width) {
-  balanced_update_body<GradT, TabT, float>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
-                                    sorted_keys, sorted_items, n_items, seg_start, n_unique_p,
-                                    opt_in, scratch, scratch_width);
-}
-
-// row-wise Adagrad with weight decay on fp32, bf16 or fp16 tables (TabT)
-template <typename GradT, typename TabT>
-__global__ void __launch_bounds__(kThreads) balanced_update_rowwise_decay_kernel(const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables,
-    int n_tables, int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
-    const __grid_constant__ PeerPtrs grad, const int64_t* __restrict__ sorted_keys,
-    const uint32_t* __restrict__ sorted_items, int64_t n_items,
-    const int64_t* __restrict__ seg_start, const int64_t* __restrict__ n_unique_p,
-    const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch, int scratch_width) {
-  balanced_update_body<GradT, TabT, float, true>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
-                                    sorted_keys, sorted_items, n_items, seg_start, n_unique_p,
-                                    opt_in, scratch, scratch_width);
-}
-
-template <typename GradT, typename TabT>
-__global__ void __launch_bounds__(kThreads) balanced_update_bf16state_kernel(const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables,
-    int n_tables, int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
-    const __grid_constant__ PeerPtrs grad, const int64_t* __restrict__ sorted_keys,
-    const uint32_t* __restrict__ sorted_items, int64_t n_items,
-    const int64_t* __restrict__ seg_start, const int64_t* __restrict__ n_unique_p,
-    const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch, int scratch_width) {
-  balanced_update_body<GradT, TabT, __nv_bfloat16>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad,
-                                    sorted_keys, sorted_items, n_items, seg_start, n_unique_p,
-                                    opt_in, scratch, scratch_width);
-}
-
-template <typename TabT, typename StateT, bool kRowDecay = false>
+template <typename TabT, typename StateT, bool kRowDecay>
 __device__ __forceinline__ void finalize_crossing_body(
     const TableDesc* __restrict__ tables, int n_tables, int lpr,
     const int64_t* __restrict__ sorted_keys, int64_t n_items, const OptimizerArgs& opt_in,
@@ -630,39 +559,14 @@ __device__ __forceinline__ void finalize_crossing_body(
   }
 }
 
+template <typename TabT, typename StateT, bool kRowDecay>
 __global__ void __launch_bounds__(kThreads)
 finalize_crossing_kernel(const TableDesc* __restrict__ tables, int n_tables, int lpr,
                          const int64_t* __restrict__ sorted_keys, int64_t n_items,
                          const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch,
                          int scratch_width) {
-  finalize_crossing_body<float, float>(tables, n_tables, lpr, sorted_keys, n_items, opt_in, scratch, scratch_width);
-}
-
-template <typename TabT>
-__global__ void __launch_bounds__(kThreads)
-finalize_crossing_tab16_kernel(const TableDesc* __restrict__ tables, int n_tables, int lpr,
-                         const int64_t* __restrict__ sorted_keys, int64_t n_items,
-                         const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch,
-                         int scratch_width) {
-  finalize_crossing_body<TabT, float>(tables, n_tables, lpr, sorted_keys, n_items, opt_in, scratch, scratch_width);
-}
-
-template <typename TabT>
-__global__ void __launch_bounds__(kThreads)
-finalize_crossing_rowwise_decay_kernel(const TableDesc* __restrict__ tables, int n_tables, int lpr,
-                         const int64_t* __restrict__ sorted_keys, int64_t n_items,
-                         const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch,
-                         int scratch_width) {
-  finalize_crossing_body<TabT, float, true>(tables, n_tables, lpr, sorted_keys, n_items, opt_in, scratch, scratch_width);
-}
-
-template <typename TabT>
-__global__ void __launch_bounds__(kThreads)
-finalize_crossing_bf16state_kernel(const TableDesc* __restrict__ tables, int n_tables, int lpr,
-                         const int64_t* __restrict__ sorted_keys, int64_t n_items,
-                         const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch,
-                         int scratch_width) {
-  finalize_crossing_body<TabT, __nv_bfloat16>(tables, n_tables, lpr, sorted_keys, n_items, opt_in, scratch, scratch_width);
+  finalize_crossing_body<TabT, StateT, kRowDecay>(tables, n_tables, lpr, sorted_keys, n_items,
+                                                  opt_in, scratch, scratch_width);
 }
 
 int grid_cap(int64_t work_warps, int sm_count, int per_sm) {
@@ -673,6 +577,23 @@ int grid_cap(int64_t work_warps, int sm_count, int per_sm) {
   return static_cast<int>(blocks);
 }
 
+// The instantiation a sorted update launch takes: calls f(type_tag<TabT>, type_tag<StateT>,
+// kRowDecay).  Only Adagrad and Adam read element-wise state, so every other optimizer takes the
+// fp32-state kernels; only row-wise Adagrad with weight decay reads the weights in its
+// accumulator pass; the emit path never touches the table, so one fp32-table instantiation serves
+// every storage type.
+template <typename F>
+void with_update_types(const OptimizerArgs& opt, int table_dtype, int state_dtype, F&& f) {
+  with_dtype(opt.kind == kOptEmit ? 0 : table_dtype, [&](auto tab) {
+    if (state_dtype == 1 && (opt.kind == kOptAdagrad || opt.kind == kOptAdam))
+      f(tab, type_tag<__nv_bfloat16>{}, std::false_type{});
+    else if (opt.kind == kOptRowwiseAdagrad && opt.weight_decay != 0.f)
+      f(tab, type_tag<float>{}, std::true_type{});
+    else
+      f(tab, type_tag<float>{}, std::false_type{});
+  });
+}
+
 }  // namespace
 
 void launch_build_keys(const InputDesc* descs, const TableDesc* tables, int n_tables, int n_inputs,
@@ -681,18 +602,15 @@ void launch_build_keys(const InputDesc* descs, const TableDesc* tables, int n_ta
   if (n_inputs <= 0 || batch <= 0) return;
   const int64_t tiles = ((batch + kTile - 1) / kTile) * n_inputs;
   const int grid = grid_cap(tiles, sm_count, 8);
-#define DE_BK(IdT, KeyT)                                                                      \
-  build_keys_kernel<IdT, KeyT><<<grid, kThreads, 0, stream>>>(                                \
-      descs, tables, n_tables, n_inputs, batch, src_batch, src, reinterpret_cast<KeyT*>(keys), \
-      items)
-  if (keys32) {
-    if (ids64) DE_BK(int64_t, uint32_t);
-    else DE_BK(int32_t, uint32_t);
-  } else {
-    if (ids64) DE_BK(int64_t, int64_t);
-    else DE_BK(int32_t, int64_t);
-  }
-#undef DE_BK
+  with_type_if<int64_t, int32_t>(ids64, [&](auto id) {
+    using IdT = typename decltype(id)::type;
+    with_type_if<uint32_t, int64_t>(keys32, [&](auto key) {
+      using KeyT = typename decltype(key)::type;
+      build_keys_kernel<IdT, KeyT><<<grid, kThreads, 0, stream>>>(
+          descs, tables, n_tables, n_inputs, batch, src_batch, src, reinterpret_cast<KeyT*>(keys),
+          items);
+    });
+  });
 }
 
 size_t sort_pairs_temp_bytes(int64_t n) {
@@ -734,47 +652,6 @@ void unique_segments(void* temp, size_t temp_bytes, const int64_t* sorted_keys, 
   finish_segments_kernel<<<1, 32, 0, stream>>>(seg_start, n_unique, n);
 }
 
-template <typename GradT, int VEC, typename TabT, typename StateT>
-static void launch_seg(int grid, cudaStream_t stream, const InputDesc* descs,
-                       const TableDesc* tables, int n_tables, int lpr, int64_t batch,
-                       int64_t grad_batch, int64_t grad_stride, const PeerPtrs& grad,
-                       const int64_t* sorted_keys, const uint32_t* sorted_items,
-                       const int64_t* seg_start, const int64_t* n_unique,
-                       const OptimizerArgs& opt, int64_t* emit_keys, float* emit_rows,
-                       int emit_width, bool row_decay) {
-  if constexpr (!std::is_same<StateT, float>::value)
-    segment_update_bf16state_kernel<GradT, VEC, TabT><<<grid, kThreads, 0, stream>>>(
-        descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
-        sorted_items, seg_start, n_unique, opt, emit_keys, emit_rows, emit_width);
-  else if (row_decay)
-    segment_update_rowwise_decay_kernel<GradT, VEC, TabT><<<grid, kThreads, 0, stream>>>(
-        descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
-        sorted_items, seg_start, n_unique, opt, emit_keys, emit_rows, emit_width);
-  else if constexpr (std::is_same<TabT, float>::value)
-    segment_update_kernel<GradT, VEC><<<grid, kThreads, 0, stream>>>(
-        descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
-        sorted_items, seg_start, n_unique, opt, emit_keys, emit_rows, emit_width);
-  else
-    segment_update_tab16_kernel<GradT, VEC, TabT><<<grid, kThreads, 0, stream>>>(
-        descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
-        sorted_items, seg_start, n_unique, opt, emit_keys, emit_rows, emit_width);
-}
-#define DE_DISPATCH_SEG(GradT, VEC, TabT, StateT)                                              \
-  launch_seg<GradT, VEC, TabT, StateT>(grid, stream, descs, tables, n_tables, lpr, batch, grad_batch,  \
-                               grad_stride, grad, sorted_keys, sorted_items, seg_start,        \
-                               n_unique, opt, emit_keys, emit_rows, emit_width, row_decay)
-#define DE_DISPATCH_SEG_G(VEC, TabT, StateT)                                                   \
-  do {                                                                                         \
-    if (act_dtype == 1) DE_DISPATCH_SEG(__nv_bfloat16, VEC, TabT, StateT);                     \
-    else if (act_dtype == 2) DE_DISPATCH_SEG(__half, VEC, TabT, StateT);                       \
-    else DE_DISPATCH_SEG(float, VEC, TabT, StateT);                                            \
-  } while (0)
-#define DE_DISPATCH_SEG_V(TabT, StateT)                                                        \
-  do {                                                                                         \
-    if (vec4) DE_DISPATCH_SEG_G(4, TabT, StateT);                                              \
-    else DE_DISPATCH_SEG_G(1, TabT, StateT);                                                   \
-  } while (0)
-
 void launch_segment_update(const InputDesc* descs, const TableDesc* tables, int n_tables,
                            int64_t batch, int64_t grad_batch, int64_t grad_stride,
                            const PeerPtrs& grad, const int64_t* sorted_keys,
@@ -796,78 +673,22 @@ void launch_segment_update(const InputDesc* descs, const TableDesc* tables, int 
   const int rpw = 32 / lpr;
   const int64_t warps = (n_items + rpw - 1) / rpw;
   const int grid = grid_cap(warps, sm_count, 8);
-  const bool row_decay = opt.kind == kOptRowwiseAdagrad && opt.weight_decay != 0.f;
-  // the emit path never touches the table: one instantiation serves every storage type; only
-  // Adagrad and Adam read element-wise state, every other optimizer takes the fp32-state kernels
-  if (state_dtype == 1 && (opt.kind == kOptAdagrad || opt.kind == kOptAdam)) {
-    if (table_dtype == 1) DE_DISPATCH_SEG_V(__nv_bfloat16, __nv_bfloat16);
-    else if (table_dtype == 2) DE_DISPATCH_SEG_V(__half, __nv_bfloat16);
-    else DE_DISPATCH_SEG_V(float, __nv_bfloat16);
-  } else if (table_dtype == 1 && opt.kind != kOptEmit) DE_DISPATCH_SEG_V(__nv_bfloat16, float);
-  else if (table_dtype == 2 && opt.kind != kOptEmit) DE_DISPATCH_SEG_V(__half, float);
-  else DE_DISPATCH_SEG_V(float, float);
-}
-
-template <typename GradT, typename TabT, typename StateT>
-static void launch_balanced_g(const InputDesc* descs, const TableDesc* tables, int n_tables,
-                              int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
-                              const PeerPtrs& grad, const int64_t* sorted_keys,
-                              const uint32_t* sorted_items, int64_t n_items,
-                              const int64_t* seg_start, const int64_t* n_unique,
-                              const OptimizerArgs& opt, float* scratch, int scratch_width,
-                              int grid, cudaStream_t stream, bool row_decay) {
-  if constexpr (!std::is_same<StateT, float>::value)
-    balanced_update_bf16state_kernel<GradT, TabT><<<grid, kThreads, 0, stream>>>(
-        descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
-        sorted_items, n_items, seg_start, n_unique, opt, scratch, scratch_width);
-  else if (row_decay)
-    balanced_update_rowwise_decay_kernel<GradT, TabT><<<grid, kThreads, 0, stream>>>(
-        descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
-        sorted_items, n_items, seg_start, n_unique, opt, scratch, scratch_width);
-  else if constexpr (std::is_same<TabT, float>::value)
-    balanced_update_kernel<GradT><<<grid, kThreads, 0, stream>>>(
-        descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
-        sorted_items, n_items, seg_start, n_unique, opt, scratch, scratch_width);
-  else
-    balanced_update_tab16_kernel<GradT, TabT><<<grid, kThreads, 0, stream>>>(
-        descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
-        sorted_items, n_items, seg_start, n_unique, opt, scratch, scratch_width);
-}
-
-template <typename TabT, typename StateT>
-static void launch_balanced(const InputDesc* descs, const TableDesc* tables, int n_tables, int lpr,
-                            int64_t batch, int64_t grad_batch, int64_t grad_stride,
-                            const PeerPtrs& grad, const int64_t* sorted_keys,
-                            const uint32_t* sorted_items, int64_t n_items,
-                            const int64_t* seg_start, const int64_t* n_unique,
-                            const OptimizerArgs& opt, float* scratch, int scratch_width,
-                            int act_dtype, int grid, cudaStream_t stream) {
-  const bool row_decay = opt.kind == kOptRowwiseAdagrad && opt.weight_decay != 0.f;
-  if (act_dtype == 1)
-    launch_balanced_g<__nv_bfloat16, TabT, StateT>(descs, tables, n_tables, lpr, batch, grad_batch,
-                                           grad_stride, grad, sorted_keys, sorted_items, n_items,
-                                           seg_start, n_unique, opt, scratch, scratch_width, grid,
-                                           stream, row_decay);
-  else if (act_dtype == 2)
-    launch_balanced_g<__half, TabT, StateT>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride,
-                                    grad, sorted_keys, sorted_items, n_items, seg_start, n_unique,
-                                    opt, scratch, scratch_width, grid, stream, row_decay);
-  else
-    launch_balanced_g<float, TabT, StateT>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride,
-                                   grad, sorted_keys, sorted_items, n_items, seg_start, n_unique,
-                                   opt, scratch, scratch_width, grid, stream, row_decay);
-  if constexpr (!std::is_same<StateT, float>::value)
-    finalize_crossing_bf16state_kernel<TabT><<<grid, kThreads, 0, stream>>>(
-        tables, n_tables, lpr, sorted_keys, n_items, opt, scratch, scratch_width);
-  else if (row_decay)
-    finalize_crossing_rowwise_decay_kernel<TabT><<<grid, kThreads, 0, stream>>>(
-        tables, n_tables, lpr, sorted_keys, n_items, opt, scratch, scratch_width);
-  else if constexpr (std::is_same<TabT, float>::value)
-    finalize_crossing_kernel<<<grid, kThreads, 0, stream>>>(tables, n_tables, lpr, sorted_keys,
-                                                            n_items, opt, scratch, scratch_width);
-  else
-    finalize_crossing_tab16_kernel<TabT><<<grid, kThreads, 0, stream>>>(
-        tables, n_tables, lpr, sorted_keys, n_items, opt, scratch, scratch_width);
+  with_update_types(opt, table_dtype, state_dtype, [&](auto tab, auto state, auto row_decay) {
+    using TabT = typename decltype(tab)::type;
+    using StateT = typename decltype(state)::type;
+    constexpr bool kRowDecay = decltype(row_decay)::value;
+    with_dtype(act_dtype, [&](auto grad_t) {
+      using GradT = typename decltype(grad_t)::type;
+      auto launch = [&](auto kernel) {
+        kernel<<<grid, kThreads, 0, stream>>>(descs, tables, n_tables, lpr, batch, grad_batch,
+                                              grad_stride, grad, sorted_keys, sorted_items,
+                                              seg_start, n_unique, opt, emit_keys, emit_rows,
+                                              emit_width);
+      };
+      if (vec4) launch(segment_update_kernel<GradT, 4, TabT, StateT, kRowDecay>);
+      else launch(segment_update_kernel<GradT, 1, TabT, StateT, kRowDecay>);
+    });
+  });
 }
 
 // Occurrence-balanced variant (vec4, tables up to 128 columns wide, fused optimizers only).
@@ -888,22 +709,19 @@ bool launch_balanced_update(const InputDesc* descs, const TableDesc* tables, int
   const int rpw = 32 / lpr;
   const int64_t n_chunks = (n_items + kChunk - 1) / kChunk;
   const int grid = grid_cap((n_chunks + rpw - 1) / rpw, sm_count, 8);
-#define DE_BAL(TabT, StateT)                                                                   \
-  launch_balanced<TabT, StateT>(descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, \
-                                grad, sorted_keys, sorted_items, n_items, seg_start, n_unique, \
-                                opt, scratch, scratch_width, act_dtype, grid, stream)
-  if (state_dtype == 1 && (opt.kind == kOptAdagrad || opt.kind == kOptAdam)) {
-    if (table_dtype == 1) DE_BAL(__nv_bfloat16, __nv_bfloat16);
-    else if (table_dtype == 2) DE_BAL(__half, __nv_bfloat16);
-    else DE_BAL(float, __nv_bfloat16);
-  } else if (table_dtype == 1) {
-    DE_BAL(__nv_bfloat16, float);
-  } else if (table_dtype == 2) {
-    DE_BAL(__half, float);
-  } else {
-    DE_BAL(float, float);
-  }
-#undef DE_BAL
+  with_update_types(opt, table_dtype, state_dtype, [&](auto tab, auto state, auto row_decay) {
+    using TabT = typename decltype(tab)::type;
+    using StateT = typename decltype(state)::type;
+    constexpr bool kRowDecay = decltype(row_decay)::value;
+    with_dtype(act_dtype, [&](auto grad_t) {
+      using GradT = typename decltype(grad_t)::type;
+      balanced_update_kernel<GradT, TabT, StateT, kRowDecay><<<grid, kThreads, 0, stream>>>(
+          descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
+          sorted_items, n_items, seg_start, n_unique, opt, scratch, scratch_width);
+    });
+    finalize_crossing_kernel<TabT, StateT, kRowDecay><<<grid, kThreads, 0, stream>>>(
+        tables, n_tables, lpr, sorted_keys, n_items, opt, scratch, scratch_width);
+  });
   return cudaGetLastError() == cudaSuccess;
 }
 

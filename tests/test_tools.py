@@ -77,7 +77,7 @@ def test_resource_usage_lists_the_hot_kernels():
     pytest.skip("extension not built")
   out = _run("tools/resource_usage.py")
   assert out.returncode == 0, out.stderr[-1000:]
-  for k in ("lookup_fwd_kernel<int, __nv_bfloat16, 4>", "scatter_add_staged_kernel",
+  for k in ("lookup_fwd_kernel<int, __nv_bfloat16, 4, float>", "scatter_add_staged_kernel",
             "interact_bwd_v2_kernel<128>", "stream_push_kernel", "gemm_tn_pair_kernel",
             "digit_scatter_kernel", "integer_lookup_kernel"):
     assert k in out.stdout, k

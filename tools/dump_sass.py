@@ -21,8 +21,8 @@ OUT = os.path.join(os.getcwd(), "sass")
 
 # (file stem, regex on the demangled name): the instantiations the DLRM / synthetic steps run
 HOT = [
-    ("lookup_fwd_i32_bf16_v4", r"lookup_fwd_kernel<int, __nv_bfloat16, 4>"),
-    ("lookup_fwd_i32_f32_v4", r"lookup_fwd_kernel<int, float, 4>"),
+    ("lookup_fwd_i32_bf16_v4", r"lookup_fwd_kernel<int, __nv_bfloat16, 4, float>"),
+    ("lookup_fwd_i32_f32_v4", r"lookup_fwd_kernel<int, float, 4, float>"),
     ("scatter_add_bwd_i32_bf16_v4", r"scatter_add_bwd_kernel<int, __nv_bfloat16, 4>"),
     ("push_segments_i32", r"push_segments_kernel<int>"),
     ("push_grad_bf16_bf16", r"push_grad_kernel<__nv_bfloat16, __nv_bfloat16>"),
@@ -33,8 +33,8 @@ HOT = [
     ("interact_bwd_apply_128", r"interact_bwd_apply_kernel<128>"),
     ("allreduce_p2p_f32", r"allreduce_p2p_kernel<(false|0)>"),
     ("allreduce_multimem_f32", r"allreduce_multimem_kernel<(false|0)>"),
-    ("segment_update_bf16_v4", r"segment_update_kernel<__nv_bfloat16, 4>"),
-    ("balanced_update_bf16", r"balanced_update_kernel<__nv_bfloat16>"),
+    ("segment_update_bf16_v4", r"segment_update_kernel<__nv_bfloat16, 4, float, float, 0>"),
+    ("balanced_update_bf16", r"balanced_update_kernel<__nv_bfloat16, float, float, 0>"),
     ("scatter_add_staged_i32_bf16", r"scatter_add_staged_kernel<int, __nv_bfloat16>"),
     ("stream_push", r"stream_push_kernel"),
     ("build_keys_i32_u32", r"build_keys_kernel<int, unsigned int>"),
