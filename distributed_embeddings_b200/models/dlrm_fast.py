@@ -175,6 +175,11 @@ class DLRMTrainStep:
     pos = 0
     if len(self.emb.dp_layers):
       if embedding_optimizer.lower() != self.dense_cfg["kind"]:
+        if embedding_optimizer.lower().startswith("rowwise_"):
+          raise ValueError(
+              f"replicated tables in the fast step are updated by the dense optimizer kernel, "
+              f"which has no row-wise form: embedding_optimizer={embedding_optimizer!r} needs "
+              f"data_parallel_threshold=None (no replicated tables)")
         raise ValueError("replicated tables in the fast step are updated by the dense optimizer "
                          "kernel: use the same embedding_optimizer and dense_optimizer ('sgd', "
                          "'adagrad' or 'adam') or data_parallel_threshold=None")

@@ -76,14 +76,22 @@ struct alignas(16) GradRoute {
   int32_t pad;
 };
 
-enum OptimizerKind : int32_t { kOptSGD = 0, kOptAdagrad = 1, kOptRowwiseAdagrad = 2, kOptAdam = 3, kOptEmit = 4 };
+enum OptimizerKind : int32_t {
+  kOptSGD = 0,
+  kOptAdagrad = 1,
+  kOptRowwiseAdagrad = 2,
+  kOptAdam = 3,
+  kOptEmit = 4,
+  kOptRowwiseAdam = 5,  // Adam with element-wise m (state0) and one fp32 v word per row (state1)
+};
 
 // One entry per (fused) local table, used by the sorted/deduplicated update path.
 struct alignas(16) TableDesc {
   void* weight;       // [rows, width]; fp32, bf16 or fp16 (`table_dtype` of the launch)
-  void* state0;       // Adagrad accumulator [rows,width] / row-wise [rows] / Adam m
-  void* state1;       // Adam v  (element-wise state: fp32 or bf16, `state_dtype` of the launch;
-                      // row-wise state is always fp32)
+  void* state0;       // Adagrad accumulator [rows,width] / row-wise [rows] / Adam m / row-wise
+                      // Adam m
+  void* state1;       // Adam v / row-wise Adam v [rows]  (element-wise state: fp32 or bf16,
+                      // `state_dtype` of the launch; row-wise state is always fp32)
   int64_t rows;
   int64_t key_base;   // first global row key of this table (prefix sum of rows)
   int32_t width;

@@ -1,8 +1,8 @@
 // Deduplicated sparse backward for sm_90a: (row key, item) pairs -> radix sort -> unique
 // segments -> one lane group per unique row sums its gradient rows (pulled from peer-mapped
 // gradient buffers when world_size > 1) and applies the optimizer update in place
-// (SGD / Adagrad / row-wise Adagrad / lazy Adam), or emits (unique_ids, unique_grad) for an
-// external optimizer.  The unique count never leaves the device (the reference copies it to the
+// (SGD / Adagrad / row-wise Adagrad / lazy Adam / lazy row-wise Adam), or emits
+// (unique_ids, unique_grad) for an external optimizer.  The unique count never leaves the device (the reference copies it to the
 // host to size its output: cc/kernels/embedding_lookup_kernels.cu:663-670).
 //
 // Capability parity: OffsetToWeightsAndRowId + cub sort/unique + segment reduce
@@ -82,10 +82,17 @@ __global__ void finish_segments_kernel(int64_t* seg_start, const int64_t* n_uniq
   if (threadIdx.x == 0 && blockIdx.x == 0) seg_start[*n_unique] = n;
 }
 
+// The row pass of the sorted update kernels, their template parameter kRow (a bit set).  A launch
+// that needs neither bit takes the kRow = 0 instantiation; the bits give the row-wise optimizers
+// instantiations of their own, so the others keep their code and registers.
+constexpr int kRowDecay = 1;  // weight decay on: the row pass reads the weights (s * g + wd * w)
+constexpr int kRowAdam = 2;   // row-wise Adam (kind kOptRowwiseAdam)
+
 // Adam bias corrections from a device-resident step count (the host scalars baked into a captured
 // CUDA graph would freeze at their capture-time values).
+template <int kRow = 0>
 __device__ __forceinline__ void resolve_step(OptimizerArgs& opt) {
-  if (opt.step_ptr != nullptr && opt.kind == kOptAdam) {
+  if (opt.step_ptr != nullptr && ((kRow & kRowAdam) || opt.kind == kOptAdam)) {
     const float t = *opt.step_ptr;
     opt.bias1 = 1.f - powf(opt.beta1, t);
     opt.bias2 = 1.f - powf(opt.beta2, t);
@@ -111,8 +118,9 @@ __device__ __forceinline__ uint32_t rounding_step(const OptimizerArgs& opt) {
 // in its own (StateT: fp32 or bf16), both widened to fp32; the optimizer runs in fp32, the weight
 // update uses the unrounded new state, and 16-bit weights and state are written back with
 // stochastic rounding (st_tab), each from its own random stream.  Every row has exactly one
-// writer per step, so each element is rounded once.  Row-wise Adagrad state is always fp32.
-template <typename TabT, int VEC, typename StateT = float>
+// writer per step, so each element is rounded once.  Row-wise state (row-wise Adagrad's
+// accumulator, row-wise Adam's v) is always fp32.
+template <typename TabT, int VEC, typename StateT = float, int kRow = 0>
 __device__ __forceinline__ void apply_update(const TableDesc& T, const OptimizerArgs& opt,
                                              int64_t row, int col, const FVec<VEC>& g,
                                              float row_sumsq_mean, uint32_t step) {
@@ -120,7 +128,20 @@ __device__ __forceinline__ void apply_update(const TableDesc& T, const Optimizer
   FVec<VEC> wv = ld_tab_rw<TabT, VEC>(w);
   FVec<VEC> gv = g;
   if (opt.weight_decay != 0.f) gv.fma(opt.weight_decay, wv);
-  if (opt.kind == kOptSGD) {
+  if constexpr ((kRow & kRowAdam) != 0) {
+    // row-wise Adam: m element-wise; row_sumsq_mean carries the row's new v (the caller advanced
+    // state1[row])
+    StateT* m = reinterpret_cast<StateT*>(T.state0) + row * T.width + col;
+    FVec<VEC> mv = ld_tab_rw<StateT, VEC>(m);
+    const float denom = sqrtf(row_sumsq_mean / opt.bias2) + opt.eps;
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) {
+      mv.v[i] = opt.beta1 * mv.v[i] + (1.f - opt.beta1) * gv.v[i];
+      const float mh = mv.v[i] / opt.bias1;
+      wv.v[i] -= opt.lr * mh / denom;
+    }
+    st_tab<StateT, VEC>(m, mv, step, T.key_base + row, col, kStreamState0);
+  } else if (opt.kind == kOptSGD) {
     wv.fma(-opt.lr, gv);
   } else if (opt.kind == kOptAdagrad) {
     StateT* a = reinterpret_cast<StateT*>(T.state0) + row * T.width + col;
@@ -205,12 +226,12 @@ __device__ __forceinline__ FVec<VEC> reduce_segment(const InputDesc* __restrict_
 }
 
 // One lane group per unique row.  TabT is the table's storage type, StateT that of the Adagrad /
-// Adam state; with_update_types() below says which combinations a launch takes.
-// kRowDecay: row-wise Adagrad with weight decay.  Its accumulator takes the row mean of the
-// squared decayed gradient (s * g + weight_decay * w), the gradient apply_update applies, so pass 1
-// reads the weights.  Those launches get instantiations of their own: the others keep their code
-// and registers.
-template <typename GradT, int VEC, typename TabT, typename StateT, bool kRowDecay>
+// Adam / row-wise Adam m state; with_update_types() below says which combinations a launch takes.
+// Row-wise Adagrad and row-wise Adam first reduce the row mean of the squared gradient over the
+// lane group (pass 1) into their fp32 word per row.  With weight decay (kRow & kRowDecay) that is
+// the decayed gradient (s * g + weight_decay * w), the gradient apply_update applies, so pass 1
+// reads the weights.
+template <typename GradT, int VEC, typename TabT, typename StateT, int kRow>
 __device__ __forceinline__ void segment_update_body(
     const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables, int n_tables,
     int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride, const PeerPtrs& grad,
@@ -220,7 +241,7 @@ __device__ __forceinline__ void segment_update_body(
     int emit_width) {
   OptimizerArgs opt = opt_in;
   if (opt.lr_ptr != nullptr) opt.lr = *opt.lr_ptr;
-  resolve_step(opt);
+  resolve_step<kRow>(opt);
   const uint32_t sr_step = rounding_step<TabT, StateT>(opt);
   const int64_t n_unique = *n_unique_p;
   const int64_t sentinel = tables[n_tables - 1].key_base + tables[n_tables - 1].rows;
@@ -251,7 +272,7 @@ __device__ __forceinline__ void segment_update_body(
     const int nvec = (W + VEC - 1) / VEC;
 
     float row_state = 0.f;
-    if (opt.kind == kOptRowwiseAdagrad) {
+    if ((kRow & kRowAdam) || opt.kind == kOptRowwiseAdagrad) {
       // pass 1: mean of squared (scaled) gradient over the whole row
       float ss = 0.f;
       if (valid) {
@@ -260,7 +281,7 @@ __device__ __forceinline__ void segment_update_body(
           if (cv < nvec) {
             FVec<VEC> g = reduce_segment<GradT, VEC>(descs, sorted_items, k0, k1, batch,
                                                      grad_batch, grad_stride, grad, cv * VEC);
-            if constexpr (kRowDecay) {
+            if constexpr ((kRow & kRowDecay) != 0) {
               // the same fp32 operations as apply_update, so the same values
               g.scale(opt.grad_scale);
               g.fma(opt.weight_decay,
@@ -280,8 +301,11 @@ __device__ __forceinline__ void segment_update_body(
       }
       for (int off = lpr >> 1; off > 0; off >>= 1) ss += __shfl_xor_sync(group_mask, ss, off);
       if (valid) {
-        float* st = reinterpret_cast<float*>(T.state0) + row;
-        row_state = *st + ss / static_cast<float>(W);
+        float* st = reinterpret_cast<float*>((kRow & kRowAdam) ? T.state1 : T.state0) + row;
+        if constexpr ((kRow & kRowAdam) != 0)
+          row_state = opt.beta2 * *st + (1.f - opt.beta2) * (ss / static_cast<float>(W));
+        else
+          row_state = *st + ss / static_cast<float>(W);
         if (li == 0) *st = row_state;
       }
       __syncwarp(group_mask);
@@ -301,7 +325,7 @@ __device__ __forceinline__ void segment_update_body(
       if (opt.kind == kOptEmit) {
         st_f32<VEC>(emit_rows + u * emit_width + col, g);
       } else {
-        apply_update<TabT, VEC, StateT>(T, opt, row, col, g, row_state, sr_step);
+        apply_update<TabT, VEC, StateT, kRow>(T, opt, row, col, g, row_state, sr_step);
       }
     }
   }
@@ -309,7 +333,7 @@ __device__ __forceinline__ void segment_update_body(
 
 // The bodies of the three update kernels stay separate inlined functions: folded into the kernels,
 // they get a different register allocation from ptxas.
-template <typename GradT, int VEC, typename TabT, typename StateT, bool kRowDecay>
+template <typename GradT, int VEC, typename TabT, typename StateT, int kRow>
 __global__ void __launch_bounds__(kThreads) segment_update_kernel(
     const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables, int n_tables,
     int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
@@ -317,7 +341,7 @@ __global__ void __launch_bounds__(kThreads) segment_update_kernel(
     const uint32_t* __restrict__ sorted_items, const int64_t* __restrict__ seg_start,
     const int64_t* __restrict__ n_unique_p, const __grid_constant__ OptimizerArgs opt_in,
     int64_t* __restrict__ emit_keys, float* __restrict__ emit_rows, int emit_width) {
-  segment_update_body<GradT, VEC, TabT, StateT, kRowDecay>(
+  segment_update_body<GradT, VEC, TabT, StateT, kRow>(
       descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
       sorted_items, seg_start, n_unique_p, opt_in, emit_keys, emit_rows, emit_width);
 }
@@ -377,18 +401,18 @@ __device__ __forceinline__ int find_table(const TableDesc* __restrict__ tables, 
 }
 
 // Apply the optimizer to one row given the complete (scaled) gradient fragment of this lane.
-// kRowDecay: row-wise Adagrad with weight decay (see segment_update_kernel).
-template <typename TabT, typename StateT, bool kRowDecay = false>
+// kRow: the row pass of row-wise Adagrad / row-wise Adam (see segment_update_body).
+template <typename TabT, typename StateT, int kRow = 0>
 __device__ __forceinline__ void apply_row(const TableDesc& T, const OptimizerArgs& opt,
                                           int64_t row, int col, FVec<4> g, int lpr,
                                           unsigned group_mask, uint32_t step) {
   const bool col_ok = col < T.width;
   float row_state = 0.f;
-  if (opt.kind == kOptRowwiseAdagrad) {
+  if ((kRow & kRowAdam) || opt.kind == kOptRowwiseAdagrad) {
     float ss = 0.f;
     if (col_ok) {
-      if constexpr (kRowDecay) {
-        // the accumulator takes the gradient apply_update applies: g + weight_decay * w
+      if constexpr ((kRow & kRowDecay) != 0) {
+        // the row word takes the gradient apply_update applies: g + weight_decay * w
         FVec<4> gd = g;
         gd.fma(opt.weight_decay,
                ld_tab_rw<TabT, 4>(reinterpret_cast<const TabT*>(T.weight) + row * T.width + col));
@@ -400,15 +424,18 @@ __device__ __forceinline__ void apply_row(const TableDesc& T, const OptimizerArg
       }
     }
     for (int off = lpr >> 1; off > 0; off >>= 1) ss += __shfl_xor_sync(group_mask, ss, off);
-    float* st = reinterpret_cast<float*>(T.state0) + row;
-    row_state = *st + ss / static_cast<float>(T.width);
+    float* st = reinterpret_cast<float*>((kRow & kRowAdam) ? T.state1 : T.state0) + row;
+    if constexpr ((kRow & kRowAdam) != 0)
+      row_state = opt.beta2 * *st + (1.f - opt.beta2) * (ss / static_cast<float>(T.width));
+    else
+      row_state = *st + ss / static_cast<float>(T.width);
     __syncwarp(group_mask);
     if (col == 0) *st = row_state;
   }
-  if (col_ok) apply_update<TabT, 4, StateT>(T, opt, row, col, g, row_state, step);
+  if (col_ok) apply_update<TabT, 4, StateT, kRow>(T, opt, row, col, g, row_state, step);
 }
 
-template <typename GradT, typename TabT, typename StateT, bool kRowDecay>
+template <typename GradT, typename TabT, typename StateT, int kRow>
 __device__ __forceinline__ void balanced_update_body(
     const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables, int n_tables,
     int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride, const PeerPtrs& grad,
@@ -417,7 +444,7 @@ __device__ __forceinline__ void balanced_update_body(
     const OptimizerArgs& opt_in, float* __restrict__ scratch, int scratch_width) {
   OptimizerArgs opt = opt_in;
   if (opt.lr_ptr != nullptr) opt.lr = *opt.lr_ptr;
-  resolve_step(opt);
+  resolve_step<kRow>(opt);
   const uint32_t sr_step = rounding_step<TabT, StateT>(opt);
   const int64_t n_unique = *n_unique_p;
   const int64_t sentinel = tables[n_tables - 1].key_base + tables[n_tables - 1].rows;
@@ -470,7 +497,7 @@ __device__ __forceinline__ void balanced_update_body(
             FVec<4> g = acc;
             g.scale(opt.grad_scale);
             if (start_done) {
-              apply_row<TabT, StateT, kRowDecay>(T, opt, run_key - T.key_base, col, g, lpr, group_mask, sr_step);
+              apply_row<TabT, StateT, kRow>(T, opt, run_key - T.key_base, col, g, lpr, group_mask, sr_step);
             } else if (col < T.width) {
               // continues a segment that started in an earlier chunk: that chunk owns the slot
               const int64_t s = segment_start_of(seg_start, n_unique, k0);
@@ -493,7 +520,7 @@ __device__ __forceinline__ void balanced_update_body(
       FVec<4> g = acc;
       g.scale(opt.grad_scale);
       if (start_done && end_done) {
-        apply_row<TabT, StateT, kRowDecay>(T, opt, run_key - T.key_base, col, g, lpr, group_mask, sr_step);
+        apply_row<TabT, StateT, kRow>(T, opt, run_key - T.key_base, col, g, lpr, group_mask, sr_step);
       } else if (col < T.width) {
         const int64_t s = start_done ? run_start : segment_start_of(seg_start, n_unique, k0);
         red_add_f32<4>(scratch + (s / kChunk) * scratch_width + col, g);
@@ -502,7 +529,7 @@ __device__ __forceinline__ void balanced_update_body(
   }
 }
 
-template <typename GradT, typename TabT, typename StateT, bool kRowDecay>
+template <typename GradT, typename TabT, typename StateT, int kRow>
 __global__ void __launch_bounds__(kThreads) balanced_update_kernel(
     const InputDesc* __restrict__ descs, const TableDesc* __restrict__ tables, int n_tables,
     int lpr, int64_t batch, int64_t grad_batch, int64_t grad_stride,
@@ -510,21 +537,21 @@ __global__ void __launch_bounds__(kThreads) balanced_update_kernel(
     const uint32_t* __restrict__ sorted_items, int64_t n_items,
     const int64_t* __restrict__ seg_start, const int64_t* __restrict__ n_unique_p,
     const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch, int scratch_width) {
-  balanced_update_body<GradT, TabT, StateT, kRowDecay>(
+  balanced_update_body<GradT, TabT, StateT, kRow>(
       descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
       sorted_items, n_items, seg_start, n_unique_p, opt_in, scratch, scratch_width);
 }
 
 // One lane group per chunk: if a segment that crosses the chunk's end border starts in this chunk,
 // its complete gradient sits in the chunk's scratch row: apply it, then clear the row.
-template <typename TabT, typename StateT, bool kRowDecay>
+template <typename TabT, typename StateT, int kRow>
 __device__ __forceinline__ void finalize_crossing_body(
     const TableDesc* __restrict__ tables, int n_tables, int lpr,
     const int64_t* __restrict__ sorted_keys, int64_t n_items, const OptimizerArgs& opt_in,
     float* __restrict__ scratch, int scratch_width) {
   OptimizerArgs opt = opt_in;
   if (opt.lr_ptr != nullptr) opt.lr = *opt.lr_ptr;
-  resolve_step(opt);
+  resolve_step<kRow>(opt);
   const uint32_t sr_step = rounding_step<TabT, StateT>(opt);
   const int64_t sentinel = tables[n_tables - 1].key_base + tables[n_tables - 1].rows;
   const int lane = threadIdx.x & 31;
@@ -555,17 +582,17 @@ __device__ __forceinline__ void finalize_crossing_body(
       z.zero();
       st_f32<4>(sp, z);
     }
-    apply_row<TabT, StateT, kRowDecay>(T, opt, key - T.key_base, col, g, lpr, group_mask, sr_step);
+    apply_row<TabT, StateT, kRow>(T, opt, key - T.key_base, col, g, lpr, group_mask, sr_step);
   }
 }
 
-template <typename TabT, typename StateT, bool kRowDecay>
+template <typename TabT, typename StateT, int kRow>
 __global__ void __launch_bounds__(kThreads)
 finalize_crossing_kernel(const TableDesc* __restrict__ tables, int n_tables, int lpr,
                          const int64_t* __restrict__ sorted_keys, int64_t n_items,
                          const __grid_constant__ OptimizerArgs opt_in, float* __restrict__ scratch,
                          int scratch_width) {
-  finalize_crossing_body<TabT, StateT, kRowDecay>(tables, n_tables, lpr, sorted_keys, n_items,
+  finalize_crossing_body<TabT, StateT, kRow>(tables, n_tables, lpr, sorted_keys, n_items,
                                                   opt_in, scratch, scratch_width);
 }
 
@@ -578,19 +605,28 @@ int grid_cap(int64_t work_warps, int sm_count, int per_sm) {
 }
 
 // The instantiation a sorted update launch takes: calls f(type_tag<TabT>, type_tag<StateT>,
-// kRowDecay).  Only Adagrad and Adam read element-wise state, so every other optimizer takes the
-// fp32-state kernels; only row-wise Adagrad with weight decay reads the weights in its
-// accumulator pass; the emit path never touches the table, so one fp32-table instantiation serves
-// every storage type.
+// kRow).  Only Adagrad, Adam and row-wise Adam read element-wise state, so every other optimizer
+// takes the fp32-state kernels; row-wise Adam has kernels of its own (kRowAdam); only the row-wise
+// optimizers with weight decay read the weights in their row pass (kRowDecay); the emit path never
+// touches the table, so one fp32-table instantiation serves every storage type.
 template <typename F>
 void with_update_types(const OptimizerArgs& opt, int table_dtype, int state_dtype, F&& f) {
+  using Plain = std::integral_constant<int, 0>;
   with_dtype(opt.kind == kOptEmit ? 0 : table_dtype, [&](auto tab) {
-    if (state_dtype == 1 && (opt.kind == kOptAdagrad || opt.kind == kOptAdam))
-      f(tab, type_tag<__nv_bfloat16>{}, std::false_type{});
-    else if (opt.kind == kOptRowwiseAdagrad && opt.weight_decay != 0.f)
-      f(tab, type_tag<float>{}, std::true_type{});
-    else
-      f(tab, type_tag<float>{}, std::false_type{});
+    if (opt.kind == kOptRowwiseAdam) {
+      with_type_if<__nv_bfloat16, float>(state_dtype == 1, [&](auto state) {
+        if (opt.weight_decay != 0.f)
+          f(tab, state, std::integral_constant<int, kRowAdam | kRowDecay>{});
+        else
+          f(tab, state, std::integral_constant<int, kRowAdam>{});
+      });
+    } else if (state_dtype == 1 && (opt.kind == kOptAdagrad || opt.kind == kOptAdam)) {
+      f(tab, type_tag<__nv_bfloat16>{}, Plain{});
+    } else if (opt.kind == kOptRowwiseAdagrad && opt.weight_decay != 0.f) {
+      f(tab, type_tag<float>{}, std::integral_constant<int, kRowDecay>{});
+    } else {
+      f(tab, type_tag<float>{}, Plain{});
+    }
   });
 }
 
@@ -673,10 +709,10 @@ void launch_segment_update(const InputDesc* descs, const TableDesc* tables, int 
   const int rpw = 32 / lpr;
   const int64_t warps = (n_items + rpw - 1) / rpw;
   const int grid = grid_cap(warps, sm_count, 8);
-  with_update_types(opt, table_dtype, state_dtype, [&](auto tab, auto state, auto row_decay) {
+  with_update_types(opt, table_dtype, state_dtype, [&](auto tab, auto state, auto row_pass) {
     using TabT = typename decltype(tab)::type;
     using StateT = typename decltype(state)::type;
-    constexpr bool kRowDecay = decltype(row_decay)::value;
+    constexpr int kRow = decltype(row_pass)::value;
     with_dtype(act_dtype, [&](auto grad_t) {
       using GradT = typename decltype(grad_t)::type;
       auto launch = [&](auto kernel) {
@@ -685,8 +721,8 @@ void launch_segment_update(const InputDesc* descs, const TableDesc* tables, int 
                                               seg_start, n_unique, opt, emit_keys, emit_rows,
                                               emit_width);
       };
-      if (vec4) launch(segment_update_kernel<GradT, 4, TabT, StateT, kRowDecay>);
-      else launch(segment_update_kernel<GradT, 1, TabT, StateT, kRowDecay>);
+      if (vec4) launch(segment_update_kernel<GradT, 4, TabT, StateT, kRow>);
+      else launch(segment_update_kernel<GradT, 1, TabT, StateT, kRow>);
     });
   });
 }
@@ -709,17 +745,17 @@ bool launch_balanced_update(const InputDesc* descs, const TableDesc* tables, int
   const int rpw = 32 / lpr;
   const int64_t n_chunks = (n_items + kChunk - 1) / kChunk;
   const int grid = grid_cap((n_chunks + rpw - 1) / rpw, sm_count, 8);
-  with_update_types(opt, table_dtype, state_dtype, [&](auto tab, auto state, auto row_decay) {
+  with_update_types(opt, table_dtype, state_dtype, [&](auto tab, auto state, auto row_pass) {
     using TabT = typename decltype(tab)::type;
     using StateT = typename decltype(state)::type;
-    constexpr bool kRowDecay = decltype(row_decay)::value;
+    constexpr int kRow = decltype(row_pass)::value;
     with_dtype(act_dtype, [&](auto grad_t) {
       using GradT = typename decltype(grad_t)::type;
-      balanced_update_kernel<GradT, TabT, StateT, kRowDecay><<<grid, kThreads, 0, stream>>>(
+      balanced_update_kernel<GradT, TabT, StateT, kRow><<<grid, kThreads, 0, stream>>>(
           descs, tables, n_tables, lpr, batch, grad_batch, grad_stride, grad, sorted_keys,
           sorted_items, n_items, seg_start, n_unique, opt, scratch, scratch_width);
     });
-    finalize_crossing_kernel<TabT, StateT, kRowDecay><<<grid, kThreads, 0, stream>>>(
+    finalize_crossing_kernel<TabT, StateT, kRow><<<grid, kThreads, 0, stream>>>(
         tables, n_tables, lpr, sorted_keys, n_items, opt, scratch, scratch_width);
   });
   return cudaGetLastError() == cudaSuccess;

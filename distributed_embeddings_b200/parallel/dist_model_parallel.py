@@ -17,7 +17,7 @@ reference (``DistributedEmbedding`` :712-1214, hybrid helpers :1217-1329).
 from __future__ import annotations
 
 import os
-from typing import Any, Dict, List, Optional, Sequence, Union
+from typing import Any, Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
@@ -596,11 +596,17 @@ class DistributedEmbedding(nn.Module):
   def set_optimizer(self, kind: str = "sgd", lr: float = 0.01, **kwargs):
     """Attach an optimizer that is applied to the model-parallel tables *inside* the backward
     kernels (no sparse gradient is materialised).  ``kind``: ``sgd`` | ``adagrad`` |
-    ``rowwise_adagrad`` | ``adam``.  Only the fused back end consumes it.
+    ``rowwise_adagrad`` | ``adam`` | ``rowwise_adam``.  Only the fused back end consumes it.
+
+    ``rowwise_adam`` is Adam with an element-wise first moment m and one fp32 second-moment word
+    per row: ``v_row = beta2 * v_row + (1 - beta2) * mean_j(g_j^2)``, ``m = beta1 * m +
+    (1 - beta1) * g``, ``w -= lr * (m / (1 - beta1^t)) / (sqrt(v_row / (1 - beta2^t)) + eps)``.
+    It keeps one table-sized state instead of Adam's two.  A column-sliced table keeps one word
+    per row in every slice, the mean over that slice's columns, as row-wise Adagrad does.
 
     Keyword arguments (any other raises ``ValueError``):
 
-    - ``eps``: added to the square root in the denominator (default 1e-7, Adam 1e-8).
+    - ``eps``: added to the square root in the denominator (default 1e-7, Adam and row-wise Adam 1e-8).
     - ``beta1``, ``beta2``: Adam's moment decay rates (0.9, 0.999).
     - ``initial_accumulator_value``: start value of the Adagrad / row-wise Adagrad accumulator
       (0.1).
@@ -608,22 +614,24 @@ class DistributedEmbedding(nn.Module):
       scaled gradient of a row before the optimizer sees it, once per step for every row that at
       least one id of the step touched (a row whose ids carry only zero gradients included).  The
       optimizers are lazy: rows no id touched, and their state, do not move.  Row-wise Adagrad
-      accumulates the mean square of this decayed gradient.
+      accumulates, and row-wise Adam averages into v, the mean square of this decayed gradient.
     - ``deterministic``: SGD only (default False).  False sends SGD without weight decay through
       one atomic scatter of the gradient rows into the tables; True, or any weight decay, takes
       the sorted update, which sums each row's gradient before it applies it.
-    - ``step``: Adam's step count to resume from (0).
-    - ``state_dtype``: storage of the Adagrad accumulator / Adam moments, ``torch.float32``
+    - ``step``: the Adam / row-wise Adam step count to resume from (0).
+    - ``state_dtype``: storage of the Adagrad accumulator / Adam moments / row-wise Adam's m
+      (its v stays one fp32 word per row), ``torch.float32``
       (default) or ``torch.bfloat16`` (half the bytes; the update runs in fp32 and stores the
       state with stochastic rounding, see the user guide, "Half-precision optimizer state")."""
     kind = kind.lower()
-    if kind not in ("sgd", "adagrad", "rowwise_adagrad", "adam"):
+    if kind not in ("sgd", "adagrad", "rowwise_adagrad", "adam", "rowwise_adam"):
       raise ValueError(f"Unsupported fused optimizer {kind}")
     state_dtype = check_state_dtype(kind, kwargs.pop("state_dtype", torch.float32))
     if state_dtype != torch.float32 and self.offload_cache_size is not None:
       raise ValueError("state_dtype=torch.bfloat16 is not supported with offload_cache_size: the "
                        "HBM row cache keeps optimizer state rows as fp32 words")
-    cfg = {"kind": kind, "lr": float(lr), "eps": 1e-7 if kind != "adam" else 1e-8,
+    cfg = {"kind": kind, "lr": float(lr),
+           "eps": 1e-8 if kind in ("adam", "rowwise_adam") else 1e-7,
            "beta1": 0.9, "beta2": 0.999, "weight_decay": 0.0, "initial_accumulator_value": 0.1,
            "deterministic": kind != "sgd", "step": 0, "state_dtype": state_dtype}
     unknown = sorted(set(kwargs) - set(cfg))
@@ -926,9 +934,9 @@ class DistributedEmbedding(nn.Module):
   def get_optimizer_state(self, all_ranks: bool = False) -> Dict[str, Any]:
     """State of the fused optimizer in the same *global, sharding independent* layout as
     :meth:`get_weights`: ``{"kind", "step", "tables": [per table: None | [slot arrays]]}`` with
-    one ``[rows, width]`` array per state slot (Adagrad accumulator; Adam m, v) or ``[rows, 1]``
-    for row-wise Adagrad (column slices of a table contribute the width-weighted mean of their
-    accumulators).  A state written by 8 column-sliced ranks loads on 4, or on one GPU.
+    one ``[rows, width]`` array per element-wise state slot (Adagrad accumulator; Adam m, v;
+    row-wise Adam m) or ``[rows, 1]`` per row-wise slot (row-wise Adagrad's accumulator, row-wise
+    Adam's v; column slices of a table contribute the width-weighted mean of their words).  A state written by 8 column-sliced ranks loads on 4, or on one GPU.
     Replicated tables are trained by the dense optimizer and have no entry (None).  Collective:
     every rank must call it; only rank 0 receives the arrays unless ``all_ranks``."""
     opt = self._fused_optimizer
@@ -940,18 +948,22 @@ class DistributedEmbedding(nn.Module):
     kind = opt["kind"]
     n_col = len(self.local_embedding_layers)
     n_slots = len(next(iter(eng.opt_state.values())))
-    per_row = kind == "rowwise_adagrad"
-    slots = []
-    for k in range(n_slots):
-      col = [eng.opt_state[m][k] for m in range(n_col)]
-      row = [eng.opt_state[n_col + j][k] for j in range(len(self.row_layers))]
-      slots.append(self._gather_global([None] * len(self.dp_layers), col, row, all_ranks,
-                                       per_row=per_row))
+    per_row = _per_row_slots(kind, n_slots)
+    slots = [self._gather_slot(k, per_row[k], all_ranks) for k in range(n_slots)]
     tables = None
     if slots and slots[0]:
       tables = [None if slots[0][t] is None else [sl[t] for sl in slots]
                 for t in range(len(self.strategy.global_configs))]
     return {"kind": kind, "step": eng.step_count(), "tables": tables}
+
+  def _gather_slot(self, k: int, per_row: bool, all_ranks: bool) -> List[Optional[np.ndarray]]:
+    """Global arrays of optimizer-state slot ``k`` (collective, see :meth:`_gather_global`)."""
+    eng = self._engine
+    n_col = len(self.local_embedding_layers)
+    col = [eng.opt_state[m][k] for m in range(n_col)]
+    row = [eng.opt_state[n_col + j][k] for j in range(len(self.row_layers))]
+    return self._gather_global([None] * len(self.dp_layers), col, row, all_ranks,
+                               per_row=per_row)
 
   def set_optimizer_state(self, state: Dict[str, Any], chunk: int = 134217728):
     """Load a state produced by :meth:`get_optimizer_state` (any sharding) - every rank passes
@@ -974,14 +986,14 @@ class DistributedEmbedding(nn.Module):
     tables = state.get("tables")
     if tables is not None:
       st = self.strategy
-      per_row = state["kind"] == "rowwise_adagrad"
       n_col = len(self.local_embedding_layers)
+      per_row = _per_row_slots(state["kind"], len(next(iter(eng.opt_state.values()))))
       with torch.no_grad():
         for s in st.shards[self.rank] if st.table_groups[1] else []:
           t = st.table_groups[1][s.table]
           for k, arr in enumerate(tables[t]):
             dst = eng.opt_state[s.local_table][k]
-            if per_row:
+            if per_row[k]:
               dst[s.row_offset:s.row_offset + s.rows].copy_(
                   torch.from_numpy(np.array(np.asarray(arr)[:, 0], dtype=np.float32)))
             else:
@@ -991,7 +1003,7 @@ class DistributedEmbedding(nn.Module):
           lo, hi = st.row_ranges[gt][self.rank]
           for k, arr in enumerate(tables[t]):
             dst = eng.opt_state[n_col + gt][k]
-            if per_row:
+            if per_row[k]:
               dst.copy_(torch.from_numpy(np.array(np.asarray(arr)[lo:hi, 0], dtype=np.float32)))
             else:
               self._assign_chunked(dst, 0, np.asarray(arr)[lo:hi], chunk)
@@ -1002,10 +1014,11 @@ class DistributedEmbedding(nn.Module):
 
   def save_optimizer_state(self, directory: str, chunk: int = 134217728) -> Optional[str]:
     """File counterpart of :meth:`get_optimizer_state`: ``optimizer.json`` (kind, step, slots)
-    plus one ``opt_<t>_slot<k>.npy`` per table and state slot in the global layout.  Adagrad /
-    Adam state is element-wise, so every rank writes its own slices in parallel like
-    :meth:`save_weights`; row-wise Adagrad needs the width-weighted mean over a table's column
-    slices and goes through the gather of :meth:`get_optimizer_state` (rank 0 writes).
+    plus one ``opt_<t>_slot<k>.npy`` per table and state slot in the global layout.  Every rank
+    writes its own slices of an element-wise slot (Adagrad, Adam, row-wise Adam's m) in parallel
+    like :meth:`save_weights`; a row-wise slot (row-wise Adagrad, row-wise Adam's v) needs the
+    width-weighted mean over a table's column slices and goes through the gather of
+    :meth:`get_optimizer_state` (rank 0 writes).
     Collective; returns the path of ``optimizer.json`` (None when there is no state)."""
     import json  # pylint: disable=import-outside-toplevel
     opt, eng = self._fused_optimizer, self._engine
@@ -1022,21 +1035,23 @@ class DistributedEmbedding(nn.Module):
     def path(t, k):
       return os.path.join(directory, f"opt_{t}_slot{k}.npy")
 
-    if kind == "rowwise_adagrad":
-      state = self.get_optimizer_state()
+    per_row = _per_row_slots(kind, n_slots)
+    rows_k = [k for k in range(n_slots) if per_row[k]]
+    elem_k = [k for k in range(n_slots) if not per_row[k]]
+    for k in rows_k:
+      arrays = self._gather_slot(k, True, False)
       if self.rank == 0:
         os.makedirs(directory, exist_ok=True)
         for t in range(n_tables):
           if has_state[t]:
-            for k, arr in enumerate(state["tables"][t]):
-              np.save(path(t, k), arr)
-    else:
+            np.save(path(t, k), arrays[t])
+    if elem_k:
       if self.rank == 0:
         os.makedirs(directory, exist_ok=True)
         for t in range(n_tables):
           if has_state[t]:
             cfg = st.global_configs[t]
-            for k in range(n_slots):
+            for k in elem_k:
               mm = np.lib.format.open_memmap(
                   path(t, k), mode="w+", dtype=np.float32,
                   shape=(int(cfg["input_dim"]), int(cfg["output_dim"])))
@@ -1045,7 +1060,7 @@ class DistributedEmbedding(nn.Module):
       n_col = len(self.local_embedding_layers)
       for s in st.shards[self.rank] if st.table_groups[1] else []:
         t = st.table_groups[1][s.table]
-        for k in range(n_slots):
+        for k in elem_k:
           mm = np.load(path(t, k), mmap_mode="r+")
           self._write_chunked(mm, 0, s.col_start,
                               eng.opt_state[s.local_table][k][s.row_offset:s.row_offset + s.rows],
@@ -1053,7 +1068,7 @@ class DistributedEmbedding(nn.Module):
           mm.flush()
       for gt, t in enumerate(st.table_groups[2]):
         lo, _ = st.row_ranges[gt][self.rank]
-        for k in range(n_slots):
+        for k in elem_k:
           mm = np.load(path(t, k), mmap_mode="r+")
           self._write_chunked(mm, lo, 0, eng.opt_state[n_col + gt][k], chunk)
           mm.flush()
@@ -1099,6 +1114,12 @@ def _drop_before_load(module, *args, **kwargs):  # pylint: disable=unused-argume
 
 
 # ------------------------------------------------------------------------- hybrid-parallel glue
+def _per_row_slots(kind: str, n_slots: int) -> Tuple[bool, ...]:
+  """Which state slots of optimizer ``kind`` hold one fp32 word per row (row-wise optimizers);
+  the others are element-wise, ``[rows, width]``."""
+  return {"rowwise_adagrad": (True,), "rowwise_adam": (False, True)}.get(kind, (False,) * n_slots)
+
+
 def _is_mp(p) -> bool:
   return bool(getattr(p, "de_local", False))
 

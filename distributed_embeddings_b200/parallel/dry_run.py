@@ -506,9 +506,10 @@ class DryOps:
     self._count("segment_update")
     tdt = self._ADT[int(table_dtype)]
     tsz = 4 if int(table_dtype) == 0 else 2
-    # Adagrad / Adam state in bf16: widened to fp32 for the update, stored with stochastic
-    # rounding (streams 1 and 2); the other optimizers ignore the code, like the kernels
-    half_state = int(state_dtype) == 1 and kind in (1, 3)
+    # Adagrad / Adam state and row-wise Adam's m in bf16: widened to fp32 for the update, stored
+    # with stochastic rounding (streams 1 and 2); the other optimizers ignore the code, like the
+    # kernels
+    half_state = int(state_dtype) == 1 and kind in (1, 3, 5)
     sdt, ssz = (torch.bfloat16, 2) if half_state else (torch.float32, 4)
 
     def state(ptr, row, width, what):
@@ -521,7 +522,7 @@ class DryOps:
     if step_ptr:
       t = float(self.world.tensor(int(step_ptr), torch.float32, 1, "optimizer step")[0])
       step = int(t)
-      if kind == 3:
+      if kind in (3, 5):
         bias1 = float(np.float32(1) - np.float32(beta1)**np.float32(t))
         bias2 = float(np.float32(1) - np.float32(beta2)**np.float32(t))
     D = self._descs(descs, 1 << 30)
@@ -592,6 +593,15 @@ class DryOps:
         if half_state:
           m16.copy_(stochastic_round(mm, sdt, step, key, stream=STREAM_STATE0))
           v16.copy_(stochastic_round(vv, sdt, step, key, stream=STREAM_STATE1))
+      elif kind == 5:
+        # row-wise Adam: v is one fp32 word per row (state1), the mean over the row's columns
+        vr = self.world.tensor(int(t["state1"]) + row * 4, torch.float32, 1, "row state")
+        vr.mul_(beta2).add_(float(np.float32(1) - np.float32(beta2)) * ((g * g).sum() / width))
+        m16, mm = state(t["state0"], row, width, "row-wise adam m")
+        mm.mul_(beta1).add_(float(np.float32(1) - np.float32(beta1)) * g)
+        wt -= lr * (mm / bias1) / ((vr / bias2).sqrt() + eps)
+        if half_state:
+          m16.copy_(stochastic_round(mm, sdt, step, key, stream=STREAM_STATE0))
       else:
         raise ValueError(f"optimizer kind {kind}")
       if tsz == 2:

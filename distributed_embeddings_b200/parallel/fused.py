@@ -49,7 +49,8 @@ from .comm import CH_BARRIER0, CH_CONSUMED, CH_GRAD, CH_IDS, CH_OUT, CommContext
 from .offload_cache import OffloadCache, split_budget
 
 _OPT_KIND = {"sgd": _native.OPT_SGD, "adagrad": _native.OPT_ADAGRAD,
-             "rowwise_adagrad": _native.OPT_ROWWISE_ADAGRAD, "adam": _native.OPT_ADAM}
+             "rowwise_adagrad": _native.OPT_ROWWISE_ADAGRAD, "adam": _native.OPT_ADAM,
+             "rowwise_adam": _native.OPT_ROWWISE_ADAM}
 _COMB = {None: 0, "sum": 0, "mean": 1}
 
 # InputDesc.flags
@@ -871,6 +872,9 @@ class FusedEngine:
         self.opt_state[m] = [like(w, opt["initial_accumulator_value"], (w.shape[0],))]
       elif kind == "adam":
         self.opt_state[m] = [like(w, 0.0, dtype=sdt), like(w, 0.0, dtype=sdt)]
+      elif kind == "rowwise_adam":
+        # m element-wise (in the state dtype), v one fp32 word per row
+        self.opt_state[m] = [like(w, 0.0, dtype=sdt), like(w, 0.0, (w.shape[0],))]
     self._tables_dirty = True
 
   @property
@@ -1268,7 +1272,7 @@ class FusedEngine:
       if not self._dry_updates:
         self.step_t.add_(1.0)  # device counter: bias corrections stay right under graph replay
       kind = _OPT_KIND[opt["kind"]]
-      if self._dry_updates and opt["kind"] == "adam":
+      if self._dry_updates and opt["kind"] in ("adam", "rowwise_adam"):
         kind = _OPT_KIND["sgd"]  # a zero gradient would still decay Adam's moments
       # a dry update has no decay either: weight_decay * w would move the weights and feed the
       # Adagrad accumulators on every warm-up pass

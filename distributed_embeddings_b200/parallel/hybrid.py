@@ -258,28 +258,29 @@ class SparseRowOptimizer:
   tensors - the ``torch`` back end of :class:`DistributedEmbedding`, i.e. the NCCL-collectives
   baseline, which has no fused update.  Same math as the fused kernels
   (``ops/csrc/sparse_update_kernels.cu``): ``sgd`` | ``adagrad`` | ``rowwise_adagrad`` | ``adam``
-  (lazy: only the touched rows advance).  Counterpart of the Keras sparse-apply kernels the
-  reference relies on (examples/benchmarks/synthetic_models/main.py:96-101).
+  | ``rowwise_adam`` (lazy: only the touched rows advance).  Counterpart of the Keras sparse-apply
+  kernels the reference relies on (examples/benchmarks/synthetic_models/main.py:96-101).
 
   bf16 / fp16 parameters keep fp32 state; their touched rows are updated in fp32 and written
   back with stochastic rounding keyed by (step, row, column), the rule of the fused kernels
   (``ops/stochastic_rounding.py``).
 
-  ``state_dtype=torch.bfloat16`` stores the Adagrad accumulator / Adam moments in bf16 like the
-  fused back end: the touched rows' state is widened to fp32, the update runs in fp32 with the
-  unrounded new state, and the state is stored with stochastic rounding (streams 1 and 2)."""
+  ``state_dtype=torch.bfloat16`` stores the Adagrad accumulator / Adam moments / row-wise Adam's
+  m in bf16 like the fused back end: the touched rows' state is widened to fp32, the update runs
+  in fp32 with the unrounded new state, and the state is stored with stochastic rounding
+  (streams 1 and 2).  Row-wise state (one word per row) stays fp32."""
 
   def __init__(self, params: Sequence[nn.Parameter], kind: str = "sgd", lr: float = 0.01,
                eps: Optional[float] = None, beta1: float = 0.9, beta2: float = 0.999,
                initial_accumulator_value: float = 0.1, weight_decay: float = 0.0,
                state_dtype: torch.dtype = torch.float32):
     kind = kind.lower()
-    if kind not in ("sgd", "adagrad", "rowwise_adagrad", "adam"):
+    if kind not in ("sgd", "adagrad", "rowwise_adagrad", "adam", "rowwise_adam"):
       raise ValueError(f"Unsupported optimizer {kind}")
     self.state_dtype = check_state_dtype(kind, state_dtype)
     self.params = [p for p in params if p.requires_grad]
     self.kind, self.lr = kind, float(lr)
-    self.eps = (1e-8 if kind == "adam" else 1e-7) if eps is None else eps
+    self.eps = (1e-8 if kind in ("adam", "rowwise_adam") else 1e-7) if eps is None else eps
     self.beta1, self.beta2, self.weight_decay = beta1, beta2, weight_decay
     self.step_count = 0
     self.state = []
@@ -293,6 +294,9 @@ class SparseRowOptimizer:
                                       device=p.device)])
       elif kind == "adam":
         self.state.append([torch.zeros_like(p, dtype=esdt), torch.zeros_like(p, dtype=esdt)])
+      elif kind == "rowwise_adam":
+        self.state.append([torch.zeros_like(p, dtype=esdt),
+                           torch.zeros((p.shape[0],), dtype=sdt, device=p.device)])
       else:
         self.state.append([])
 
@@ -328,6 +332,13 @@ class SparseRowOptimizer:
         acc = st[0][idx] + (val * val).mean(dim=1)
         st[0][idx] = acc
         p.index_add_(0, idx, val / (acc.sqrt().unsqueeze(1) + self.eps), alpha=-self.lr)
+      elif self.kind == "rowwise_adam":
+        v = self.beta2 * st[1][idx] + (1 - self.beta2) * (val * val).mean(dim=1)
+        m = self.beta1 * st[0][idx] + (1 - self.beta1) * val
+        st[0][idx], st[1][idx] = m, v
+        b1 = 1 - self.beta1**self.step_count
+        b2 = 1 - self.beta2**self.step_count
+        p.index_add_(0, idx, (m / b1) / ((v / b2).sqrt().unsqueeze(1) + self.eps), alpha=-self.lr)
       else:
         m = self.beta1 * st[0][idx] + (1 - self.beta1) * val
         v = self.beta2 * st[1][idx] + (1 - self.beta2) * val * val
@@ -353,6 +364,14 @@ class SparseRowOptimizer:
       acc = st[0][idx] + (val * val).mean(dim=1)
       st[0][idx] = acc
       w = w - self.lr * val / (acc.sqrt().unsqueeze(1) + self.eps)
+    elif self.kind == "rowwise_adam":
+      v = self.beta2 * st[1][idx] + (1 - self.beta2) * (val * val).mean(dim=1)
+      m = self.beta1 * st[0][idx].float() + (1 - self.beta1) * val
+      st[1][idx] = v
+      self._store_state(st[0], idx, m, STREAM_STATE0)
+      b1 = 1 - self.beta1**self.step_count
+      b2 = 1 - self.beta2**self.step_count
+      w = w - self.lr * (m / b1) / ((v / b2).sqrt().unsqueeze(1) + self.eps)
     else:
       m = self.beta1 * st[0][idx].float() + (1 - self.beta1) * val
       v = self.beta2 * st[1][idx].float() + (1 - self.beta2) * val * val

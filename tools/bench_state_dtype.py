@@ -1,22 +1,25 @@
 #!/usr/bin/env python
-"""fp32 versus bf16 optimizer state (Adagrad accumulator, Adam moments) in the single-GPU DLRM
-training step.
+"""fp32 versus bf16 optimizer state (Adagrad accumulator, Adam moments, row-wise Adam's m) in the
+single-GPU DLRM training step.
 
   python tools/bench_state_dtype.py [--steps 30] [--warmup 5] [--repeats 3] [--loss-steps 40]
-                                    [--profile]
+                                    [--profile] [--optimizers adagrad,adam,rowwise_adam]
 
 One invocation, one GPU, the MLPerf tables capped at ``--max-rows`` (default 20M:
 ``dlrm-mlperf-20m`` of ``bench.py``, whose id generator this uses), ``DLRMTrainStep`` (CUDA graph,
 bf16 compute) at global batch 65536.  At 20M rows only the bf16-state and the smaller fp32-state
 configurations fit one 80 GB card; ``--max-rows 5000000`` fits all of them:
 
-1. Adagrad and Adam x {fp32, bf16} tables x {fp32, bf16} state, alternating, ``--repeats`` times
+1. ``--optimizers`` (default Adagrad and Adam; ``rowwise_adam`` adds row-wise Adam, whose bf16
+   state is its m: v stays one fp32 word per row) x {fp32, bf16} tables x {fp32, bf16} state,
+   alternating, ``--repeats`` times
    each: device-timed ms per step (CUDA events around ``--steps`` graph replays; median and spread
    over the repeats), samples/s and ``torch.cuda.max_memory_allocated``.  A configuration whose
    tables and state alone exceed the card's memory is reported with its planned GiB and not run;
    one that runs out of memory while building its step is reported as such;
 2. for every configuration with both state dtypes, the loss after ``--loss-steps`` seeded steps and
-   its difference to the fp32-state run;
+   its difference to the fp32-state run; with Adam and row-wise Adam both run, the loss of each
+   after ``--loss-steps`` seeded steps (the two differ by design);
 3. with ``--profile``: one extra profiled run per configuration (``torch.profiler``, CUDA
    activities), the update kernels' mean µs per step and the bytes/s they achieve on the bytes the
    update must move (per touched element: weight read + write, state read + write, from the
@@ -41,8 +44,9 @@ from bench import gen_ids  # noqa: E402
 from distributed_embeddings_b200.models.dlrm import mlperf_table_sizes  # noqa: E402
 
 _DTYPES = {"fp32": torch.float32, "bf16": torch.bfloat16}
-_SLOTS = {"adagrad": 1, "adam": 2}
-_LR = {"adagrad": 0.01, "adam": 0.0001}
+_SLOTS = {"adagrad": 1, "adam": 2, "rowwise_adam": 1}   # element-wise state slots
+_ROW_SLOTS = {"adagrad": 0, "adam": 0, "rowwise_adam": 1}  # fp32 words per row
+_LR = {"adagrad": 0.01, "adam": 0.0001, "rowwise_adam": 0.0001}
 _UPDATE_KERNELS = ("segment_update", "balanced_update", "finalize_crossing")
 DIM = 128
 
@@ -56,8 +60,8 @@ def gpu_info():
 
 def planned_gib(sizes, kind, table_dtype, state_dtype):
   elems = sum(sizes) * DIM
-  return elems * (_DTYPES[table_dtype].itemsize + _SLOTS[kind] * _DTYPES[state_dtype].itemsize) \
-      / 2**30
+  return (elems * (_DTYPES[table_dtype].itemsize + _SLOTS[kind] * _DTYPES[state_dtype].itemsize) +
+          sum(sizes) * 4 * _ROW_SLOTS[kind]) / 2**30
 
 
 def make_pool(sizes, b):
@@ -73,10 +77,11 @@ def make_pool(sizes, b):
 
 def update_bytes(pool, kind, table_dtype, state_dtype):
   """Bytes the fused update moves per step, averaged over the pool: every touched element's
-  weight and state are read and written once."""
+  weight and state are read and written once (row-wise state: one fp32 word per touched row)."""
   per_elem = 2 * (_DTYPES[table_dtype].itemsize + _SLOTS[kind] * _DTYPES[state_dtype].itemsize)
+  per_row = DIM * per_elem + 2 * 4 * _ROW_SLOTS[kind]
   rows = [sum(int(torch.unique(c).numel()) for c in cat) for _, cat, _ in pool]
-  return sum(rows) / len(rows) * DIM * per_elem
+  return sum(rows) / len(rows) * per_row
 
 
 def run(cfg, args, pool, steps, mode="time"):
@@ -147,7 +152,12 @@ def main():
   ap.add_argument("--global-batch", type=int, default=65536)
   ap.add_argument("--max-rows", type=int, default=20_000_000)
   ap.add_argument("--profile", action="store_true")
+  ap.add_argument("--optimizers", default="adagrad,adam",
+                  help="comma-separated subset of adagrad, adam, rowwise_adam")
   args = ap.parse_args()
+  kinds = [k for k in args.optimizers.split(",") if k]
+  if not kinds or any(k not in _SLOTS for k in kinds):
+    ap.error(f"--optimizers: a comma-separated subset of {', '.join(_SLOTS)}")
   if not torch.cuda.is_available():
     raise SystemExit("bench_state_dtype.py needs a CUDA GPU")
   torch.cuda.set_device(0)
@@ -156,7 +166,7 @@ def main():
   out = {"gpu": gpu_info(), "max_rows": args.max_rows, "rows": sum(sizes),
          "global_batch": args.global_batch, "steps": args.steps, "card_gib": round(card_gib, 1)}
   pool = make_pool(sizes, args.global_batch)
-  cfgs = [(k, t, s) for k in ("adagrad", "adam") for t in ("fp32", "bf16") for s in ("fp32", "bf16")]
+  cfgs = [(k, t, s) for k in kinds for t in ("fp32", "bf16") for s in ("fp32", "bf16")]
   planned = {c: planned_gib(sizes, *c) for c in cfgs}
   # tables and state alone must leave room for the step's buffers (a few GiB at batch 65536)
   runnable = [c for c in cfgs if planned[c] < card_gib - 6.0]
@@ -186,7 +196,7 @@ def main():
   out["runs"] = results
   ok = {(e["optimizer"], e["table_dtype"], e["state_dtype"]) for e in results if "not_run" not in e}
   losses = []
-  for k in ("adagrad", "adam"):
+  for k in kinds:
     for t in ("fp32", "bf16"):
       if (k, t, "fp32") in ok and (k, t, "bf16") in ok:
         l32 = run((k, t, "fp32"), args, pool, args.loss_steps, mode="loss")["loss"]
@@ -194,6 +204,16 @@ def main():
         losses.append({"optimizer": k, "table_dtype": t, "fp32_state": l32, "bf16_state": l16,
                        "relative_difference": abs(l16 - l32) / abs(l32)})
   out["loss_after_steps"] = {"steps": args.loss_steps, "pairs": losses}
+  versus = []
+  for t in ("fp32", "bf16"):
+    for sd in ("fp32", "bf16"):
+      if ("adam", t, sd) in ok and ("rowwise_adam", t, sd) in ok:
+        la = run(("adam", t, sd), args, pool, args.loss_steps, mode="loss")["loss"]
+        lr_ = run(("rowwise_adam", t, sd), args, pool, args.loss_steps, mode="loss")["loss"]
+        versus.append({"table_dtype": t, "state_dtype": sd, "adam": la, "rowwise_adam": lr_,
+                       "difference": lr_ - la})
+  if versus:
+    out["rowwise_adam_vs_adam_loss"] = {"steps": args.loss_steps, "pairs": versus}
   print(json.dumps(out))
 
 

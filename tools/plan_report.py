@@ -61,9 +61,14 @@ def main(argv=None):
   ap.add_argument("--hbm-gib", type=float, default=79.0, help="per-GPU memory to check against")
   ap.add_argument("--optimizer-slots", type=int, default=0,
                   help="state copies per table element (adagrad 1, adam 2)")
+  ap.add_argument("--optimizer-row-slots", type=int, default=0,
+                  help="fp32 state words per table row of the model-parallel tables (row-wise "
+                       "adagrad 1 with --optimizer-slots 0, row-wise adam 1 with --optimizer-slots "
+                       "1)")
   ap.add_argument("--state-dtype", default="fp32", choices=["fp32", "bf16"],
-                  help="storage of the Adagrad / Adam state of the model-parallel tables "
-                       "(set_optimizer(state_dtype=...)); replicated tables stay fp32")
+                  help="storage of the element-wise Adagrad / Adam / row-wise Adam state of the "
+                       "model-parallel tables (set_optimizer(state_dtype=...)); row words and "
+                       "replicated tables stay fp32")
   ap.add_argument("--table-dtype", default="fp32", choices=["fp32", "bf16", "fp16"],
                   help="storage of the model-parallel tables (DistributedEmbedding(table_dtype="
                        "...)): their table and gather bytes at its element size; optimizer slots "
@@ -121,19 +126,38 @@ def main(argv=None):
     shapes = [(int(st.local_configs[r][m]["input_dim"]), int(st.local_configs[r][m]["output_dim"]))
               for m in ms]
     sets = split_budget(args.offload_cache_size, shapes)
-    return sum(cache_bytes(n, spill[m], w, [w] * args.optimizer_slots)
+    return sum(cache_bytes(n, spill[m], w, [w] * args.optimizer_slots +
+                           [1] * args.optimizer_row_slots)
                for n, m, (_, w) in zip(sets, ms, shapes)) / 2**30
+
+  def row_gib(r):
+    """(HBM, host) GiB of rank r's fp32 row words: one per slot and local row of a
+    model-parallel table (table-parallel, column slices, row slices)."""
+    hbm = host = 0
+    if st.table_groups[1]:
+      for c in st.local_configs[r]:
+        if c.get("cpu_offload"):
+          host += int(c["input_dim"])
+        else:
+          hbm += int(c["input_dim"])
+    for gt in range(len(st.table_groups[2])):
+      lo, hi = st.row_ranges[gt][r]
+      hbm += hi - lo
+    words = 4 * args.optimizer_row_slots
+    return hbm * words / 2**30, host * words / 2**30
 
   for r in range(args.world):
     n_tab = len(st.local_configs[r]) if st.table_groups[1] else 0
     cols = sum(int(st.local_configs[r][m]["output_dim"]) for m in st.local_maps[r]) \
         if st.table_groups[1] else 0
     cgib = cache_gib(r)
-    gib = ((mem[r]["hbm_elements"] - dp_elems) * per_elem + dp_elems * per_elem_dp) / 2**30 + cgib
+    rgib, rhost = row_gib(r)
+    gib = ((mem[r]["hbm_elements"] - dp_elems) * per_elem + dp_elems * per_elem_dp) / 2**30 + \
+        cgib + rgib
     gather = (tr["ranks"][r]["gather_bytes"] - dp_gather) * esz / 4 + dp_gather
     ranks.append({"rank": r, "fused_tables": n_tab, "inputs": len(st.input_ids_list[r]),
                   "exchanged_columns": cols, "hbm_gib": round(gib, 2),
-                  "host_gib": round(mem[r]["host_elements"] * per_elem / 2**30, 2),
+                  "host_gib": round(mem[r]["host_elements"] * per_elem / 2**30 + rhost, 2),
                   "cache_gib": round(cgib, 6),
                   "gather_mb": round(gather / 1e6, 1),
                   "nvlink_out_mb": round(tr["ranks"][r]["nvlink_out_bytes"] / 1e6, 1),
@@ -145,6 +169,8 @@ def main(argv=None):
          "table_parallel": len(st.table_groups[1]), "row_sliced": len(st.table_groups[2]),
          "gather_imbalance": round(tr["gather_imbalance"], 3),
          "nvlink_imbalance": round(tr["nvlink_imbalance"], 3), "ranks": ranks}
+  if args.optimizer_row_slots:
+    rep["optimizer_row_slots"] = args.optimizer_row_slots
   if args.json:
     print(json.dumps(rep))
     return rep
