@@ -7,9 +7,10 @@ math as one static schedule over preallocated buffers:
 * dense parameters live in one flat fp32 master buffer with a bf16 shadow (one fused kernel does
   SGD + re-cast + gradient zeroing); gradients live in one flat buffer (symmetric memory when
   world > 1) that the one-shot NVLink all-reduce kernel reduces in place;
-* MLP layers: cuBLASLt bf16 GEMMs with fused bias+ReLU epilogues forward, plain GEMMs backward
-  (K padded 13->16 and 479->480 so every layer meets the TMA alignment rules of the GEMM kernels), fused
-  ReLU-backward+bias-gradient kernel;
+* MLP layers: cuBLASLt bf16 GEMMs forward (fused bias+ReLU epilogues) and for the weight
+  gradients (K padded 13->16 and 479->480 so every layer meets the TMA alignment rules of the GEMM
+  kernels); the data gradient of a layer above a ReLU is one first-party wgmma GEMM that applies the
+  ReLU backward and sums the bias gradient of the layer below in its epilogue;
 * dot interaction forward/backward: tensor-core kernels; the forward's head waits for the
   embedding owners' "output ready" signals, the backward pushes every piece of the embedding
   gradient straight into its owner's receive buffer over NVLink and signals "gradient ready";
@@ -52,6 +53,22 @@ FUSED_UPDATE_MIN_ROWS = 20000
 
 def _pad8(n: int) -> int:
   return (n + 7) // 8 * 8
+
+
+def _fused_dgrad(L) -> bool:
+  """Whether the data gradient of layer ``L`` (its input a ReLU output) runs as one
+  ``gemm_dgrad_relu_bias`` kernel instead of ``torch.mm`` + ``relu_bwd_bias``.  The kernel needs
+  N = in_f <= 2048 columns, and 8-element rows (TMA strides of 16 bytes) for dy and W^T.
+  tools/bench_dgrad.py times both on the DLRM shapes (DESIGN §8): the fused kernel is faster on
+  every one of them."""
+  return L.in_f == L.in_pad and L.in_f <= 2048 and L.out_f % 8 == 0
+
+
+def _dgrad_block_n(L) -> int:
+  """Tile width of the fused dgrad GEMM: 128 for K = out_f <= 256, where the shorter main loop
+  leaves the epilogue the larger share and the 128-wide tile's deeper pipeline (5 stages instead
+  of 3) wins (tools/bench_dgrad.py, DESIGN §8); else the kernel's choice."""
+  return 128 if L.out_f <= 256 else 0
 
 
 class _Layer:
@@ -102,10 +119,11 @@ class DLRMTrainStep:
                fused_update_min_rows: int = FUSED_UPDATE_MIN_ROWS):
     if gemm not in ("cublas", "fused_dgrad", "tcgen05", "tcgen05_pair"):
       raise ValueError("gemm must be cublas | fused_dgrad | tcgen05 | tcgen05_pair")
-    # cublas: cuBLASLt everywhere.  fused_dgrad: forward/wgrad on cuBLASLt, dgrad on the
-    # first-party wgmma kernel with the ReLU-backward mask + bias gradient fused in its epilogue.
-    # tcgen05: forward layers on the first-party kernel as well.  tcgen05_pair: same, with the
-    # 2-CTA cluster kernel for layers at least 256 wide.  (The option names are historical.)
+    # Every value runs the data gradients below a ReLU on the first-party wgmma kernel with the
+    # ReLU-backward mask + bias gradient fused in its epilogue (see _dgrad_relu).  cublas:
+    # cuBLASLt for the forward and weight-gradient GEMMs; fused_dgrad is the same schedule, kept
+    # as a name.  tcgen05: forward layers on the first-party kernel as well.  tcgen05_pair: same,
+    # with the 2-CTA cluster kernel for layers at least 256 wide.  (The names are historical.)
     self.gemm = gemm
     self.dcn = getattr(model, "interaction", "dot") == "dcnv2"
     hots = getattr(model, "multi_hot_sizes", None)
@@ -268,11 +286,10 @@ class DLRMTrainStep:
     self._eval_graph = None
 
   def _refresh_transposes(self):
-    """K-major copies of W^T for the dgrad GEMMs (2.4 M elements, a few microseconds)."""
-    if self.gemm == "cublas":
-      return
+    """K-major copies of W^T for the fused dgrad GEMMs (1.9 M elements, a few microseconds)."""
     for L in self.bottom[1:] + self.top[1:]:
-      L.w16T.copy_(L.w16.t())
+      if _fused_dgrad(L):
+        L.w16T.copy_(L.w16.t())
 
   def _linear_fwd(self, L, x):
     if self.gemm in ("tcgen05", "tcgen05_pair"):
@@ -297,11 +314,11 @@ class DLRMTrainStep:
 
   def _dgrad_relu(self, L, x_below, dx, gb_below):
     """dx = (dy @ W) * (x_below > 0); gb_below += colsum(dx)."""
-    if self.gemm == "cublas":
+    if _fused_dgrad(L):
+      self.ops.gemm_dgrad_relu_bias(L.dy, L.w16T, x_below, dx, gb_below, _dgrad_block_n(L))
+    else:
       torch.mm(L.dy, L.w16, out=dx)
       self.ops.relu_bwd_bias(dx, x_below, gb_below)
-    else:
-      self.ops.gemm_dgrad_relu_bias(L.dy, L.w16T, x_below, dx, gb_below, 0)
 
   # ------------------------------------------------------------------ buffers
   def _alloc(self, b: int):

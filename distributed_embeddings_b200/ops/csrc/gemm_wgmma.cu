@@ -7,8 +7,10 @@
 // * two consumer warpgroups each own 64 rows of the 128-row tile and issue asynchronous
 //   wgmma.mma_async m64n128k16 (bf16 in, fp32 accumulate in registers) straight from shared-memory
 //   matrix descriptors; one wgmma group stays in flight while the previous stage is released;
-// * the epilogue adds the bias / applies ReLU (or the ReLU-backward mask and column sums) on the
-//   register accumulators and stores bf16 pairs.
+// * the epilogue adds the bias / applies ReLU on the register accumulators and stores bf16 pairs;
+//   the dgrad epilogue (EPI 2) masks them against the ReLU output, which was copied to shared
+//   memory while the main loop ran, sums the columns, and stores the tile from shared memory in
+//   16-byte chunks.
 // Warpgroup roles: warpgroup 0 = TMA producer (one thread), warpgroups 1..2 = MMA + epilogue.
 //
 // Replaces the cuBLAS GEMM + separate bias/activation ops that TF/XLA runs for the reference's
@@ -18,6 +20,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <atomic>
 #include <mutex>
 
 #include "de_b200.h"
@@ -107,8 +110,41 @@ __device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUte
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
-__device__ __forceinline__ void consumer_bar_sync() {  // the 256 threads of warpgroups 1..2
-  asm volatile("bar.sync 1, 256;" ::: "memory");
+// 16-byte asynchronous global -> shared copy (L2 only); src_bytes = 0 fills zeros, reads nothing
+__device__ __forceinline__ void cp_async_16(void* smem_dst, const void* src, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_addr(smem_dst)),
+               "l"(src), "r"(src_bytes)
+               : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() {
+  asm volatile("cp.async.commit_group;" ::: "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() {
+  asm volatile("cp.async.wait_group 0;" ::: "memory");
+}
+// shared-memory accesses by address: the 1024-byte realignment of the dynamic window hides the
+// address space from the compiler, which would otherwise emit generic loads and stores
+__device__ __forceinline__ uint32_t lds_b32(uint32_t a) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
+  return v;
+}
+__device__ __forceinline__ void sts_b32(uint32_t a, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint4 lds_b128(uint32_t a) {
+  uint4 v;
+  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
+               : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
+               : "r"(a)
+               : "memory");
+  return v;
+}
+__device__ __forceinline__ void red_add_f32(float* gmem, float v) {
+  asm volatile("red.global.add.f32 [%0], %1;" ::"l"(gmem), "f"(v) : "memory");
+}
+__device__ __forceinline__ void warpgroup_bar_sync(int cw) {  // the 128 threads of warpgroup 1 + cw
+  asm volatile("bar.sync %0, 128;" ::"r"(2 + cw) : "memory");
 }
 
 __device__ __forceinline__ void wgmma_fence() {
@@ -159,16 +195,35 @@ __device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_byte_ad
   return d;
 }
 
-template <int BLOCK_N, int STAGES>
+template <int BLOCK_N, int STAGES, int EPI = 0>
 struct SmemLayout {
   static constexpr int kABytes = BLOCK_M * BLOCK_K * 2;
   static constexpr int kBBytes = BLOCK_N * BLOCK_K * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kColsumOffset = STAGES * kStageBytes;
+  // EPI 2: each consumer warpgroup's 64 x BLOCK_N tile of the ReLU output, which the epilogue
+  // overwrites with the masked result before it is stored.  Rows are padded by 16 bytes, so the
+  // 8 rows x 4 words a warp touches per accumulator fragment fall into 32 different banks.
+  static constexpr int kActRowBytes = BLOCK_N * 2 + 16;
+  static constexpr int kActWgBytes = 64 * kActRowBytes;
+  static constexpr int kActOffset = STAGES * kStageBytes;
+  // EPI 2: per-warp column sums of the current tile, [consumer warp 0..7][BLOCK_N] fp32
+  static constexpr int kColsumOffset = kActOffset + (EPI == 2 ? 2 * kActWgBytes : 0);
   static constexpr int kBarOffset = kColsumOffset + kMaxColsum * 4;
+  static_assert(8 * BLOCK_N <= kMaxColsum, "per-warp column sums exceed their region");
   static constexpr int kNumBars = 2 * STAGES;  // full / empty per stage
-  static constexpr int kTotal = kBarOffset + kNumBars * 8;
+  // tile index of the k block in each stage (-1: no more tiles), written by the producer
+  static constexpr int kTileOffset = kBarOffset + kNumBars * 8;
+  static constexpr int kTotal = kTileOffset + STAGES * 4;
 };
+
+// Dynamic tile scheduling of gemm_tn_fused_kernel: after its first tile (blockIdx.x), a CTA takes
+// the next one from a device counter, so a CTA that becomes resident late (the GEMM shares the
+// GPU with other streams' kernels) takes fewer tiles instead of setting the kernel's end.  Word 0
+// counts handed-out tiles, word 1 the CTAs that found none left; the last of those resets both,
+// so every launch (graph replays included) starts from zero.  Launches cycle through the slots,
+// so kernels on different streams that run at the same time use different counters.
+constexpr int kSchedSlots = 256;
+__device__ unsigned int g_tile_sched[kSchedSlots][2];
 
 // Main loop + epilogue of one consumer warpgroup (cw = 0/1: rows [cw*64, cw*64+64) of the tile).
 // CLUSTER: the empty barriers of both CTAs of a 2-CTA cluster are released (their producers
@@ -182,11 +237,33 @@ __device__ __forceinline__ void consumer_tile(uint8_t* smem, uint64_t* full_bar,
                                               int num_kb, int cw, const bf16* __restrict__ bias,
                                               bf16* __restrict__ C, int64_t ldc, int M, int N,
                                               const bf16* __restrict__ act, int64_t ldact,
-                                              float* s_colsum, float (&acc)[BLOCK_N / WGMMA_N][64]) {
-  using L = SmemLayout<BLOCK_N, STAGES>;
+                                              float* colsum, float (&acc)[BLOCK_N / WGMMA_N][64]) {
+  using L = SmemLayout<BLOCK_N, STAGES, EPI>;
   constexpr int NB = BLOCK_N / WGMMA_N;
   const int lane = threadIdx.x & 31, warp_in_wg = (threadIdx.x >> 5) & 3;
   const bool releaser = warp_in_wg == 0 && lane == 0;
+  // wgmma D fragment: register 4j + 2i + c holds row 16*warp + lane/4 + 8i, column
+  // 8j + 2*(lane%4) + c of the warpgroup's 64 x 128 block
+  const int row0 = m0 + cw * 64 + warp_in_wg * 16 + (lane >> 2);
+  // EPI 2: the warpgroup's 64 rows of the ReLU output are copied to shared memory (16-byte
+  // chunks, coalesced) while the main loop runs, so the epilogue does not wait on global memory
+  uint8_t* s_act = smem + L::kActOffset + cw * L::kActWgBytes;
+  const uint32_t s_act_a = smem_addr(s_act);
+  const uint32_t s_part_a = smem_addr(smem + L::kColsumOffset) + cw * 4 * BLOCK_N * 4;
+  constexpr int kRowChunks = BLOCK_N / 8;  // 16-byte chunks per row; N % 8 == 0: all in or out
+  const int wt = threadIdx.x & 127;
+  if constexpr (EPI == 2) {
+    warpgroup_bar_sync(cw);  // the previous tile's stores have read the buffer
+#pragma unroll 4
+    for (int c = wt; c < 64 * kRowChunks; c += 128) {
+      const int r = c / kRowChunks, cc = c % kRowChunks;
+      const int row = m0 + cw * 64 + r, col = n0 + cc * 8;
+      const bool ok = row < M && col < N;  // out of range: zeros, i.e. masked
+      cp_async_16(s_act + r * L::kActRowBytes + cc * 16,
+                  act + (ok ? static_cast<int64_t>(row) * ldact + col : 0), ok ? 16u : 0u);
+    }
+    cp_async_commit();
+  }
   int prev_stage = -1;
   for (int kb = 0; kb < num_kb; ++kb) {
     mbar_wait(&full_bar[stage], phase);
@@ -238,9 +315,11 @@ __device__ __forceinline__ void consumer_tile(uint8_t* smem, uint64_t* full_bar,
     }
   }
 
-  // ---- epilogue on the register accumulators. wgmma D fragment: register 4j + 2i + c holds
-  // row 16*warp + lane/4 + 8i, column 8j + 2*(lane%4) + c of the warpgroup's 64 x 128 block.
-  const int row0 = m0 + cw * 64 + warp_in_wg * 16 + (lane >> 2);
+  // ---- epilogue on the register accumulators
+  if constexpr (EPI == 2) {
+    cp_async_wait_all();
+    warpgroup_bar_sync(cw);
+  }
 #pragma unroll
   for (int nb = 0; nb < NB; ++nb) {
 #pragma unroll
@@ -258,15 +337,16 @@ __device__ __forceinline__ void consumer_tile(uint8_t* smem, uint64_t* full_bar,
       for (int i = 0; i < 2; ++i) {
         const int row = row0 + 8 * i;
         float v0 = acc[nb][4 * j + 2 * i], v1 = acc[nb][4 * j + 2 * i + 1];
-        if (EPI == 2) {
-          float2 af = make_float2(0.f, 0.f);
-          if (row < M && col_ok)
-            af = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(
-                act + static_cast<int64_t>(row) * ldact + col));
-          v0 = af.x > 0.f ? v0 : 0.f;
-          v1 = af.y > 0.f ? v1 : 0.f;
+        if constexpr (EPI == 2) {
+          // the act pair under (v0, v1) is replaced by the masked result, stored below
+          const uint32_t sp = s_act_a + (row - m0 - cw * 64) * L::kActRowBytes + (col - n0) * 2;
+          const uint32_t a = lds_b32(sp);  // bf16 pair, column col in the low half
+          v0 = __uint_as_float(a << 16) > 0.f ? v0 : 0.f;
+          v1 = __uint_as_float(a & 0xffff0000u) > 0.f ? v1 : 0.f;
           cs0 += v0;
           cs1 += v1;
+          const __nv_bfloat162 r = __floats2bfloat162_rn(v0, v1);
+          sts_b32(sp, *reinterpret_cast<const uint32_t*>(&r));
         } else {
           v0 += b0;
           v1 += b1;
@@ -274,10 +354,10 @@ __device__ __forceinline__ void consumer_tile(uint8_t* smem, uint64_t* full_bar,
             v0 = fmaxf(v0, 0.f);
             v1 = fmaxf(v1, 0.f);
           }
+          if (row < M && col_ok)
+            *reinterpret_cast<__nv_bfloat162*>(C + static_cast<int64_t>(row) * ldc + col) =
+                __floats2bfloat162_rn(v0, v1);
         }
-        if (row < M && col_ok)
-          *reinterpret_cast<__nv_bfloat162*>(C + static_cast<int64_t>(row) * ldc + col) =
-              __floats2bfloat162_rn(v0, v1);
       }
       if (EPI == 2) {
         // lanes with the same lane % 4 hold the same two columns: sum the warp's 16 rows
@@ -286,32 +366,54 @@ __device__ __forceinline__ void consumer_tile(uint8_t* smem, uint64_t* full_bar,
           cs0 += __shfl_xor_sync(0xffffffffu, cs0, sft);
           cs1 += __shfl_xor_sync(0xffffffffu, cs1, sft);
         }
-        if (lane < 4 && col_ok) {
-          atomicAdd(&s_colsum[col], cs0);
-          atomicAdd(&s_colsum[col + 1], cs1);
+        if (lane < 4) {  // this warp's slot: plain stores, summed over the warps below
+          const uint32_t sp = s_part_a + (warp_in_wg * BLOCK_N + col - n0) * 4;
+          sts_b32(sp, __float_as_uint(cs0));
+          sts_b32(sp + 4, __float_as_uint(cs1));
         }
       }
+    }
+  }
+  if constexpr (EPI == 2) {  // the masked tile, in 16-byte coalesced stores
+    warpgroup_bar_sync(cw);
+    // column sums of the warpgroup's 64 rows: one fp32 reduction per column into colsum
+    for (int c = wt; c < BLOCK_N; c += 128) {
+      const uint32_t sp = s_part_a + c * 4;
+      const float v = __uint_as_float(lds_b32(sp)) + __uint_as_float(lds_b32(sp + BLOCK_N * 4)) +
+                      __uint_as_float(lds_b32(sp + 2 * BLOCK_N * 4)) +
+                      __uint_as_float(lds_b32(sp + 3 * BLOCK_N * 4));
+      if (n0 + c < N && v != 0.f) red_add_f32(colsum + n0 + c, v);
+    }
+#pragma unroll 4
+    for (int c = wt; c < 64 * kRowChunks; c += 128) {
+      const int r = c / kRowChunks, cc = c % kRowChunks;
+      const int row = m0 + cw * 64 + r, col = n0 + cc * 8;
+      if (row < M && col < N)
+        *reinterpret_cast<uint4*>(C + static_cast<int64_t>(row) * ldc + col) =
+            lds_b128(s_act_a + r * L::kActRowBytes + cc * 16);
     }
   }
 }
 
 // Persistent kernel: one CTA per SM walks the output tiles (n fastest so that concurrently
-// running CTAs share A rows in L2).  The producer runs up to STAGES k blocks ahead, across tile
-// boundaries, so the next tile's operands stream in while the epilogue of this one runs.
+// running CTAs share A rows in L2), taking each next tile from g_tile_sched.  The producer runs up
+// to STAGES k blocks ahead, across tile boundaries, so the next tile's operands stream in while
+// the epilogue of this one runs; it passes each tile's index to the consumers in s_tile.
 template <int BLOCK_N, int STAGES, int EPI>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tn_fused_kernel(const __grid_constant__ CUtensorMap tma_a,
                      const __grid_constant__ CUtensorMap tma_b, const bf16* __restrict__ bias,
                      bf16* __restrict__ C, int64_t ldc, int M, int N, int K,
-                     const bf16* __restrict__ act, int64_t ldact, float* __restrict__ colsum) {
-  using L = SmemLayout<BLOCK_N, STAGES>;
+                     const bf16* __restrict__ act, int64_t ldact, float* __restrict__ colsum,
+                     int sched_slot) {
+  using L = SmemLayout<BLOCK_N, STAGES, EPI>;
   extern __shared__ uint8_t smem_raw[];
   // the swizzled tiles need 1024-byte alignment
   uint8_t* smem = reinterpret_cast<uint8_t*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  float* s_colsum = reinterpret_cast<float*>(smem + L::kColsumOffset);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::kBarOffset);
   uint64_t* empty_bar = full_bar + STAGES;
+  volatile int* s_tile = reinterpret_cast<int*>(smem + L::kTileOffset);
 
   const int wg = threadIdx.x >> 7;
   const int num_kb = (K + BLOCK_K - 1) / BLOCK_K;
@@ -334,12 +436,21 @@ gemm_tn_fused_kernel(const __grid_constant__ CUtensorMap tma_a,
   if (wg == 0) {
     // ===================== TMA producer =====================
     if (threadIdx.x == 0) {
+      unsigned int* sched = g_tile_sched[sched_slot];
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      for (int tile = blockIdx.x;;) {
+        // ask for the next tile now; the answer arrives while this one's loads are issued
+        const int next = static_cast<int>(gridDim.x + atomicAdd(&sched[0], 1u));
+        const bool done = tile >= num_tiles;
         const int m0 = (tile / tiles_n) * BLOCK_M, n0 = (tile % tiles_n) * BLOCK_N;
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
+          if (kb == 0) s_tile[stage] = done ? -1 : tile;
+          if (done) {  // the consumers read -1 and stop
+            mbar_arrive(&full_bar[stage]);
+            break;
+          }
           uint8_t* sa = smem + stage * L::kStageBytes;
           uint8_t* sb = sa + L::kABytes;
           mbar_expect_tx(&full_bar[stage], L::kStageBytes);
@@ -350,15 +461,20 @@ gemm_tn_fused_kernel(const __grid_constant__ CUtensorMap tma_a,
             phase ^= 1;
           }
         }
+        if (done) break;
+        tile = next;
+      }
+      // this CTA took its last counter value: the last CTA to get here resets the counter
+      __threadfence();
+      if (atomicAdd(&sched[1], 1u) == gridDim.x - 1) {
+        __threadfence();
+        atomicExch(&sched[0], 0u);
+        atomicExch(&sched[1], 0u);
       }
     }
   } else {
     // ===================== MMA + epilogue (warpgroups 1..2) =====================
     const int cw = wg - 1;
-    if (EPI == 2) {
-      for (int i = threadIdx.x - 128; i < kMaxColsum; i += 256) s_colsum[i] = 0.f;
-      consumer_bar_sync();
-    }
     float acc[BLOCK_N / WGMMA_N][64];
 #pragma unroll
     for (int nb = 0; nb < BLOCK_N / WGMMA_N; ++nb)
@@ -366,18 +482,14 @@ gemm_tn_fused_kernel(const __grid_constant__ CUtensorMap tma_a,
       for (int r = 0; r < 64; ++r) acc[nb][r] = 0.f;
     int stage = 0;
     uint32_t phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    for (;;) {
+      mbar_wait(&full_bar[stage], phase);  // first k block of the next tile, or the end
+      const int tile = s_tile[stage];
+      if (tile < 0) break;
       const int m0 = (tile / tiles_n) * BLOCK_M, n0 = (tile % tiles_n) * BLOCK_N;
       consumer_tile<BLOCK_N, STAGES, EPI, false>(smem, full_bar, empty_bar, stage, phase, m0, n0,
                                                  num_kb, cw, bias, C, ldc, M, N, act, ldact,
-                                                 s_colsum, acc);
-    }
-    if (EPI == 2) {
-      consumer_bar_sync();
-      for (int i = threadIdx.x - 128; i < N && i < kMaxColsum; i += 256) {
-        const float vsum = s_colsum[i];
-        if (vsum != 0.f) atomicAdd(colsum + i, vsum);
-      }
+                                                 colsum, acc);
     }
   }
 }
@@ -514,11 +626,16 @@ bool make_tensor_map(CUtensorMap* map, const void* ptr, int64_t rows, int64_t co
   return r == CUDA_SUCCESS;
 }
 
+int next_sched_slot() {
+  static std::atomic<unsigned int> seq{0};
+  return static_cast<int>(seq.fetch_add(1, std::memory_order_relaxed) % kSchedSlots);
+}
+
 template <int BLOCK_N, int STAGES, int EPI>
 bool launch_one(const CUtensorMap& ta, const CUtensorMap& tb, const void* bias, void* C,
                 int64_t ldc, int M, int N, int K, const void* act, int64_t ldact, float* colsum,
                 int sm_count, cudaStream_t stream) {
-  using L = SmemLayout<BLOCK_N, STAGES>;
+  using L = SmemLayout<BLOCK_N, STAGES, EPI>;
   const size_t smem = L::kTotal + 1024;
   static_assert(L::kTotal + 1024 <= 227 * 1024, "exceeds the 227 KB of shared memory per block");
   const int tiles = ((N + BLOCK_N - 1) / BLOCK_N) * ((M + BLOCK_M - 1) / BLOCK_M);
@@ -527,10 +644,12 @@ bool launch_one(const CUtensorMap& ta, const CUtensorMap& tb, const void* bias, 
                        cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
   gemm_tn_fused_kernel<BLOCK_N, STAGES, EPI><<<grid, kGemmThreads, smem, stream>>>(
       ta, tb, reinterpret_cast<const bf16*>(bias), reinterpret_cast<bf16*>(C), ldc, M, N, K,
-      reinterpret_cast<const bf16*>(act), ldact, colsum);
+      reinterpret_cast<const bf16*>(act), ldact, colsum, next_sched_slot());
   return cudaGetLastError() == cudaSuccess;
 }
 
+// EPI 2 gives one pipeline stage to the shared-memory copy of the ReLU output (BLOCK_N = 256:
+// 64 KB, 128: 32 KB)
 template <int BLOCK_N, int STAGES>
 bool launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const void* bias, void* C,
                 int64_t ldc, int M, int N, int K, int epi, const void* act, int64_t ldact,
@@ -541,8 +660,8 @@ bool launch_cfg(const CUtensorMap& ta, const CUtensorMap& tb, const void* bias, 
   if (epi == 1)
     return launch_one<BLOCK_N, STAGES, 1>(ta, tb, bias, C, ldc, M, N, K, act, ldact, colsum,
                                           sm_count, stream);
-  return launch_one<BLOCK_N, STAGES, 2>(ta, tb, bias, C, ldc, M, N, K, act, ldact, colsum,
-                                        sm_count, stream);
+  return launch_one<BLOCK_N, STAGES - 1, 2>(ta, tb, bias, C, ldc, M, N, K, act, ldact, colsum,
+                                            sm_count, stream);
 }
 
 }  // namespace
