@@ -90,7 +90,8 @@ class DLRMTrainStep:
   ``dense_optimizer`` (``sgd`` | ``adagrad`` | ``adam``, hyperparameters in
   ``dense_optimizer_kwargs``) updates the MLPs and any replicated tables with the shared
   learning rate.  Replicated tables (``data_parallel_threshold``) need
-  ``dense_optimizer == embedding_optimizer``.
+  ``dense_optimizer == embedding_optimizer``, so the row-wise optimizers and ``ftrl`` need a model
+  without replicated tables.
 
   ``fused_table_update``: on one GPU with the atomic SGD embedding update, the interaction
   backward applies the update of the tables with at least ``fused_update_min_rows`` rows
@@ -198,6 +199,12 @@ class DLRMTrainStep:
               f"replicated tables in the fast step are updated by the dense optimizer kernel, "
               f"which has no row-wise form: embedding_optimizer={embedding_optimizer!r} needs "
               f"data_parallel_threshold=None (no replicated tables)")
+        if embedding_optimizer.lower() == "ftrl":
+          raise ValueError(
+              "replicated tables in the fast step are updated by the dense optimizer kernel, "
+              "which has no FTRL: a dense FTRL step would set every row the step does not touch "
+              "to the closed form of its z.  embedding_optimizer='ftrl' needs "
+              "data_parallel_threshold=None (no replicated tables)")
         raise ValueError("replicated tables in the fast step are updated by the dense optimizer "
                          "kernel: use the same embedding_optimizer and dense_optimizer ('sgd', "
                          "'adagrad' or 'adam') or data_parallel_threshold=None")

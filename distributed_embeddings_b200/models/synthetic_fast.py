@@ -45,7 +45,9 @@ class SyntheticTrainStep:
 
   ``dense_optimizer`` (``sgd`` | ``adagrad`` | ``adam``, hyperparameters in
   ``dense_optimizer_kwargs``) updates the MLP with the shared learning rate; the reference's
-  configuration is ``embedding_optimizer="adagrad", dense_optimizer="adagrad"``."""
+  configuration is ``embedding_optimizer="adagrad", dense_optimizer="adagrad"``.
+  ``embedding_optimizer`` is any kind of ``DistributedEmbedding.set_optimizer`` (``ftrl``
+  included), with its hyperparameters in ``embedding_optimizer_kwargs``."""
 
   def __init__(self, model: SyntheticModel, lr: float = 0.001, embedding_optimizer: str = "adagrad",
                use_cuda_graph: bool = True, embedding_optimizer_kwargs: Optional[dict] = None,

@@ -26,7 +26,9 @@ class HybridTrainer:
     model: module taking ``(numerical, categorical)``; must expose ``embedding``
       (DistributedEmbedding) and ``dense_parameters()``.
     lr: learning rate (dense SGD and fused embedding optimizer share it like the reference).
-    embedding_optimizer: ``sgd`` | ``adagrad`` | ``rowwise_adagrad`` | ``adam`` | ``rowwise_adam``.
+    embedding_optimizer: ``sgd`` | ``adagrad`` | ``rowwise_adagrad`` | ``adam`` | ``rowwise_adam``
+      | ``ftrl``; its hyperparameters in ``embedding_optimizer_kwargs`` go to both the fused
+      optimizer and the torch back end's :class:`SparseRowOptimizer`.
     scheduler: optional :class:`LearningRateScheduler`.
     dense_optimizer: ``sgd`` | ``adagrad`` | ``adam`` for the dense parameters (MLPs and
       replicated tables), hyperparameters in ``dense_optimizer_kwargs`` (see

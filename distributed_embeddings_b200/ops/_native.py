@@ -65,6 +65,7 @@ DTYPE_CODE = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
 
 OPT_SGD, OPT_ADAGRAD, OPT_ROWWISE_ADAGRAD, OPT_ADAM, OPT_EMIT = 0, 1, 2, 3, 4
 OPT_ROWWISE_ADAM = 5
+OPT_FTRL = 6
 MAX_PEERS = 16
 
 

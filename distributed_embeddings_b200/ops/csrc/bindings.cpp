@@ -356,7 +356,9 @@ void segment_update(const Tensor& descs, const Tensor& tables, int64_t n_tables,
                     double weight_decay, int64_t lr_ptr, const c10::optional<Tensor>& emit_keys,
                     const c10::optional<Tensor>& emit_rows, int64_t max_width, int64_t act_dtype,
                     bool vec4, const c10::optional<Tensor>& scratch, int64_t step_ptr,
-                    int64_t table_dtype, int64_t state_dtype) {
+                    int64_t table_dtype, int64_t state_dtype, double lr_power = -0.5,
+                    double l1 = 0.0, double l2 = 0.0, double l2_shrinkage = 0.0,
+                    double ftrl_beta = 0.0) {
   c10::cuda::CUDAGuard guard(descs.device());
   TORCH_CHECK(table_dtype >= 0 && table_dtype <= 2, "table_dtype: 0 fp32, 1 bf16, 2 fp16");
   TORCH_CHECK(state_dtype == 0 || state_dtype == 1, "state_dtype: 0 fp32, 1 bf16");
@@ -372,6 +374,11 @@ void segment_update(const Tensor& descs, const Tensor& tables, int64_t n_tables,
   opt.weight_decay = static_cast<float>(weight_decay);
   opt.lr_ptr = reinterpret_cast<const float*>(lr_ptr);
   opt.step_ptr = reinterpret_cast<const float*>(step_ptr);
+  opt.lr_power = static_cast<float>(lr_power);
+  opt.l1 = static_cast<float>(l1);
+  opt.l2 = static_cast<float>(l2);
+  opt.l2_shrinkage = static_cast<float>(l2_shrinkage);
+  opt.ftrl_beta = static_cast<float>(ftrl_beta);
   if (opt.kind == de::kOptEmit) TORCH_CHECK(emit_keys.has_value() && emit_rows.has_value());
   // occurrence-balanced path: immune to id skew (needs a zeroed scratch of >= n_items/32 rows)
   if (scratch.has_value() && vec4 && max_width <= 128 && opt.kind != de::kOptEmit) {
@@ -1442,7 +1449,9 @@ TORCH_LIBRARY(de_b200, m) {
       "Tensor seg_start, Tensor n_unique, int opt_kind, float lr, float eps, float beta1, "
       "float beta2, float bias1, float bias2, float grad_scale, float weight_decay, int lr_ptr, "
       "Tensor? emit_keys, Tensor? emit_rows, int max_width, int act_dtype, bool vec4, "
-      "Tensor? scratch, int step_ptr, int table_dtype=0, int state_dtype=0) -> ()",
+      "Tensor? scratch, int step_ptr, int table_dtype=0, int state_dtype=0, "
+      "float lr_power=-0.5, float l1=0., float l2=0., float l2_shrinkage=0., "
+      "float ftrl_beta=0.) -> ()",
       &segment_update);
   m.def(
       "embedding_lookup_fwd(Tensor param, Tensor values, Tensor? offsets, int hotness, int batch, "

@@ -83,14 +83,15 @@ enum OptimizerKind : int32_t {
   kOptAdam = 3,
   kOptEmit = 4,
   kOptRowwiseAdam = 5,  // Adam with element-wise m (state0) and one fp32 v word per row (state1)
+  kOptFtrl = 6,         // FTRL-Proximal: accumulator n (state0) and linear term z (state1)
 };
 
 // One entry per (fused) local table, used by the sorted/deduplicated update path.
 struct alignas(16) TableDesc {
   void* weight;       // [rows, width]; fp32, bf16 or fp16 (`table_dtype` of the launch)
   void* state0;       // Adagrad accumulator [rows,width] / row-wise [rows] / Adam m / row-wise
-                      // Adam m
-  void* state1;       // Adam v / row-wise Adam v [rows]  (element-wise state: fp32 or bf16,
+                      // Adam m / FTRL n
+  void* state1;       // Adam v / row-wise Adam v [rows] / FTRL z  (element-wise state: fp32 or bf16,
                       // `state_dtype` of the launch; row-wise state is always fp32)
   int64_t rows;
   int64_t key_base;   // first global row key of this table (prefix sum of rows)
@@ -110,6 +111,11 @@ struct OptimizerArgs {
   const float* step_ptr;  // optional device-resident Adam step count t (bias1/bias2 are then
                           // recomputed as 1 - beta^t on the device; graph replay safe); it
                           // also keys the stochastic rounding of 16-bit tables
+  // FTRL-Proximal (kind kOptFtrl; the other kinds ignore them): P(n) = n^(-lr_power)
+  float lr_power;
+  float l1, l2;
+  float l2_shrinkage;
+  float ftrl_beta;     // Keras's beta: adds beta / (2 lr) to l2
 };
 
 // ---- pooled lookup forward (+ optional fused push to peer output buffers) ------------------

@@ -1,7 +1,7 @@
 // Deduplicated sparse backward for sm_90a: (row key, item) pairs -> radix sort -> unique
 // segments -> one lane group per unique row sums its gradient rows (pulled from peer-mapped
 // gradient buffers when world_size > 1) and applies the optimizer update in place
-// (SGD / Adagrad / row-wise Adagrad / lazy Adam / lazy row-wise Adam), or emits
+// (SGD / Adagrad / row-wise Adagrad / lazy Adam / lazy row-wise Adam / FTRL-Proximal), or emits
 // (unique_ids, unique_grad) for an external optimizer.  The unique count never leaves the device (the reference copies it to the
 // host to size its output: cc/kernels/embedding_lookup_kernels.cu:663-670).
 //
@@ -83,10 +83,11 @@ __global__ void finish_segments_kernel(int64_t* seg_start, const int64_t* n_uniq
 }
 
 // The row pass of the sorted update kernels, their template parameter kRow (a bit set).  A launch
-// that needs neither bit takes the kRow = 0 instantiation; the bits give the row-wise optimizers
-// instantiations of their own, so the others keep their code and registers.
+// that needs none of the bits takes the kRow = 0 instantiation; the bits give the row-wise
+// optimizers and FTRL instantiations of their own, so the others keep their code and registers.
 constexpr int kRowDecay = 1;  // weight decay on: the row pass reads the weights (s * g + wd * w)
 constexpr int kRowAdam = 2;   // row-wise Adam (kind kOptRowwiseAdam)
+constexpr int kRowFtrl = 4;   // FTRL-Proximal (kind kOptFtrl): no row pass, its own apply_update
 
 // Adam bias corrections from a device-resident step count (the host scalars baked into a captured
 // CUDA graph would freeze at their capture-time values).
@@ -114,12 +115,22 @@ __device__ __forceinline__ uint32_t rounding_step(const OptimizerArgs& opt) {
 }
 
 // ------------------------------------------------------------------ per-row optimizer apply
+// FTRL's P(n) = n^(-lr_power); the default lr_power = -0.5 takes the square root.
+__device__ __forceinline__ float ftrl_pow(float n, float lr_power) {
+  return lr_power == -0.5f ? sqrtf(n) : powf(n, -lr_power);
+}
+
 // The weight is read in its storage type (TabT: fp32, bf16 or fp16) and the Adagrad / Adam state
 // in its own (StateT: fp32 or bf16), both widened to fp32; the optimizer runs in fp32, the weight
 // update uses the unrounded new state, and 16-bit weights and state are written back with
 // stochastic rounding (st_tab), each from its own random stream.  Every row has exactly one
 // writer per step, so each element is rounded once.  Row-wise state (row-wise Adagrad's
 // accumulator, row-wise Adam's v) is always fp32.
+//
+// FTRL-Proximal (TensorFlow's ApplyFtrlV2 with Keras's beta), g the decayed gradient:
+//   n' = n + g^2,  sigma = (P(n') - P(n)) / lr,  z += g + 2 l2_shrinkage w - sigma w,
+//   w = |z| > l1 ? (sign(z) l1 - z) / ((beta + P(n')) / lr + 2 l2) : 0,  n = n'.
+// At lr = 0 the row, n and z keep their bits (sigma would divide by zero).
 template <typename TabT, int VEC, typename StateT = float, int kRow = 0>
 __device__ __forceinline__ void apply_update(const TableDesc& T, const OptimizerArgs& opt,
                                              int64_t row, int col, const FVec<VEC>& g,
@@ -128,7 +139,24 @@ __device__ __forceinline__ void apply_update(const TableDesc& T, const Optimizer
   FVec<VEC> wv = ld_tab_rw<TabT, VEC>(w);
   FVec<VEC> gv = g;
   if (opt.weight_decay != 0.f) gv.fma(opt.weight_decay, wv);
-  if constexpr ((kRow & kRowAdam) != 0) {
+  if constexpr ((kRow & kRowFtrl) != 0) {
+    if (opt.lr == 0.f) return;
+    StateT* n = reinterpret_cast<StateT*>(T.state0) + row * T.width + col;
+    StateT* z = reinterpret_cast<StateT*>(T.state1) + row * T.width + col;
+    FVec<VEC> nv = ld_tab_rw<StateT, VEC>(n), zv = ld_tab_rw<StateT, VEC>(z);
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) {
+      const float n_new = fmaf(gv.v[i], gv.v[i], nv.v[i]);
+      const float p_new = ftrl_pow(n_new, opt.lr_power);
+      const float sigma = (p_new - ftrl_pow(nv.v[i], opt.lr_power)) / opt.lr;
+      zv.v[i] += gv.v[i] + 2.f * opt.l2_shrinkage * wv.v[i] - sigma * wv.v[i];
+      const float q = (opt.ftrl_beta + p_new) / opt.lr + 2.f * opt.l2;
+      wv.v[i] = fabsf(zv.v[i]) > opt.l1 ? (copysignf(opt.l1, zv.v[i]) - zv.v[i]) / q : 0.f;
+      nv.v[i] = n_new;
+    }
+    st_tab<StateT, VEC>(n, nv, step, T.key_base + row, col, kStreamState0);
+    st_tab<StateT, VEC>(z, zv, step, T.key_base + row, col, kStreamState1);
+  } else if constexpr ((kRow & kRowAdam) != 0) {
     // row-wise Adam: m element-wise; row_sumsq_mean carries the row's new v (the caller advanced
     // state1[row])
     StateT* m = reinterpret_cast<StateT*>(T.state0) + row * T.width + col;
@@ -272,7 +300,7 @@ __device__ __forceinline__ void segment_update_body(
     const int nvec = (W + VEC - 1) / VEC;
 
     float row_state = 0.f;
-    if ((kRow & kRowAdam) || opt.kind == kOptRowwiseAdagrad) {
+    if (!(kRow & kRowFtrl) && ((kRow & kRowAdam) || opt.kind == kOptRowwiseAdagrad)) {
       // pass 1: mean of squared (scaled) gradient over the whole row
       float ss = 0.f;
       if (valid) {
@@ -401,14 +429,14 @@ __device__ __forceinline__ int find_table(const TableDesc* __restrict__ tables, 
 }
 
 // Apply the optimizer to one row given the complete (scaled) gradient fragment of this lane.
-// kRow: the row pass of row-wise Adagrad / row-wise Adam (see segment_update_body).
+// kRow: the row pass of row-wise Adagrad / row-wise Adam, or FTRL (see segment_update_body).
 template <typename TabT, typename StateT, int kRow = 0>
 __device__ __forceinline__ void apply_row(const TableDesc& T, const OptimizerArgs& opt,
                                           int64_t row, int col, FVec<4> g, int lpr,
                                           unsigned group_mask, uint32_t step) {
   const bool col_ok = col < T.width;
   float row_state = 0.f;
-  if ((kRow & kRowAdam) || opt.kind == kOptRowwiseAdagrad) {
+  if (!(kRow & kRowFtrl) && ((kRow & kRowAdam) || opt.kind == kOptRowwiseAdagrad)) {
     float ss = 0.f;
     if (col_ok) {
       if constexpr ((kRow & kRowDecay) != 0) {
@@ -605,15 +633,20 @@ int grid_cap(int64_t work_warps, int sm_count, int per_sm) {
 }
 
 // The instantiation a sorted update launch takes: calls f(type_tag<TabT>, type_tag<StateT>,
-// kRow).  Only Adagrad, Adam and row-wise Adam read element-wise state, so every other optimizer
-// takes the fp32-state kernels; row-wise Adam has kernels of its own (kRowAdam); only the row-wise
-// optimizers with weight decay read the weights in their row pass (kRowDecay); the emit path never
-// touches the table, so one fp32-table instantiation serves every storage type.
+// kRow).  Only Adagrad, Adam, row-wise Adam and FTRL read element-wise state, so every other
+// optimizer takes the fp32-state kernels; row-wise Adam (kRowAdam) and FTRL (kRowFtrl) have
+// kernels of their own; only the row-wise optimizers with weight decay read the weights in their
+// row pass (kRowDecay); the emit path never touches the table, so one fp32-table instantiation
+// serves every storage type.
 template <typename F>
 void with_update_types(const OptimizerArgs& opt, int table_dtype, int state_dtype, F&& f) {
   using Plain = std::integral_constant<int, 0>;
   with_dtype(opt.kind == kOptEmit ? 0 : table_dtype, [&](auto tab) {
-    if (opt.kind == kOptRowwiseAdam) {
+    if (opt.kind == kOptFtrl) {
+      with_type_if<__nv_bfloat16, float>(state_dtype == 1, [&](auto state) {
+        f(tab, state, std::integral_constant<int, kRowFtrl>{});
+      });
+    } else if (opt.kind == kOptRowwiseAdam) {
       with_type_if<__nv_bfloat16, float>(state_dtype == 1, [&](auto state) {
         if (opt.weight_decay != 0.f)
           f(tab, state, std::integral_constant<int, kRowAdam | kRowDecay>{});

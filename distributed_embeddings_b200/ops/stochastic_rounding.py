@@ -23,9 +23,10 @@ with the same rule.  Each stored quantity draws from its own stream of the hash,
 decisions of a weight and of its state are independent:
 
 * stream 0: the weight (the bits of half-precision tables, unchanged by the streams);
-* stream 1: ``state0`` (the Adagrad accumulator, Adam's and row-wise Adam's ``m``);
-* stream 2: ``state1`` (Adam's ``v``; row-wise Adam's ``v`` is one fp32 word per row and is
-  never rounded).
+* stream 1: ``state0`` (the Adagrad accumulator, Adam's and row-wise Adam's ``m``, FTRL's
+  accumulator ``n``);
+* stream 2: ``state1`` (Adam's ``v``, FTRL's linear term ``z``; row-wise Adam's ``v`` is one fp32
+  word per row and is never rounded).
 
 The stream is folded into the step seed: ``mix((step + 0x9E3779B9 + stream * 0x632BE5AB) mod
 2**32)``.  Two streams draw the same bits only at step offsets of about 1.7e9, far beyond the

@@ -596,7 +596,8 @@ class DistributedEmbedding(nn.Module):
   def set_optimizer(self, kind: str = "sgd", lr: float = 0.01, **kwargs):
     """Attach an optimizer that is applied to the model-parallel tables *inside* the backward
     kernels (no sparse gradient is materialised).  ``kind``: ``sgd`` | ``adagrad`` |
-    ``rowwise_adagrad`` | ``adam`` | ``rowwise_adam``.  Only the fused back end consumes it.
+    ``rowwise_adagrad`` | ``adam`` | ``rowwise_adam`` | ``ftrl``.  Only the fused back end
+    consumes it.
 
     ``rowwise_adam`` is Adam with an element-wise first moment m and one fp32 second-moment word
     per row: ``v_row = beta2 * v_row + (1 - beta2) * mean_j(g_j^2)``, ``m = beta1 * m +
@@ -604,12 +605,22 @@ class DistributedEmbedding(nn.Module):
     It keeps one table-sized state instead of Adam's two.  A column-sliced table keeps one word
     per row in every slice, the mean over that slice's columns, as row-wise Adagrad does.
 
+    ``ftrl`` is FTRL-Proximal (McMahan et al. 2013; Keras ``Ftrl``, TensorFlow ``ApplyFtrlV2``)
+    with an element-wise accumulator n and linear term z.  With ``P(x) = x^(-lr_power)``, for a
+    touched row: ``n' = n + g^2``, ``z += g + 2 * l2_shrinkage * w - (P(n') - P(n)) / lr * w``,
+    ``w = (sign(z) * l1 - z) / ((beta + P(n')) / lr + 2 * l2)`` where ``|z| > l1``, else 0;
+    ``n = n'``.  The L1 term sets the rows it applies to exactly to zero.  At ``lr == 0`` (the
+    first step of a warm-up schedule) rows and state do not move.
+
     Keyword arguments (any other raises ``ValueError``):
 
     - ``eps``: added to the square root in the denominator (default 1e-7, Adam and row-wise Adam 1e-8).
     - ``beta1``, ``beta2``: Adam's moment decay rates (0.9, 0.999).
-    - ``initial_accumulator_value``: start value of the Adagrad / row-wise Adagrad accumulator
-      (0.1).
+    - ``initial_accumulator_value``: start value of the Adagrad / row-wise Adagrad / FTRL
+      accumulator (0.1).
+    - ``lr_power`` (-0.5, at most 0), ``l1``, ``l2``, ``l2_shrinkage``, ``beta`` (0, at least 0):
+      FTRL only, Keras's ``learning_rate_power``, ``l1_regularization_strength``,
+      ``l2_regularization_strength``, ``l2_shrinkage_regularization_strength`` and ``beta``.
     - ``weight_decay``: L2 decay (default 0).  ``weight_decay * w`` is added to the summed,
       scaled gradient of a row before the optimizer sees it, once per step for every row that at
       least one id of the step touched (a row whose ids carry only zero gradients included).  The
@@ -620,11 +631,11 @@ class DistributedEmbedding(nn.Module):
       the sorted update, which sums each row's gradient before it applies it.
     - ``step``: the Adam / row-wise Adam step count to resume from (0).
     - ``state_dtype``: storage of the Adagrad accumulator / Adam moments / row-wise Adam's m
-      (its v stays one fp32 word per row), ``torch.float32``
+      (its v stays one fp32 word per row) / FTRL's n and z, ``torch.float32``
       (default) or ``torch.bfloat16`` (half the bytes; the update runs in fp32 and stores the
       state with stochastic rounding, see the user guide, "Half-precision optimizer state")."""
     kind = kind.lower()
-    if kind not in ("sgd", "adagrad", "rowwise_adagrad", "adam", "rowwise_adam"):
+    if kind not in ("sgd", "adagrad", "rowwise_adagrad", "adam", "rowwise_adam", "ftrl"):
       raise ValueError(f"Unsupported fused optimizer {kind}")
     state_dtype = check_state_dtype(kind, kwargs.pop("state_dtype", torch.float32))
     if state_dtype != torch.float32 and self.offload_cache_size is not None:
@@ -634,11 +645,15 @@ class DistributedEmbedding(nn.Module):
            "eps": 1e-8 if kind in ("adam", "rowwise_adam") else 1e-7,
            "beta1": 0.9, "beta2": 0.999, "weight_decay": 0.0, "initial_accumulator_value": 0.1,
            "deterministic": kind != "sgd", "step": 0, "state_dtype": state_dtype}
+    if kind == "ftrl":
+      cfg.update(FTRL_DEFAULTS)
     unknown = sorted(set(kwargs) - set(cfg))
     if unknown:
       raise ValueError(f"unknown fused optimizer argument(s) {unknown}; the known ones are "
                        f"{sorted(set(cfg) - {'kind', 'lr'})}")
     cfg.update(kwargs)
+    if kind == "ftrl":
+      check_ftrl_args(cfg)
     self._fused_optimizer = cfg
     if self._engine is not None:
       self._engine.reset_optimizer_state()
@@ -1111,6 +1126,21 @@ def _flush_before_state_dict(module, prefix, keep_vars):  # pylint: disable=unus
 
 def _drop_before_load(module, *args, **kwargs):  # pylint: disable=unused-argument
   module._drop_offload_cache()  # pylint: disable=protected-access
+
+
+# FTRL's hyperparameters and their defaults (Keras ``Ftrl``: learning_rate_power,
+# l1_regularization_strength, l2_regularization_strength, l2_shrinkage_regularization_strength,
+# beta); ``initial_accumulator_value`` is shared with Adagrad
+FTRL_DEFAULTS = {"lr_power": -0.5, "l1": 0.0, "l2": 0.0, "l2_shrinkage": 0.0, "beta": 0.0}
+
+
+def check_ftrl_args(cfg: Dict[str, Any]):
+  """Keras's checks of FTRL's hyperparameters: ``lr_power <= 0``, the others ``>= 0``."""
+  if not float(cfg["lr_power"]) <= 0.0:
+    raise ValueError(f"ftrl: lr_power must be <= 0, got {cfg['lr_power']}")
+  for k in ("initial_accumulator_value", "l1", "l2", "l2_shrinkage", "beta"):
+    if not float(cfg[k]) >= 0.0:
+      raise ValueError(f"ftrl: {k} must be >= 0, got {cfg[k]}")
 
 
 # ------------------------------------------------------------------------- hybrid-parallel glue

@@ -502,14 +502,15 @@ class DryOps:
   def segment_update(self, descs, tables, n_tables, batch, grad_batch, grad_stride, grad_ptrs,
                      keys, items, seg, n_unique, kind, lr, eps, beta1, beta2, bias1, bias2,
                      grad_scale, weight_decay, lr_ptr, emit_keys, emit_rows, max_width, act_dtype,
-                     vec4, scratch, step_ptr, table_dtype=0, state_dtype=0):
+                     vec4, scratch, step_ptr, table_dtype=0, state_dtype=0, lr_power=-0.5,
+                     l1=0.0, l2=0.0, l2_shrinkage=0.0, ftrl_beta=0.0):
     self._count("segment_update")
     tdt = self._ADT[int(table_dtype)]
     tsz = 4 if int(table_dtype) == 0 else 2
-    # Adagrad / Adam state and row-wise Adam's m in bf16: widened to fp32 for the update, stored
-    # with stochastic rounding (streams 1 and 2); the other optimizers ignore the code, like the
-    # kernels
-    half_state = int(state_dtype) == 1 and kind in (1, 3, 5)
+    # Adagrad / Adam / FTRL state and row-wise Adam's m in bf16: widened to fp32 for the update,
+    # stored with stochastic rounding (streams 1 and 2); the other optimizers ignore the code, like
+    # the kernels
+    half_state = int(state_dtype) == 1 and kind in (1, 3, 5, 6)
     sdt, ssz = (torch.bfloat16, 2) if half_state else (torch.float32, 4)
 
     def state(ptr, row, width, what):
@@ -519,6 +520,8 @@ class DryOps:
     # the kernels take the optimizer constants in fp32 and form 1 - beta and the bias
     # corrections in fp32 from them
     beta1, beta2 = float(np.float32(beta1)), float(np.float32(beta2))
+    lr_power, l1, l2, l2_shrinkage, ftrl_beta = (
+        float(np.float32(x)) for x in (lr_power, l1, l2, l2_shrinkage, ftrl_beta))
     if step_ptr:
       t = float(self.world.tensor(int(step_ptr), torch.float32, 1, "optimizer step")[0])
       step = int(t)
@@ -602,6 +605,22 @@ class DryOps:
         wt -= lr * (mm / bias1) / ((vr / bias2).sqrt() + eps)
         if half_state:
           m16.copy_(stochastic_round(mm, sdt, step, key, stream=STREAM_STATE0))
+      elif kind == 6:
+        # FTRL-Proximal: n (state0) and z (state1); at lr == 0 nothing moves
+        if lr == 0.0:
+          continue
+        n16, n = state(t["state0"], row, width, "ftrl n")
+        z16, z = state(t["state1"], row, width, "ftrl z")
+        pw = (lambda x: x.sqrt()) if lr_power == -0.5 else (lambda x: x.pow(-lr_power))
+        n_new = n + g * g
+        p_new = pw(n_new)
+        z += g + 2 * l2_shrinkage * wt - (p_new - pw(n)) / lr * wt
+        q = (ftrl_beta + p_new) / lr + 2 * l2
+        wt.copy_(torch.where(z.abs() > l1, (torch.sign(z) * l1 - z) / q, torch.zeros_like(z)))
+        n.copy_(n_new)
+        if half_state:
+          n16.copy_(stochastic_round(n, sdt, step, key, stream=STREAM_STATE0))
+          z16.copy_(stochastic_round(z, sdt, step, key, stream=STREAM_STATE1))
       else:
         raise ValueError(f"optimizer kind {kind}")
       if tsz == 2:

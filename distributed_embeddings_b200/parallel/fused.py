@@ -50,7 +50,7 @@ from .offload_cache import OffloadCache, split_budget
 
 _OPT_KIND = {"sgd": _native.OPT_SGD, "adagrad": _native.OPT_ADAGRAD,
              "rowwise_adagrad": _native.OPT_ROWWISE_ADAGRAD, "adam": _native.OPT_ADAM,
-             "rowwise_adam": _native.OPT_ROWWISE_ADAM}
+             "rowwise_adam": _native.OPT_ROWWISE_ADAM, "ftrl": _native.OPT_FTRL}
 _COMB = {None: 0, "sum": 0, "mean": 1}
 
 # InputDesc.flags
@@ -875,6 +875,10 @@ class FusedEngine:
       elif kind == "rowwise_adam":
         # m element-wise (in the state dtype), v one fp32 word per row
         self.opt_state[m] = [like(w, 0.0, dtype=sdt), like(w, 0.0, (w.shape[0],))]
+      elif kind == "ftrl":
+        # accumulator n and linear term z, both element-wise in the state dtype
+        self.opt_state[m] = [like(w, opt["initial_accumulator_value"], dtype=sdt),
+                             like(w, 0.0, dtype=sdt)]
     self._tables_dirty = True
 
   @property
@@ -1272,17 +1276,22 @@ class FusedEngine:
       if not self._dry_updates:
         self.step_t.add_(1.0)  # device counter: bias corrections stay right under graph replay
       kind = _OPT_KIND[opt["kind"]]
-      if self._dry_updates and opt["kind"] in ("adam", "rowwise_adam"):
-        kind = _OPT_KIND["sgd"]  # a zero gradient would still decay Adam's moments
+      if self._dry_updates and opt["kind"] in ("adam", "rowwise_adam", "ftrl"):
+        # a zero gradient would still decay Adam's moments, and would set FTRL's weights to the
+        # closed form of z
+        kind = _OPT_KIND["sgd"]
       # a dry update has no decay either: weight_decay * w would move the weights and feed the
       # Adagrad accumulators on every warm-up pass
       wd = 0.0 if self._dry_updates else opt["weight_decay"]
+      # FTRL's hyperparameters trail the op's arguments (the other kinds launch without them)
+      ftrl = tuple(opt[k] for k in ("lr_power", "l1", "l2", "l2_shrinkage", "beta")) \
+          if kind == _native.OPT_FTRL else ()
       ops.segment_update(self.mpdesc, self.tdesc, n_mp, B, B, self.recv_width, self.recv_ptr,
                          keys, items, seg, n_unique, kind, opt["lr"],
                          opt["eps"], opt["beta1"], opt["beta2"], 1.0, 1.0, gscale,
                          wd, self.lr_t.data_ptr(), None, None, self.max_width,
                          self.act, self.vec4, self._balanced_scratch(), self.step_t.data_ptr(),
-                         self.tab, DTYPE_CODE[self.state_dtype])
+                         self.tab, DTYPE_CODE[self.state_dtype], *ftrl)
       if multi:
         ops.sync_only(self._sync(signal=CH_CONSUMED))
       return [None] * n_mp

@@ -21,7 +21,7 @@ from torch import nn
 from ..ops.stochastic_rounding import (HALF_DTYPES, STREAM_STATE0, STREAM_STATE1,
                                        check_state_dtype, stochastic_round)
 from .comm import CommContext, dist_ready
-from .dist_model_parallel import _is_mp, broadcast_variables
+from .dist_model_parallel import FTRL_DEFAULTS, _is_mp, broadcast_variables, check_ftrl_args
 
 
 def _world(group=None) -> int:
@@ -258,25 +258,33 @@ class SparseRowOptimizer:
   tensors - the ``torch`` back end of :class:`DistributedEmbedding`, i.e. the NCCL-collectives
   baseline, which has no fused update.  Same math as the fused kernels
   (``ops/csrc/sparse_update_kernels.cu``): ``sgd`` | ``adagrad`` | ``rowwise_adagrad`` | ``adam``
-  | ``rowwise_adam`` (lazy: only the touched rows advance).  Counterpart of the Keras sparse-apply
-  kernels the reference relies on (examples/benchmarks/synthetic_models/main.py:96-101).
+  | ``rowwise_adam`` | ``ftrl`` (lazy: only the touched rows advance).  ``ftrl`` takes the
+  keyword arguments of ``DistributedEmbedding.set_optimizer("ftrl")`` (``lr_power``, ``l1``,
+  ``l2``, ``l2_shrinkage``, ``beta``); the other kinds reject them.  Counterpart of the Keras
+  sparse-apply kernels the reference relies on (examples/benchmarks/synthetic_models/main.py:96-101).
 
   bf16 / fp16 parameters keep fp32 state; their touched rows are updated in fp32 and written
   back with stochastic rounding keyed by (step, row, column), the rule of the fused kernels
   (``ops/stochastic_rounding.py``).
 
   ``state_dtype=torch.bfloat16`` stores the Adagrad accumulator / Adam moments / row-wise Adam's
-  m in bf16 like the fused back end: the touched rows' state is widened to fp32, the update runs
-  in fp32 with the unrounded new state, and the state is stored with stochastic rounding
-  (streams 1 and 2).  Row-wise state (one word per row) stays fp32."""
+  m / FTRL's n and z in bf16 like the fused back end: the touched rows' state is widened to fp32,
+  the update runs in fp32 with the unrounded new state, and the state is stored with stochastic
+  rounding (streams 1 and 2).  Row-wise state (one word per row) stays fp32."""
 
   def __init__(self, params: Sequence[nn.Parameter], kind: str = "sgd", lr: float = 0.01,
                eps: Optional[float] = None, beta1: float = 0.9, beta2: float = 0.999,
                initial_accumulator_value: float = 0.1, weight_decay: float = 0.0,
-               state_dtype: torch.dtype = torch.float32):
+               state_dtype: torch.dtype = torch.float32, **ftrl):
     kind = kind.lower()
-    if kind not in ("sgd", "adagrad", "rowwise_adagrad", "adam", "rowwise_adam"):
+    if kind not in ("sgd", "adagrad", "rowwise_adagrad", "adam", "rowwise_adam", "ftrl"):
       raise ValueError(f"Unsupported optimizer {kind}")
+    unknown = sorted(set(ftrl) - (set(FTRL_DEFAULTS) if kind == "ftrl" else set()))
+    if unknown:
+      raise ValueError(f"unknown fused optimizer argument(s) {unknown} for {kind}")
+    self.ftrl = dict(FTRL_DEFAULTS, initial_accumulator_value=initial_accumulator_value, **ftrl)
+    if kind == "ftrl":
+      check_ftrl_args(self.ftrl)
     self.state_dtype = check_state_dtype(kind, state_dtype)
     self.params = [p for p in params if p.requires_grad]
     self.kind, self.lr = kind, float(lr)
@@ -297,6 +305,9 @@ class SparseRowOptimizer:
       elif kind == "rowwise_adam":
         self.state.append([torch.zeros_like(p, dtype=esdt),
                            torch.zeros((p.shape[0],), dtype=sdt, device=p.device)])
+      elif kind == "ftrl":
+        self.state.append([torch.full_like(p, initial_accumulator_value, dtype=esdt),
+                           torch.zeros_like(p, dtype=esdt)])
       else:
         self.state.append([])
 
@@ -339,6 +350,9 @@ class SparseRowOptimizer:
         b1 = 1 - self.beta1**self.step_count
         b2 = 1 - self.beta2**self.step_count
         p.index_add_(0, idx, (m / b1) / ((v / b2).sqrt().unsqueeze(1) + self.eps), alpha=-self.lr)
+      elif self.kind == "ftrl":
+        if self.lr != 0.0:
+          p[idx], st[0][idx], st[1][idx] = self._ftrl(p[idx], val, st[0][idx], st[1][idx])
       else:
         m = self.beta1 * st[0][idx] + (1 - self.beta1) * val
         v = self.beta2 * st[1][idx] + (1 - self.beta2) * val * val
@@ -372,6 +386,12 @@ class SparseRowOptimizer:
       b1 = 1 - self.beta1**self.step_count
       b2 = 1 - self.beta2**self.step_count
       w = w - self.lr * (m / b1) / ((v / b2).sqrt().unsqueeze(1) + self.eps)
+    elif self.kind == "ftrl":
+      if self.lr == 0.0:
+        return  # rows and state keep their bits
+      w, n, z = self._ftrl(w, val, st[0][idx].float(), st[1][idx].float())
+      self._store_state(st[0], idx, n, STREAM_STATE0)
+      self._store_state(st[1], idx, z, STREAM_STATE1)
     else:
       m = self.beta1 * st[0][idx].float() + (1 - self.beta1) * val
       v = self.beta2 * st[1][idx].float() + (1 - self.beta2) * val * val
@@ -384,6 +404,18 @@ class SparseRowOptimizer:
       p[idx] = stochastic_round(w, p.dtype, self.step_count, idx).to(p.device)
     else:
       p[idx] = w
+
+  def _ftrl(self, w, g, n, z):
+    """FTRL-Proximal on rows ``w`` with decayed gradient ``g``, accumulator ``n`` and linear term
+    ``z`` (lr != 0); returns the new (w, n, z)."""
+    c = self.ftrl
+    pw = (lambda x: x.sqrt()) if c["lr_power"] == -0.5 else (lambda x: x.pow(-c["lr_power"]))
+    n_new = n + g * g
+    p_new = pw(n_new)
+    z = z + g + 2 * c["l2_shrinkage"] * w - (p_new - pw(n)) / self.lr * w
+    q = (c["beta"] + p_new) / self.lr + 2 * c["l2"]
+    w = torch.where(z.abs() > c["l1"], (torch.sign(z) * c["l1"] - z) / q, torch.zeros_like(z))
+    return w, n_new, z
 
   def _store_state(self, s, idx, x, stream):
     """Store fp32 state rows ``x`` at ``idx``: as is, or stochastically rounded into bf16."""

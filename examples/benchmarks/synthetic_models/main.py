@@ -38,7 +38,7 @@ def main():
   p.add_argument("--dp_input", action="store_true")
   p.add_argument("--model", default="tiny", choices=sorted(synthetic_models_v3))
   p.add_argument("--optimizer", default="sgd", choices=["sgd", "adagrad", "rowwise_adagrad", "adam",
-                                                     "rowwise_adam"])
+                                                     "rowwise_adam", "ftrl"])
   p.add_argument("--dense_optimizer", default="sgd", choices=["sgd", "adagrad", "adam"],
                  help="optimizer of the MLP (--embedding_api de); the reference uses --optimizer's")
   p.add_argument("--column_slice_threshold", type=int, default=None)
@@ -103,7 +103,7 @@ def main():
 
   if args.embedding_api == "de":
     lr = {"sgd": 0.03, "adagrad": 0.001, "rowwise_adagrad": 0.001, "adam": 0.001,
-          "rowwise_adam": 0.001}[args.optimizer]
+          "rowwise_adam": 0.001, "ftrl": 0.01}[args.optimizer]
     opt_kwargs = {"state_dtype": {"fp32": torch.float32,
                                   "bf16": torch.bfloat16}[args.optimizer_state_dtype]}
     from distributed_embeddings_b200.models.synthetic_fast import SyntheticTrainStep

@@ -72,10 +72,10 @@ def parse():
                  help="storage of the model-parallel embedding tables (bf16 / fp16: half the "
                       "memory, stochastically rounded updates)")
   p.add_argument("--embedding_optimizer", default="sgd",
-                 choices=["sgd", "adagrad", "rowwise_adagrad", "adam", "rowwise_adam"],
+                 choices=["sgd", "adagrad", "rowwise_adagrad", "adam", "rowwise_adam", "ftrl"],
                  help="fused optimizer of the model-parallel tables")
   p.add_argument("--optimizer_state_dtype", default="fp32", choices=["fp32", "bf16"],
-                 help="storage of the Adagrad / Adam state (row-wise Adam: its m) of the "
+                 help="storage of the Adagrad / Adam / FTRL state (row-wise Adam: its m) of the "
                       "model-parallel tables (bf16: half the memory, stochastically rounded)")
   p.add_argument("--warmup_steps", type=int, default=8000)
   p.add_argument("--decay_start_step", type=int, default=48000)

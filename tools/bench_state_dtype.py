@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""fp32 versus bf16 optimizer state (Adagrad accumulator, Adam moments, row-wise Adam's m) in the
-single-GPU DLRM training step.
+"""fp32 versus bf16 optimizer state (Adagrad accumulator, Adam moments, row-wise Adam's m, FTRL's
+n and z) in the single-GPU DLRM training step.
 
   python tools/bench_state_dtype.py [--steps 30] [--warmup 5] [--repeats 3] [--loss-steps 40]
-                                    [--profile] [--optimizers adagrad,adam,rowwise_adam]
+                                    [--profile] [--optimizers adagrad,adam,rowwise_adam,ftrl]
 
 One invocation, one GPU, the MLPerf tables capped at ``--max-rows`` (default 20M:
 ``dlrm-mlperf-20m`` of ``bench.py``, whose id generator this uses), ``DLRMTrainStep`` (CUDA graph,
@@ -11,7 +11,8 @@ bf16 compute) at global batch 65536.  At 20M rows only the bf16-state and the sm
 configurations fit one 80 GB card; ``--max-rows 5000000`` fits all of them:
 
 1. ``--optimizers`` (default Adagrad and Adam; ``rowwise_adam`` adds row-wise Adam, whose bf16
-   state is its m: v stays one fp32 word per row) x {fp32, bf16} tables x {fp32, bf16} state,
+   state is its m: v stays one fp32 word per row; ``ftrl`` adds FTRL, two element-wise slots
+   like Adam) x {fp32, bf16} tables x {fp32, bf16} state,
    alternating, ``--repeats`` times
    each: device-timed ms per step (CUDA events around ``--steps`` graph replays; median and spread
    over the repeats), samples/s and ``torch.cuda.max_memory_allocated``.  A configuration whose
@@ -44,9 +45,9 @@ from bench import gen_ids  # noqa: E402
 from distributed_embeddings_b200.models.dlrm import mlperf_table_sizes  # noqa: E402
 
 _DTYPES = {"fp32": torch.float32, "bf16": torch.bfloat16}
-_SLOTS = {"adagrad": 1, "adam": 2, "rowwise_adam": 1}   # element-wise state slots
-_ROW_SLOTS = {"adagrad": 0, "adam": 0, "rowwise_adam": 1}  # fp32 words per row
-_LR = {"adagrad": 0.01, "adam": 0.0001, "rowwise_adam": 0.0001}
+_SLOTS = {"adagrad": 1, "adam": 2, "rowwise_adam": 1, "ftrl": 2}   # element-wise state slots
+_ROW_SLOTS = {"adagrad": 0, "adam": 0, "rowwise_adam": 1, "ftrl": 0}  # fp32 words per row
+_LR = {"adagrad": 0.01, "adam": 0.0001, "rowwise_adam": 0.0001, "ftrl": 0.01}
 _UPDATE_KERNELS = ("segment_update", "balanced_update", "finalize_crossing")
 DIM = 128
 
@@ -153,7 +154,7 @@ def main():
   ap.add_argument("--max-rows", type=int, default=20_000_000)
   ap.add_argument("--profile", action="store_true")
   ap.add_argument("--optimizers", default="adagrad,adam",
-                  help="comma-separated subset of adagrad, adam, rowwise_adam")
+                  help="comma-separated subset of adagrad, adam, rowwise_adam, ftrl")
   args = ap.parse_args()
   kinds = [k for k in args.optimizers.split(",") if k]
   if not kinds or any(k not in _SLOTS for k in kinds):
