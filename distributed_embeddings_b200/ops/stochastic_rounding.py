@@ -67,20 +67,6 @@ def random_bits(step: int, keys, cols, stream: int = STREAM_WEIGHT) -> np.ndarra
   return _mix(h ^ cols).astype(np.uint32)
 
 
-def check_state_dtype(kind: str, state_dtype: torch.dtype) -> torch.dtype:
-  """Validate the storage dtype of an optimizer's per-element state; returns it."""
-  if state_dtype not in (torch.float32, torch.bfloat16):
-    raise ValueError(
-        f"optimizer state_dtype must be torch.float32 or torch.bfloat16, not {state_dtype} "
-        "(fp16 cannot hold it: an Adagrad accumulator can pass 65504 and Adam's v underflows)")
-  if state_dtype == torch.bfloat16 and kind == "sgd":
-    raise ValueError("state_dtype=torch.bfloat16 needs an optimizer with state: sgd has none")
-  if state_dtype == torch.bfloat16 and kind == "rowwise_adagrad":
-    raise ValueError("state_dtype=torch.bfloat16 does not apply to rowwise_adagrad: its one "
-                     "fp32 word per row stays fp32")
-  return state_dtype
-
-
 def _ordered(bits: np.ndarray) -> np.ndarray:
   b = bits.astype(np.int32)
   return np.where(b & 0x8000, -(b & 0x7FFF), b)

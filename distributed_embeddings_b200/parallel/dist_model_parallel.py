@@ -17,7 +17,7 @@ reference (``DistributedEmbedding`` :712-1214, hybrid helpers :1217-1329).
 from __future__ import annotations
 
 import os
-from typing import Any, Dict, List, Optional, Sequence, Tuple, Union
+from typing import Any, Dict, List, Optional, Sequence, Union
 
 import numpy as np
 import torch
@@ -27,9 +27,9 @@ from torch import nn
 from ..layers.embedding import Embedding, config_from_layer
 from ..ops import embedding_lookup_ops as elo
 from ..ops.ragged import RaggedIds, SparseIds
-from ..ops.stochastic_rounding import check_state_dtype
 from ..utils import initializers
 from .comm import dist_ready
+from .embedding_optimizers import OPTIMIZERS, check_state_dtype
 from .strategy import DistEmbeddingStrategy, STRATEGIES, suggest_column_slice_threshold
 
 
@@ -635,25 +635,23 @@ class DistributedEmbedding(nn.Module):
       (default) or ``torch.bfloat16`` (half the bytes; the update runs in fp32 and stores the
       state with stochastic rounding, see the user guide, "Half-precision optimizer state")."""
     kind = kind.lower()
-    if kind not in ("sgd", "adagrad", "rowwise_adagrad", "adam", "rowwise_adam", "ftrl"):
+    if kind not in OPTIMIZERS:
       raise ValueError(f"Unsupported fused optimizer {kind}")
+    entry = OPTIMIZERS[kind]
     state_dtype = check_state_dtype(kind, kwargs.pop("state_dtype", torch.float32))
     if state_dtype != torch.float32 and self.offload_cache_size is not None:
       raise ValueError("state_dtype=torch.bfloat16 is not supported with offload_cache_size: the "
                        "HBM row cache keeps optimizer state rows as fp32 words")
-    cfg = {"kind": kind, "lr": float(lr),
-           "eps": 1e-8 if kind in ("adam", "rowwise_adam") else 1e-7,
+    cfg = {"kind": kind, "lr": float(lr), "eps": entry.eps,
            "beta1": 0.9, "beta2": 0.999, "weight_decay": 0.0, "initial_accumulator_value": 0.1,
-           "deterministic": kind != "sgd", "step": 0, "state_dtype": state_dtype}
-    if kind == "ftrl":
-      cfg.update(FTRL_DEFAULTS)
+           "deterministic": kind != "sgd", "step": 0, "state_dtype": state_dtype, **entry.hyper}
     unknown = sorted(set(kwargs) - set(cfg))
     if unknown:
       raise ValueError(f"unknown fused optimizer argument(s) {unknown}; the known ones are "
                        f"{sorted(set(cfg) - {'kind', 'lr'})}")
     cfg.update(kwargs)
-    if kind == "ftrl":
-      check_ftrl_args(cfg)
+    if entry.check is not None:
+      entry.check(cfg)
     self._fused_optimizer = cfg
     if self._engine is not None:
       self._engine.reset_optimizer_state()
@@ -961,10 +959,8 @@ class DistributedEmbedding(nn.Module):
       return {"kind": opt["kind"] if opt else None, "step": eng.step_count() if eng else 0,
               "tables": None}
     kind = opt["kind"]
-    n_col = len(self.local_embedding_layers)
-    n_slots = len(next(iter(eng.opt_state.values())))
-    per_row = _per_row_slots(kind, n_slots)
-    slots = [self._gather_slot(k, per_row[k], all_ranks) for k in range(n_slots)]
+    slots = [self._gather_slot(k, s.per_row, all_ranks)
+             for k, s in enumerate(OPTIMIZERS[kind].slots)]
     tables = None
     if slots and slots[0]:
       tables = [None if slots[0][t] is None else [sl[t] for sl in slots]
@@ -1002,7 +998,7 @@ class DistributedEmbedding(nn.Module):
     if tables is not None:
       st = self.strategy
       n_col = len(self.local_embedding_layers)
-      per_row = _per_row_slots(state["kind"], len(next(iter(eng.opt_state.values()))))
+      per_row = [s.per_row for s in OPTIMIZERS[state["kind"]].slots]
       with torch.no_grad():
         for s in st.shards[self.rank] if st.table_groups[1] else []:
           t = st.table_groups[1][s.table]
@@ -1042,7 +1038,8 @@ class DistributedEmbedding(nn.Module):
       return None
     st = self.strategy
     kind = opt["kind"]
-    n_slots = len(next(iter(eng.opt_state.values())))
+    per_row = [s.per_row for s in OPTIMIZERS[kind].slots]
+    n_slots = len(per_row)
     n_tables = len(st.global_configs)
     meta_path = os.path.join(directory, "optimizer.json")
     has_state = [t not in st.table_groups[0] for t in range(n_tables)]
@@ -1050,7 +1047,6 @@ class DistributedEmbedding(nn.Module):
     def path(t, k):
       return os.path.join(directory, f"opt_{t}_slot{k}.npy")
 
-    per_row = _per_row_slots(kind, n_slots)
     rows_k = [k for k in range(n_slots) if per_row[k]]
     elem_k = [k for k in range(n_slots) if not per_row[k]]
     for k in rows_k:
@@ -1128,28 +1124,7 @@ def _drop_before_load(module, *args, **kwargs):  # pylint: disable=unused-argume
   module._drop_offload_cache()  # pylint: disable=protected-access
 
 
-# FTRL's hyperparameters and their defaults (Keras ``Ftrl``: learning_rate_power,
-# l1_regularization_strength, l2_regularization_strength, l2_shrinkage_regularization_strength,
-# beta); ``initial_accumulator_value`` is shared with Adagrad
-FTRL_DEFAULTS = {"lr_power": -0.5, "l1": 0.0, "l2": 0.0, "l2_shrinkage": 0.0, "beta": 0.0}
-
-
-def check_ftrl_args(cfg: Dict[str, Any]):
-  """Keras's checks of FTRL's hyperparameters: ``lr_power <= 0``, the others ``>= 0``."""
-  if not float(cfg["lr_power"]) <= 0.0:
-    raise ValueError(f"ftrl: lr_power must be <= 0, got {cfg['lr_power']}")
-  for k in ("initial_accumulator_value", "l1", "l2", "l2_shrinkage", "beta"):
-    if not float(cfg[k]) >= 0.0:
-      raise ValueError(f"ftrl: {k} must be >= 0, got {cfg[k]}")
-
-
 # ------------------------------------------------------------------------- hybrid-parallel glue
-def _per_row_slots(kind: str, n_slots: int) -> Tuple[bool, ...]:
-  """Which state slots of optimizer ``kind`` hold one fp32 word per row (row-wise optimizers);
-  the others are element-wise, ``[rows, width]``."""
-  return {"rowwise_adagrad": (True,), "rowwise_adam": (False, True)}.get(kind, (False,) * n_slots)
-
-
 def _is_mp(p) -> bool:
   return bool(getattr(p, "de_local", False))
 

@@ -31,9 +31,11 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import numpy as np
 import torch
 
-from ..ops._native import GRAD_ROUTE, INPUT_DESC, MAX_PEERS, TABLE_DESC
+from ..ops._native import (GRAD_ROUTE, INPUT_DESC, MAX_PEERS, OPT_ADAGRAD, OPT_ADAM, OPT_EMIT,
+                           OPT_FTRL, OPT_ROWWISE_ADAGRAD, OPT_ROWWISE_ADAM, OPT_SGD, TABLE_DESC)
 from ..ops.stochastic_rounding import STREAM_STATE0, STREAM_STATE1, stochastic_round
 from . import fused as _fused
+from .embedding_optimizers import BY_CODE
 
 
 class DryWorld:
@@ -510,7 +512,7 @@ class DryOps:
     # Adagrad / Adam / FTRL state and row-wise Adam's m in bf16: widened to fp32 for the update,
     # stored with stochastic rounding (streams 1 and 2); the other optimizers ignore the code, like
     # the kernels
-    half_state = int(state_dtype) == 1 and kind in (1, 3, 5, 6)
+    half_state = int(state_dtype) == 1 and kind in BY_CODE and BY_CODE[kind].elementwise_state
     sdt, ssz = (torch.bfloat16, 2) if half_state else (torch.float32, 4)
 
     def state(ptr, row, width, what):
@@ -525,7 +527,7 @@ class DryOps:
     if step_ptr:
       t = float(self.world.tensor(int(step_ptr), torch.float32, 1, "optimizer step")[0])
       step = int(t)
-      if kind in (3, 5):
+      if kind in (OPT_ADAM, OPT_ROWWISE_ADAM):
         bias1 = float(np.float32(1) - np.float32(beta1)**np.float32(t))
         bias2 = float(np.float32(1) - np.float32(beta2)**np.float32(t))
     D = self._descs(descs, 1 << 30)
@@ -541,7 +543,7 @@ class DryOps:
       k0, k1 = int(seg[u]), int(seg[u + 1])
       key = int(keys[k0])
       if key >= sentinel:
-        if kind == 4:
+        if kind == OPT_EMIT:
           emit_keys[u] = sentinel
         continue
       m = max(i for i, b in enumerate(bases) if b <= key)
@@ -565,7 +567,7 @@ class DryOps:
                                 gdt, width, "gradient source")
         acc += w * src.float()
       g = acc * grad_scale
-      if kind == 4:
+      if kind == OPT_EMIT:
         emit_keys[u] = key
         emit_rows[u, :width] = g
         continue
@@ -575,19 +577,19 @@ class DryOps:
         w16, wt = wt, wt.float()
       if weight_decay:
         g = g + weight_decay * wt
-      if kind == 0:
+      if kind == OPT_SGD:
         wt -= lr * g
-      elif kind == 1:
+      elif kind == OPT_ADAGRAD:
         a16, a = state(t["state0"], row, width, "state0")
         a += g * g
         wt -= lr * g / (a.sqrt() + eps)
         if half_state:
           a16.copy_(stochastic_round(a, sdt, step, key, stream=STREAM_STATE0))
-      elif kind == 2:
+      elif kind == OPT_ROWWISE_ADAGRAD:
         a = self.world.tensor(int(t["state0"]) + row * 4, torch.float32, 1, "row state")
         a += (g * g).sum() / width
         wt -= lr * g / (a.sqrt() + eps)
-      elif kind == 3:
+      elif kind == OPT_ADAM:
         m16, mm = state(t["state0"], row, width, "adam m")
         v16, vv = state(t["state1"], row, width, "adam v")
         mm.mul_(beta1).add_(float(np.float32(1) - np.float32(beta1)) * g)
@@ -596,7 +598,7 @@ class DryOps:
         if half_state:
           m16.copy_(stochastic_round(mm, sdt, step, key, stream=STREAM_STATE0))
           v16.copy_(stochastic_round(vv, sdt, step, key, stream=STREAM_STATE1))
-      elif kind == 5:
+      elif kind == OPT_ROWWISE_ADAM:
         # row-wise Adam: v is one fp32 word per row (state1), the mean over the row's columns
         vr = self.world.tensor(int(t["state1"]) + row * 4, torch.float32, 1, "row state")
         vr.mul_(beta2).add_(float(np.float32(1) - np.float32(beta2)) * ((g * g).sum() / width))
@@ -605,7 +607,7 @@ class DryOps:
         wt -= lr * (mm / bias1) / ((vr / bias2).sqrt() + eps)
         if half_state:
           m16.copy_(stochastic_round(mm, sdt, step, key, stream=STREAM_STATE0))
-      elif kind == 6:
+      elif kind == OPT_FTRL:
         # FTRL-Proximal: n (state0) and z (state1); at lr == 0 nothing moves
         if lr == 0.0:
           continue

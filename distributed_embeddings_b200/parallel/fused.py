@@ -46,11 +46,9 @@ from ..ops._native import DTYPE_CODE, GRAD_ROUTE, INPUT_DESC, TABLE_DESC
 from ..ops.ragged import RaggedIds
 from ..utils import nvtx
 from .comm import CH_BARRIER0, CH_CONSUMED, CH_GRAD, CH_IDS, CH_OUT, CommContext
+from .embedding_optimizers import OPTIMIZERS, state_slots
 from .offload_cache import OffloadCache, split_budget
 
-_OPT_KIND = {"sgd": _native.OPT_SGD, "adagrad": _native.OPT_ADAGRAD,
-             "rowwise_adagrad": _native.OPT_ROWWISE_ADAGRAD, "adam": _native.OPT_ADAM,
-             "rowwise_adam": _native.OPT_ROWWISE_ADAM, "ftrl": _native.OPT_FTRL}
 _COMB = {None: 0, "sum": 0, "mean": 1}
 
 # InputDesc.flags
@@ -853,32 +851,17 @@ class FusedEngine:
     opt = self.de._fused_optimizer
     if opt is None:
       return
-    kind = opt["kind"]
     self.step_t.fill_(float(opt.get("step", 0)))
 
-    sdt = self.state_dtype
-
-    def like(w, value, shape=None, dtype=torch.float32):
-      # (a bf16 initial value is the round-to-nearest of ``value``)
-      t = torch.full(shape or tuple(w.shape), value, dtype=dtype, device=w.device)
+    def alloc(shape, value, dtype, device):
+      t = torch.full(shape, value, dtype=dtype, device=device)
       # state of offloaded tables stays on the host (pinned, read zero-copy by the kernels)
-      return t.pin_memory() if not (w.is_cuda or self.dry) else t
+      return t.pin_memory() if not (t.is_cuda or self.dry) else t
 
-    for m, layer in enumerate(self.mp_layers):
-      w = _weight(layer)
-      if kind == "adagrad":
-        self.opt_state[m] = [like(w, opt["initial_accumulator_value"], dtype=sdt)]
-      elif kind == "rowwise_adagrad":
-        self.opt_state[m] = [like(w, opt["initial_accumulator_value"], (w.shape[0],))]
-      elif kind == "adam":
-        self.opt_state[m] = [like(w, 0.0, dtype=sdt), like(w, 0.0, dtype=sdt)]
-      elif kind == "rowwise_adam":
-        # m element-wise (in the state dtype), v one fp32 word per row
-        self.opt_state[m] = [like(w, 0.0, dtype=sdt), like(w, 0.0, (w.shape[0],))]
-      elif kind == "ftrl":
-        # accumulator n and linear term z, both element-wise in the state dtype
-        self.opt_state[m] = [like(w, opt["initial_accumulator_value"], dtype=sdt),
-                             like(w, 0.0, dtype=sdt)]
+    if OPTIMIZERS[opt["kind"]].slots:
+      for m, layer in enumerate(self.mp_layers):
+        self.opt_state[m] = state_slots(opt["kind"], _weight(layer), self.state_dtype,
+                                        torch.float32, opt["initial_accumulator_value"], alloc)
     self._tables_dirty = True
 
   @property
@@ -1275,23 +1258,23 @@ class FusedEngine:
     if opt is not None:
       if not self._dry_updates:
         self.step_t.add_(1.0)  # device counter: bias corrections stay right under graph replay
-      kind = _OPT_KIND[opt["kind"]]
-      if self._dry_updates and opt["kind"] in ("adam", "rowwise_adam", "ftrl"):
+      entry = OPTIMIZERS[opt["kind"]]
+      if self._dry_updates and entry.moves_on_zero_grad:
         # a zero gradient would still decay Adam's moments, and would set FTRL's weights to the
         # closed form of z
-        kind = _OPT_KIND["sgd"]
+        entry = OPTIMIZERS["sgd"]
       # a dry update has no decay either: weight_decay * w would move the weights and feed the
       # Adagrad accumulators on every warm-up pass
       wd = 0.0 if self._dry_updates else opt["weight_decay"]
-      # FTRL's hyperparameters trail the op's arguments (the other kinds launch without them)
-      ftrl = tuple(opt[k] for k in ("lr_power", "l1", "l2", "l2_shrinkage", "beta")) \
-          if kind == _native.OPT_FTRL else ()
       ops.segment_update(self.mpdesc, self.tdesc, n_mp, B, B, self.recv_width, self.recv_ptr,
-                         keys, items, seg, n_unique, kind, opt["lr"],
+                         keys, items, seg, n_unique, entry.code, opt["lr"],
                          opt["eps"], opt["beta1"], opt["beta2"], 1.0, 1.0, gscale,
                          wd, self.lr_t.data_ptr(), None, None, self.max_width,
                          self.act, self.vec4, self._balanced_scratch(), self.step_t.data_ptr(),
-                         self.tab, DTYPE_CODE[self.state_dtype], *ftrl)
+                         self.tab, DTYPE_CODE[self.state_dtype],
+                         # FTRL's hyperparameters trail the op's arguments (the other kinds
+                         # launch without them)
+                         *(opt[k] for k in entry.hyper))
       if multi:
         ops.sync_only(self._sync(signal=CH_CONSUMED))
       return [None] * n_mp

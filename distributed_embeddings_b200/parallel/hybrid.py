@@ -18,10 +18,11 @@ import torch
 import torch.distributed as dist
 from torch import nn
 
-from ..ops.stochastic_rounding import (HALF_DTYPES, STREAM_STATE0, STREAM_STATE1,
-                                       check_state_dtype, stochastic_round)
+from ..ops.stochastic_rounding import (HALF_DTYPES, STREAM_STATE0, STREAM_STATE1, STREAM_WEIGHT,
+                                       stochastic_round)
 from .comm import CommContext, dist_ready
-from .dist_model_parallel import FTRL_DEFAULTS, _is_mp, broadcast_variables, check_ftrl_args
+from .dist_model_parallel import _is_mp, broadcast_variables
+from .embedding_optimizers import OPTIMIZERS, check_state_dtype, state_slots
 
 
 def _world(group=None) -> int:
@@ -277,133 +278,81 @@ class SparseRowOptimizer:
                initial_accumulator_value: float = 0.1, weight_decay: float = 0.0,
                state_dtype: torch.dtype = torch.float32, **ftrl):
     kind = kind.lower()
-    if kind not in ("sgd", "adagrad", "rowwise_adagrad", "adam", "rowwise_adam", "ftrl"):
+    if kind not in OPTIMIZERS:
       raise ValueError(f"Unsupported optimizer {kind}")
-    unknown = sorted(set(ftrl) - (set(FTRL_DEFAULTS) if kind == "ftrl" else set()))
+    entry = OPTIMIZERS[kind]
+    unknown = sorted(set(ftrl) - set(entry.hyper))
     if unknown:
       raise ValueError(f"unknown fused optimizer argument(s) {unknown} for {kind}")
-    self.ftrl = dict(FTRL_DEFAULTS, initial_accumulator_value=initial_accumulator_value, **ftrl)
-    if kind == "ftrl":
-      check_ftrl_args(self.ftrl)
+    self.ftrl = dict(entry.hyper, initial_accumulator_value=initial_accumulator_value, **ftrl)
+    if entry.check is not None:
+      entry.check(self.ftrl)
     self.state_dtype = check_state_dtype(kind, state_dtype)
     self.params = [p for p in params if p.requires_grad]
     self.kind, self.lr = kind, float(lr)
-    self.eps = (1e-8 if kind in ("adam", "rowwise_adam") else 1e-7) if eps is None else eps
+    self.eps = entry.eps if eps is None else eps
     self.beta1, self.beta2, self.weight_decay = beta1, beta2, weight_decay
     self.step_count = 0
     self.state = []
     for p in self.params:
-      sdt = torch.float32 if p.dtype in HALF_DTYPES else p.dtype  # half tables: fp32 state
+      sdt = torch.promote_types(p.dtype, torch.float32)  # half tables: fp32 state
       esdt = torch.bfloat16 if self.state_dtype == torch.bfloat16 else sdt  # element-wise state
-      if kind == "adagrad":
-        self.state.append([torch.full_like(p, initial_accumulator_value, dtype=esdt)])
-      elif kind == "rowwise_adagrad":
-        self.state.append([torch.full((p.shape[0],), initial_accumulator_value, dtype=sdt,
-                                      device=p.device)])
-      elif kind == "adam":
-        self.state.append([torch.zeros_like(p, dtype=esdt), torch.zeros_like(p, dtype=esdt)])
-      elif kind == "rowwise_adam":
-        self.state.append([torch.zeros_like(p, dtype=esdt),
-                           torch.zeros((p.shape[0],), dtype=sdt, device=p.device)])
-      elif kind == "ftrl":
-        self.state.append([torch.full_like(p, initial_accumulator_value, dtype=esdt),
-                           torch.zeros_like(p, dtype=esdt)])
-      else:
-        self.state.append([])
+      self.state.append(state_slots(kind, p, esdt, sdt, initial_accumulator_value))
 
   def set_lr(self, lr: float):
     self.lr = float(lr)
 
   @torch.no_grad()
   def step(self):
+    """Update the touched rows of every table in ``promote_types(dtype, float32)``, in the
+    kernels' order of operations; store 16-bit weights and bf16 state with stochastic
+    rounding."""
     self.step_count += 1
     for p, st in zip(self.params, self.state):
       g = p.grad
       if g is None:
         continue
+      p.grad = None
       if g.is_sparse:
         g = g.coalesce()
         idx, val = g.indices()[0], g.values().to(p.dtype)
       else:
         idx = torch.arange(p.shape[0], device=p.device)
         val = g.to(p.dtype)
-      if p.dtype in HALF_DTYPES or self.state_dtype != torch.float32:
-        self._step_half(p, st, idx, val.float())
-        p.grad = None
-        continue
+      if self.kind == "ftrl" and self.lr == 0.0:
+        continue  # rows and state keep their bits
+      cdt = torch.promote_types(p.dtype, torch.float32)
+      w, val = p[idx].to(cdt), val.to(cdt)
       if self.weight_decay:
-        val = val + self.weight_decay * p[idx]
-      if self.kind == "sgd":
-        p.index_add_(0, idx, val, alpha=-self.lr)
-      elif self.kind == "adagrad":
-        acc = st[0][idx] + val * val
-        st[0][idx] = acc
-        p.index_add_(0, idx, val / (acc.sqrt() + self.eps), alpha=-self.lr)
-      elif self.kind == "rowwise_adagrad":
-        acc = st[0][idx] + (val * val).mean(dim=1)
-        st[0][idx] = acc
-        p.index_add_(0, idx, val / (acc.sqrt().unsqueeze(1) + self.eps), alpha=-self.lr)
-      elif self.kind == "rowwise_adam":
-        v = self.beta2 * st[1][idx] + (1 - self.beta2) * (val * val).mean(dim=1)
-        m = self.beta1 * st[0][idx] + (1 - self.beta1) * val
-        st[0][idx], st[1][idx] = m, v
-        b1 = 1 - self.beta1**self.step_count
-        b2 = 1 - self.beta2**self.step_count
-        p.index_add_(0, idx, (m / b1) / ((v / b2).sqrt().unsqueeze(1) + self.eps), alpha=-self.lr)
-      elif self.kind == "ftrl":
-        if self.lr != 0.0:
-          p[idx], st[0][idx], st[1][idx] = self._ftrl(p[idx], val, st[0][idx], st[1][idx])
-      else:
-        m = self.beta1 * st[0][idx] + (1 - self.beta1) * val
-        v = self.beta2 * st[1][idx] + (1 - self.beta2) * val * val
-        st[0][idx], st[1][idx] = m, v
-        b1 = 1 - self.beta1**self.step_count
-        b2 = 1 - self.beta2**self.step_count
-        p.index_add_(0, idx, (m / b1) / ((v / b2).sqrt() + self.eps), alpha=-self.lr)
-      p.grad = None
+        val = val + self.weight_decay * w
+      w, new_state = self._update(w, val, [s[idx].to(cdt) for s in st])
+      self._store(p, idx, w, STREAM_WEIGHT)
+      for s, x, stream in zip(st, new_state, (STREAM_STATE0, STREAM_STATE1)):
+        self._store(s, idx, x, stream)
 
-  def _step_half(self, p, st, idx, val):
-    """fp32 update of the rows ``idx`` of a bf16 / fp16 table or of a table with bf16 state;
-    16-bit values are stochastically rounded back."""
-    w = p[idx].float()
-    if self.weight_decay:
-      val = val + self.weight_decay * w
+  def _update(self, w, g, state):
+    """One step of the optimizer on rows ``w`` with decayed gradient ``g`` and the rows' state
+    slots; returns the new weights and state."""
+    b1 = 1 - self.beta1**self.step_count
+    b2 = 1 - self.beta2**self.step_count
     if self.kind == "sgd":
-      w = w - self.lr * val
-    elif self.kind == "adagrad":
-      acc = st[0][idx].float() + val * val
-      self._store_state(st[0], idx, acc, STREAM_STATE0)
-      w = w - self.lr * val / (acc.sqrt() + self.eps)
-    elif self.kind == "rowwise_adagrad":
-      acc = st[0][idx] + (val * val).mean(dim=1)
-      st[0][idx] = acc
-      w = w - self.lr * val / (acc.sqrt().unsqueeze(1) + self.eps)
-    elif self.kind == "rowwise_adam":
-      v = self.beta2 * st[1][idx] + (1 - self.beta2) * (val * val).mean(dim=1)
-      m = self.beta1 * st[0][idx].float() + (1 - self.beta1) * val
-      st[1][idx] = v
-      self._store_state(st[0], idx, m, STREAM_STATE0)
-      b1 = 1 - self.beta1**self.step_count
-      b2 = 1 - self.beta2**self.step_count
-      w = w - self.lr * (m / b1) / ((v / b2).sqrt().unsqueeze(1) + self.eps)
-    elif self.kind == "ftrl":
-      if self.lr == 0.0:
-        return  # rows and state keep their bits
-      w, n, z = self._ftrl(w, val, st[0][idx].float(), st[1][idx].float())
-      self._store_state(st[0], idx, n, STREAM_STATE0)
-      self._store_state(st[1], idx, z, STREAM_STATE1)
-    else:
-      m = self.beta1 * st[0][idx].float() + (1 - self.beta1) * val
-      v = self.beta2 * st[1][idx].float() + (1 - self.beta2) * val * val
-      self._store_state(st[0], idx, m, STREAM_STATE0)
-      self._store_state(st[1], idx, v, STREAM_STATE1)
-      b1 = 1 - self.beta1**self.step_count
-      b2 = 1 - self.beta2**self.step_count
-      w = w - self.lr * (m / b1) / ((v / b2).sqrt() + self.eps)
-    if p.dtype in HALF_DTYPES:
-      p[idx] = stochastic_round(w, p.dtype, self.step_count, idx).to(p.device)
-    else:
-      p[idx] = w
+      return w - self.lr * g, []
+    if self.kind == "adagrad":
+      acc = state[0] + g * g
+      return w - self.lr * g / (acc.sqrt() + self.eps), [acc]
+    if self.kind == "rowwise_adagrad":
+      acc = state[0] + (g * g).mean(dim=1)
+      return w - self.lr * g / (acc.sqrt().unsqueeze(1) + self.eps), [acc]
+    if self.kind == "adam":
+      m = self.beta1 * state[0] + (1 - self.beta1) * g
+      v = self.beta2 * state[1] + (1 - self.beta2) * g * g
+      return w - self.lr * (m / b1) / ((v / b2).sqrt() + self.eps), [m, v]
+    if self.kind == "rowwise_adam":
+      m = self.beta1 * state[0] + (1 - self.beta1) * g
+      v = self.beta2 * state[1] + (1 - self.beta2) * (g * g).mean(dim=1)
+      return w - self.lr * (m / b1) / ((v / b2).sqrt().unsqueeze(1) + self.eps), [m, v]
+    w, n, z = self._ftrl(w, g, state[0], state[1])
+    return w, [n, z]
 
   def _ftrl(self, w, g, n, z):
     """FTRL-Proximal on rows ``w`` with decayed gradient ``g``, accumulator ``n`` and linear term
@@ -417,9 +366,10 @@ class SparseRowOptimizer:
     w = torch.where(z.abs() > c["l1"], (torch.sign(z) * c["l1"] - z) / q, torch.zeros_like(z))
     return w, n_new, z
 
-  def _store_state(self, s, idx, x, stream):
-    """Store fp32 state rows ``x`` at ``idx``: as is, or stochastically rounded into bf16."""
-    if s.dtype in HALF_DTYPES:
-      s[idx] = stochastic_round(x, s.dtype, self.step_count, idx, stream=stream).to(s.device)
+  def _store(self, dst, idx, x, stream):
+    """Store rows ``x`` at ``idx`` of a table or state slot: as is, or stochastically rounded
+    into a 16-bit ``dst``."""
+    if dst.dtype in HALF_DTYPES:
+      dst[idx] = stochastic_round(x, dst.dtype, self.step_count, idx, stream=stream).to(dst.device)
     else:
-      s[idx] = x
+      dst[idx] = x

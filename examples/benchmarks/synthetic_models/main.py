@@ -27,6 +27,7 @@ from distributed_embeddings_b200.models.configs import scaled, summary, syntheti
 from distributed_embeddings_b200.models.synthetic import (InputGenerator, SyntheticModel,
                                                            SyntheticModelNative)
 from distributed_embeddings_b200.models.trainer import HybridTrainer
+from distributed_embeddings_b200.parallel.embedding_optimizers import NAMES as EMBEDDING_OPTIMIZERS
 
 
 def main():
@@ -37,8 +38,7 @@ def main():
   p.add_argument("--num_steps", type=int, default=100)
   p.add_argument("--dp_input", action="store_true")
   p.add_argument("--model", default="tiny", choices=sorted(synthetic_models_v3))
-  p.add_argument("--optimizer", default="sgd", choices=["sgd", "adagrad", "rowwise_adagrad", "adam",
-                                                     "rowwise_adam", "ftrl"])
+  p.add_argument("--optimizer", default="sgd", choices=EMBEDDING_OPTIMIZERS)
   p.add_argument("--dense_optimizer", default="sgd", choices=["sgd", "adagrad", "adam"],
                  help="optimizer of the MLP (--embedding_api de); the reference uses --optimizer's")
   p.add_argument("--column_slice_threshold", type=int, default=None)

@@ -25,6 +25,7 @@ import torch.distributed as dist
 import distributed_embeddings_b200 as de
 from distributed_embeddings_b200.models.dlrm import DLRM, MLPERF_DCNV2_MULTI_HOT_SIZES
 from distributed_embeddings_b200.models.trainer import HybridTrainer
+from distributed_embeddings_b200.parallel.embedding_optimizers import NAMES as EMBEDDING_OPTIMIZERS
 from distributed_embeddings_b200.utils.criteo import DummyDataset, RawBinaryDataset
 from distributed_embeddings_b200.utils.lr_schedule import LearningRateScheduler
 from distributed_embeddings_b200.utils.metrics import binary_auc
@@ -72,7 +73,7 @@ def parse():
                  help="storage of the model-parallel embedding tables (bf16 / fp16: half the "
                       "memory, stochastically rounded updates)")
   p.add_argument("--embedding_optimizer", default="sgd",
-                 choices=["sgd", "adagrad", "rowwise_adagrad", "adam", "rowwise_adam", "ftrl"],
+                 choices=EMBEDDING_OPTIMIZERS,
                  help="fused optimizer of the model-parallel tables")
   p.add_argument("--optimizer_state_dtype", default="fp32", choices=["fp32", "bf16"],
                  help="storage of the Adagrad / Adam / FTRL state (row-wise Adam: its m) of the "
