@@ -476,11 +476,15 @@ Tensor embedding_lookup_fwd(const Tensor& param, const Tensor& values,
   int64_t lanes_per_row = 1;
   while (lanes_per_row < (width + 3) / 4 && lanes_per_row < 32) lanes_per_row *= 2;
   const int64_t ts = std::max<int64_t>(32 / lanes_per_row, std::min<int64_t>(32, 64 / avg_hot));
+  // vector loads need the table's base on their own width: a contiguous view at an odd element
+  // offset takes the scalar path
+  const uintptr_t base = reinterpret_cast<uintptr_t>(param.data_ptr());
+  const bool vec4 = width % 4 == 0 && base % (4 * param.element_size()) == 0;
   de::launch_lookup_fwd(reinterpret_cast<const de::InputDesc*>(dd.data_ptr()), 1, batch, batch,
                         batch, width, src, dst, 0, values.scalar_type() == at::kLong,
-                        out_bf16 ? 1 : tdt, width % 4 == 0, sm_count(), cur_stream(),
-                        de::no_sync(), static_cast<int>(std::max<int64_t>(1, ts)), tdt,
-                        width % 8 == 0 && reinterpret_cast<uintptr_t>(param.data_ptr()) % 16 == 0);
+                        out_bf16 ? 1 : tdt, vec4, sm_count(), cur_stream(), de::no_sync(),
+                        static_cast<int>(std::max<int64_t>(1, ts)), tdt,
+                        width % 8 == 0 && base % 16 == 0);
   check_launch();
   return out;
 }
@@ -505,8 +509,10 @@ void embedding_scatter_add(Tensor dst, const Tensor& values, const c10::optional
   gp.p[0] = grad.data_ptr();
   const int gdt = dtype_code(grad.scalar_type());
   const int64_t gstride = grad.stride(0);
+  // 4-wide gradient loads and 4-wide reductions into dst: both bases on the 16-byte grid
   const bool vec4 = (width % 4 == 0) && (gstride % 4 == 0) &&
-                    (reinterpret_cast<uintptr_t>(grad.data_ptr()) % 16 == 0);
+                    (reinterpret_cast<uintptr_t>(grad.data_ptr()) % 16 == 0) &&
+                    (reinterpret_cast<uintptr_t>(dst.data_ptr()) % 16 == 0);
   de::launch_scatter_add_bwd(reinterpret_cast<const de::InputDesc*>(dd.data_ptr()), 1, batch,
                              batch, batch, gstride, src, gp, 0, static_cast<float>(scale), nullptr,
                              values.scalar_type() == at::kLong, gdt, vec4, sm_count(),

@@ -40,8 +40,9 @@ def _sample_ids_cpu(values, offsets, hotness, batch):
   return sample, counts
 
 
-def _lookup_fwd_cpu(param, values, offsets, hotness, batch, combiner):
-  """Pooled in fp32 whatever the table dtype; the result has the table's dtype."""
+def _lookup_fwd_cpu(param, values, offsets, hotness, batch, combiner, out_dtype=None):
+  """Pooled in fp32 whatever the table dtype and rounded once to ``out_dtype`` (default: the
+  table's dtype)."""
   rows, width = param.shape
   flat = values.reshape(-1).to(torch.int64)
   sample, counts = _sample_ids_cpu(flat, offsets, hotness, batch)
@@ -52,7 +53,7 @@ def _lookup_fwd_cpu(param, values, offsets, hotness, batch, combiner):
   out.index_add_(0, sample, gathered)
   if combiner == 1:
     out = out / counts.clamp(min=1).unsqueeze(1).to(acc)
-  return out.to(param.dtype)
+  return out.to(param.dtype if out_dtype is None else out_dtype)
 
 
 def _lookup_grad_cpu(values, offsets, hotness, batch, combiner, grad, num_rows):
@@ -74,8 +75,9 @@ def lookup_forward(param, values, offsets, hotness, batch, combiner, out_bf16=Fa
   if param.is_cuda:
     return _native.require().embedding_lookup_fwd(param, values.contiguous(), offsets, hotness,
                                                   batch, combiner, out_bf16)
-  out = _lookup_fwd_cpu(param, values, offsets, hotness, batch, combiner)
-  return out.to(torch.bfloat16) if out_bf16 else out
+  # fp32 pooling rounded once: an fp16 table must not pass through fp16 on its way to bf16
+  return _lookup_fwd_cpu(param, values, offsets, hotness, batch, combiner,
+                         torch.bfloat16 if out_bf16 else None)
 
 
 def lookup_grad_sparse(values, offsets, hotness, batch, combiner, grad,
