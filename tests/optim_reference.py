@@ -233,12 +233,12 @@ def worst_table_ratio(out, bound, got):
   return worst
 
 
-def half_within(got16, ref, bound, dtype, step, keys, stream=0):
+def half_within(got16, ref, bound, dtype, step, keys, stream=0, mask=False):
   """16-bit result check: the kernel rounds its fp32 value x, known to lie in
   [ref - bound, ref + bound], stochastically with the bits of ``ops/stochastic_rounding.py``.  That
   rule is monotone in x for fixed bits, so the result must lie between the rounding of the two
   ends (rounded outward to fp32): exactly the reference's rounding wherever the interval holds no
-  16-bit value.  Returns the number of elements outside."""
+  16-bit value.  Returns the number of elements outside (``mask``: whether each one is inside)."""
   from distributed_embeddings_b200.ops.stochastic_rounding import stochastic_round
   lo = (ref - bound).numpy()
   hi = (ref + bound).numpy()
@@ -250,4 +250,5 @@ def half_within(got16, ref, bound, dtype, step, keys, stream=0):
   r_lo = stochastic_round(torch.from_numpy(lo32), dtype, step, keys, stream=stream).float()
   r_hi = stochastic_round(torch.from_numpy(hi32), dtype, step, keys, stream=stream).float()
   g = torch.as_tensor(got16).float()
-  return int(((g < r_lo) | (g > r_hi)).sum())
+  outside = (g < r_lo) | (g > r_hi)
+  return ~outside.numpy() if mask else int(outside.sum())

@@ -30,6 +30,7 @@ import torch
 import distributed_embeddings_b200 as de
 from distributed_embeddings_b200.ops.ragged import RaggedIds
 from distributed_embeddings_b200.parallel import dry_run
+from distributed_embeddings_b200.parallel.embedding_optimizers import OPTIMIZERS
 from distributed_embeddings_b200.parallel.hybrid import SparseRowOptimizer
 from optim_reference import (TABLE_DEFECTS, f32, half_within,  # pylint: disable=wrong-import-order
                              table_step, worst_table_ratio)
@@ -65,8 +66,9 @@ def _draw(case, step):
   for i, t in enumerate(case["imap"]):
     h = case["hots"][i]
     if h == "ragged":
-      lens = torch.randint(0, 9, (B,), generator=gen).tolist()
-      lens[:3] = [0, 1, 8]
+      most = case.get("ragged_max", 8)
+      lens = torch.randint(0, most + 1, (B,), generator=gen).tolist()
+      lens[:3] = [0, 1, most]
       lo_id = ZERO_ROW + 1 if case.get("edges") and t == case["imap"][0] else 0
       ids.append([torch.randint(lo_id, rows[t], (n,), generator=gen).tolist() for n in lens])
       continue
@@ -146,56 +148,127 @@ def _initial_state(kind, rows, width, sdt=torch.float32):
   return []
 
 
-def _state_of(demb, kind, t, rows, width, sdt):
-  st = demb.get_optimizer_state()
-  if st["tables"] is None:
-    return _initial_state(kind, rows, width, sdt), st["step"]
-  slots = [np.asarray(a, dtype=np.float32) for a in st["tables"][t]]
-  if kind == "rowwise_adagrad":
-    slots = [slots[0][:, 0]]
-  return slots, st["step"]
-
-
 # ------------------------------------------------------------------ per-step check
-def _check_step(case, kind, before, state, after, state_after, occ, t, step, scale=1.0,
-                slack=1.0, weights_only=False):
-  """Compare one table after one step with the float64 step from its state before.  ``slack``
-  widens the bounds for implementations without fma (every product rounded on its own);
-  ``weights_only`` leaves the state slots unchecked."""
-  rows, vals = occ
-  cfg = {"eps": 1e-8 if kind == "adam" else 1e-7, "beta1": 0.9, "beta2": 0.999,
-         "weight_decay": case.get("wd", 0.0)}
-  out, bound, touched = table_step(kind, before, state, rows, vals, scale, case["lrs"][step],
-                                   step + 1, cfg, atomic=_expected_route(case, kind) == "atomic")
-  bound = {k: slack * b for k, b in bound.items()}
-  if weights_only:
-    out, bound = {"p": out["p"]}, {"p": bound["p"]}
+class Spec:
+  """What the driver needs to know about one optimizer kind: its keyword arguments, its state at
+  the start, and the float64 model of one step on one column range of a table (a column slice
+  keeps its own row words).  The row-wise Adam and FTRL tests pass their own."""
+
+  def __init__(self, kind):
+    self.kind = kind
+    self.slots = OPTIMIZERS[kind].slots
+
+  def opt(self, case):  # pylint: disable=unused-argument
+    return {}
+
+  def initial(self, rows, width, sdt):
+    return _initial_state(self.kind, rows, width, sdt)
+
+  def model(self, case, before, state, occ, step, scale):
+    cfg = {"eps": OPTIMIZERS[self.kind].eps, "beta1": 0.9, "beta2": 0.999,
+           "weight_decay": case.get("wd", 0.0)}
+    return table_step(self.kind, before, state, occ[0], occ[1], scale, case["lrs"][step],
+                      step + 1, cfg, atomic=_expected_route(case, self.kind) == "atomic")
+
+  def finish(self, case, zeros):
+    """Checks over the whole run; ``zeros``: weights that a step with lr > 0 touched and left
+    exactly zero."""
+
+
+SPECS = {k: Spec(k) for k in KINDS}
+_SLOT_NAMES = {"p": "weight", "s0": "state slot 0", "s1": "state slot 1"}
+
+
+def _slices(demb, t, width):
+  """Column ranges of table ``t`` that keep their own row words (the whole row unless sliced)."""
+  st = demb.strategy
+  if t not in st.table_groups[1]:
+    return [(0, width)]
+  gt = st.table_groups[1].index(t)
+  return sorted({(s.col_start, s.col_end) for shards in st.shards for s in shards
+                 if s.table == gt})
+
+
+def _pieces(des, t, width):
+  """Where table ``t`` lives: (rank, local table, first local row, first global row, rows, first
+  column, end column) of every shard."""
+  st = des[0].strategy
+  assert t not in st.table_groups[0], "replicated tables are not updated by the engine"
+  if t in st.table_groups[1]:
+    gt = st.table_groups[1].index(t)
+    return [(r, s.local_table, s.row_offset, 0, s.rows, s.col_start, s.col_end)
+            for r, shards in enumerate(st.shards) for s in shards if s.table == gt]
+  gt = st.table_groups[2].index(t)
+  return [(r, len(des[r].local_embedding_layers) + gt, 0, lo, hi - lo, 0, width)
+          for r, (lo, hi) in enumerate(st.row_ranges[gt]) if hi > lo]
+
+
+def _read_shards(des, t, width):
+  """Every shard of table ``t`` as the engine of its rank holds it: global rows, columns, the
+  16-bit rounding key of each row (``key_base`` of the local table plus the row inside it) and
+  the state slots, read from ``opt_state`` at the shard's rows (a per-row slot: the shard's own
+  words, not the exported width-weighted mean)."""
+  out = []
+  for r, m, l0, g0, n, c0, c1 in _pieces(des, t, width):
+    eng = des[r]._engine
+    st = eng.opt_state.get(m, [])
+    slots = [np.asarray(x[l0:l0 + n].float().cpu().numpy(), dtype=np.float32) for x in st]
+    out.append({"rank": r, "table": m, "rows": np.arange(g0, g0 + n), "cols": (c0, c1),
+                "keys": int(eng.tdesc_np["key_base"][m]) + l0 + np.arange(n), "slots": slots})
+  return out
+
+
+def _read_global(demb, kind, t, rows, width, case):
+  """World 1 on the GPU (the table may sit in the HBM row cache): the exported state, rows keyed
+  from ``case['key_base']``."""
+  st = demb.get_optimizer_state()
+  slots = []
+  if st["tables"] is not None:
+    slots = [np.asarray(a, dtype=np.float32)[:, 0] if s.per_row else np.asarray(a, np.float32)
+             for a, s in zip(st["tables"][t], OPTIMIZERS[kind].slots)]
+  return [{"rank": 0, "table": t, "rows": np.arange(rows), "cols": (0, width),
+           "keys": np.arange(rows) + case.get("key_base", 0), "slots": slots}]
+
+
+def _check_shard(case, spec, t, step, sh, out, bound, touched, after_t, slack):
+  """One shard of table ``t`` after ``step`` against the float64 model of its column range:
+  untouched rows bit-identical, touched fp32 values within ``slack`` times the bounds, touched
+  16-bit values between the roundings of the bound's ends at the shard's keys.  A failure names
+  the table, the slot, the row and the column."""
+  rows, (c0, c1) = sh["rows"], sh["cols"]
   tdt = case.get("table_dtype", torch.float32)
   sdt = case.get("state_dtype", torch.float32)
-  got = {"p": after}
-  for k, s in zip(("s0", "s1"), state_after):
-    got[k] = s
-  if tdt == torch.float32 and sdt == torch.float32:
-    r = worst_table_ratio(out, bound, got)
-    assert r <= 1.0, f"table {t} step {step}: worst error / bound {r}"
-    return touched
-  idx = np.nonzero(touched)[0]
-  keys = idx + case.get("key_base", 0)
-  for k, stream in (("p", 0), ("s0", 1), ("s1", 2)):
+  got = {"p": after_t[rows, c0:c1]}
+  dts = {"p": tdt}
+  for j, (x, s) in enumerate(zip(sh["slots"], spec.slots)):
+    got[f"s{j}"] = x
+    dts[f"s{j}"] = torch.float32 if s.per_row else sdt
+  hit = touched[rows]
+  for k, g in got.items():
     if k not in out:
       continue
-    g = torch.as_tensor(np.asarray(got[k], dtype=np.float64))
-    dt = tdt if k == "p" else sdt
-    unt = ~torch.as_tensor(touched)
-    assert torch.equal(g[unt], out[k][unt]), f"untouched rows of {k} changed"
-    if dt == torch.float32:
-      part = {k: out[k][idx]}
-      r = worst_table_ratio(part, {k: bound[k][idx]}, {k: g[idx].numpy()})
-      assert r <= 1.0, f"{k}: worst error / bound {r}"
-    else:
-      bad = half_within(g[idx], out[k][idx], bound[k][idx], dt, step + 1, keys, stream)
-      assert bad == 0, f"{k}: {bad} 16-bit values outside the rounding of the bound"
-  return touched
+    g = torch.as_tensor(np.asarray(g, dtype=np.float64))
+    o, b = out[k][rows], slack * bound[k][rows]
+    mask = torch.as_tensor(hit).view(-1, *([1] * (g.dim() - 1))).expand_as(g)
+    err = (g - o).abs()
+    bad = ~torch.isfinite(g) | (~mask & (err != 0))
+    if dts[k] == torch.float32:
+      bad |= mask & (err > b)
+    elif hit.any():
+      idx = np.nonzero(hit)[0]
+      inside = half_within(g[idx], o[idx], b[idx], dts[k], step + 1, sh["keys"][idx],
+                           {"p": 0, "s0": 1, "s1": 2}[k], mask=True)
+      bad[torch.as_tensor(idx)] |= torch.as_tensor(~inside)
+    if bad.any():
+      e = [int(x) for x in torch.nonzero(bad)[0]]
+      i = e[0]
+      col = f" column {c0 + e[1]}" if len(e) > 1 else ""
+      raise AssertionError(
+          f"table {t} {_SLOT_NAMES[k]} row {int(rows[i])}{col} after step {step} (rank "
+          f"{sh['rank']}, local table {sh['table']}, key {int(sh['keys'][i])}, "
+          f"{'touched' if hit[i] else 'untouched'}): got {float(g[tuple(e)])!r}, float64 model "
+          f"{float(o[tuple(e)])!r} +- {float(b[tuple(e)])!r} ({dts[k]}); "
+          f"{int(bad.sum())} values outside")
 
 
 class _Counting:
@@ -235,10 +308,23 @@ def _expected_route(case, kind):
 
 
 # ------------------------------------------------------------------ driver (GPU and interpreter)
-def _run(case, kind, world=1, dev=None):
-  """Run ``case`` for ``len(case['lrs'])`` steps and check every step."""
+def _run(case, kind, world=1, dev=None, plan=None, route=None, world_cls=dry_run.DryWorld,
+         slack=None, spec=None):
+  """Run ``case`` for ``len(case['lrs'])`` steps and check every step: on one GPU rank (``dev``)
+  or through the plan interpreter on ``world`` ranks, whose ops ``world_cls`` may replay on the
+  kernels.  ``plan``: extra DistributedEmbedding arguments (slicing); ``route``: the update route
+  every launch must take ("any": one of the sorted routes); ``slack``: factor on the bounds
+  (default 3 for the interpreter, which computes in torch fp32 ops without fma, 1 on the GPU);
+  ``spec``: the optimizer's :class:`Spec`.
+
+  The state is read after every step from the engine: on the GPU through
+  ``get_optimizer_state``, in the interpreter per shard from ``opt_state`` (the rows of a column
+  slice keep their own row words), so every slot is checked at every step and world size, with
+  16-bit values rounded at the keys of the rank that owns them."""
+  spec = spec or SPECS[kind]
   embs = [{"input_dim": r, "output_dim": w, "combiner": c} for r, w, c in case["tables"]]
   kw = dict(input_table_map=list(case["imap"]), strategy="basic")
+  kw.update(plan or {})
   if case.get("table_dtype", torch.float32) != torch.float32:
     kw["table_dtype"] = case["table_dtype"]
   if case.get("compute_dtype"):
@@ -246,15 +332,18 @@ def _run(case, kind, world=1, dev=None):
   if case.get("cache"):
     small = case["tables"][0]
     kw.update(gpu_embedding_size=small[0] * small[1] + 1, offload_cache_size=case["cache"])
-  opt = {"weight_decay": case.get("wd", 0.0)}
+  opt = dict(spec.opt(case), weight_decay=case.get("wd", 0.0))
   if case.get("deterministic"):
     opt["deterministic"] = True
-  if case.get("state_dtype", torch.float32) != torch.float32:
-    opt["state_dtype"] = case["state_dtype"]
+  sdt = case.get("state_dtype", torch.float32)
+  if sdt != torch.float32:
+    opt["state_dtype"] = sdt
   cdt = case.get("compute_dtype", torch.float32)
+  if slack is None:
+    slack = 3.0 if dev is None else 1.0
   torch.manual_seed(case.get("seed", 0))
   if dev is None:
-    sim, des = dry_run.build_engines(embs, world, dp_input=True, **kw)
+    sim, des = dry_run.build_engines(embs, world, world_cls, dp_input=True, **kw)
   else:
     sim, des = None, [de.DistributedEmbedding(embs, device=dev, backend="fused", world_size=1,
                                               rank=0, **kw)]
@@ -263,22 +352,23 @@ def _run(case, kind, world=1, dev=None):
   for d in des:
     d.set_weights(tables)
     d.set_optimizer(kind, lr=case["lrs"][0], **opt)
+    assert d._fused_optimizer["eps"] == OPTIMIZERS[kind].eps
     if any(h == "ragged" for h in case["hots"]):
-      d.ragged_capacity = 8
+      d.ragged_capacity = case.get("ragged_max", 8)
   demb = des[0]
-  routes = []
+  slices = [_slices(demb, t, w) if dev is None else [(0, w)]
+            for t, (_, w, _) in enumerate(case["tables"])]
+  states = [{(c0, c1): spec.initial(r, c1 - c0, sdt) for c0, c1 in slices[t]}
+            for t, (r, _, _) in enumerate(case["tables"])]
+  routes, zeros = set(), 0
   for step, lr in enumerate(case["lrs"]):
     if step and lr != case["lrs"][step - 1]:
       for d in des:
         d.set_learning_rate(lr)
     ids, grad = _draw(case, step)
     grad = grad.to(cdt)  # the values the kernels read
-    B = case["batch"]
-    lb = B // world
-    sdt = case.get("state_dtype", torch.float32)
+    lb = case["batch"] // world
     before = _weights(des, world)
-    states = [_state_of(demb, kind, t, r, w, sdt)[0] if world == 1 else
-              _initial_state(kind, r, w, sdt) for t, (r, w, _) in enumerate(case["tables"])]
 
     def rank_fn(r):
       d = des[r]
@@ -290,29 +380,38 @@ def _run(case, kind, world=1, dev=None):
       out.backward(grad[r * lb:(r + 1) * lb].to(out.device))
       return eng.ops.routes
     if dev is None:
-      got_routes = dry_run.run_ranks(sim, rank_fn)[0]
+      for got in dry_run.run_ranks(sim, rank_fn):
+        routes |= set(got)
     else:
-      got_routes = rank_fn(0)
+      routes |= set(rank_fn(0))
       torch.cuda.synchronize()
-    routes = list(got_routes)
     if case.get("edges"):
       _check_edge_layout(case, ids, des[0]._engine)
     after = _weights(des, world)
-    st_after = demb.get_optimizer_state() if world == 1 else None
-    if world == 1 and kind == "adam":
-      assert st_after["step"] == step + 1
+    if kind in ("adam", "rowwise_adam"):  # the step of the bias corrections, on every rank
+      assert [d._engine.step_count() for d in des] == [step + 1] * len(des)
     for t, (r, w, _) in enumerate(case["tables"]):
-      occ = _occurrences(case, ids, grad.float(), t)
-      sa = _state_of(demb, kind, t, r, w, sdt)[0] if world == 1 else []
-      # the state is checked at world 1, the weights at every size (from the initial state: the
-      # multi-rank cases take one step); the interpreter computes in torch fp32 ops without fma:
-      # three times the kernel's bounds
-      assert world == 1 or len(case["lrs"]) == 1
-      _check_step(case, kind, before[t], states[t], after[t], sa, occ, t, step, 1.0 / world,
-                  slack=3.0 if dev is None else 1.0, weights_only=world > 1)
-  want = _expected_route(case, kind)
-  assert routes and set(routes) == {want if want != "atomic" else "scatter_add_bwd"}, \
-      (routes, want)
+      rows, vals = _occurrences(case, ids, grad.float(), t)
+      shards = _read_shards(des, t, w) if dev is None else _read_global(demb, kind, t, r, w, case)
+      touched = None
+      for c0, c1 in slices[t]:
+        o, b, touched = spec.model(case, before[t][:, c0:c1], states[t][(c0, c1)],
+                                   (rows, vals[:, c0:c1]), step, 1.0 / world)
+        new = [x.copy() for x in states[t][(c0, c1)]]
+        for sh in shards:
+          if sh["cols"] != (c0, c1):
+            continue
+          _check_shard(case, spec, t, step, sh, o, b, touched, after[t], slack)
+          for k, x in enumerate(sh["slots"]):
+            new[k][sh["rows"]] = x
+        states[t][(c0, c1)] = new
+      zeros += int((after[t][touched] == 0.0).sum()) if lr > 0 else 0
+  spec.finish(case, zeros)
+  want = route or _expected_route(case, kind)
+  if want == "any":
+    assert routes and routes <= {"balanced", "per_row_vec4", "per_row_vec1"}, routes
+  else:
+    assert routes == {want if want != "atomic" else "scatter_add_bwd"}, (routes, want)
   return des
 
 

@@ -27,6 +27,24 @@ can be separate allocations on the same device.
 * After every op the mirrors are reset from the host buffers, so a failure names the first op,
   rank, buffer and element that diverged.
 
+Kernel-authoritative updates (``MirrorWorld(authoritative=True)``, ``test_update_conformance.py``):
+the fp32 math of row-wise Adam and FTRL (``powf``, ``(P(n') - P(n)) / lr``, the ``l1``
+threshold) may differ from the interpreter's torch ops by far more than a few ulps, so no ulp
+tolerance can be both safe and tight.  There, a ``segment_update`` with an optimizer still runs
+the interpreter first (the bounds-checked oracle for addressing), then the kernel, and:
+
+* in the weight and state buffers of the op's tables, every row whose key is not among the op's
+  ``n_unique`` sorted keys must be bit-identical to the host, and the touched rows are copied from
+  the mirrors into the host buffers, so later ops, later steps and the test's float64 model all
+  see the kernel's numbers;
+* every other buffer is compared as above, the balanced route's ``scratch`` included (it must
+  be all zero again after the op);
+* zero weights are then stored as +0.0: the kernels keep the sign of a -0.0 weight through a
+  one-id pool, the interpreter's sum does not.
+
+With at most two ids per sample, every pooled sum has at most two terms and is exact in any
+order, so the other ops stay bit-exact on the non-dyadic values the updates produce.
+
 A CPU self-check runs the same harness with a second ``DryWorld`` as the "device" and the
 interpreter as the "kernels": it must reproduce the interpreter byte for byte.
 """
@@ -43,6 +61,7 @@ import torch
 from distributed_embeddings_b200.ops import _native
 from distributed_embeddings_b200.ops._native import GRAD_ROUTE, INPUT_DESC, TABLE_DESC
 from distributed_embeddings_b200.parallel import dry_run
+from distributed_embeddings_b200.parallel.embedding_optimizers import BY_CODE
 from test_dry_run import run_inplace_plan, run_plan  # pylint: disable=wrong-import-order
 
 GUARD = 256          # guard bytes behind every mirror
@@ -131,10 +150,11 @@ def _ordered16(raw: torch.Tensor) -> np.ndarray:
 class MirrorWorld(dry_run.DryWorld):
   """A ``DryWorld`` whose engines replay every op on device mirrors (see the module doc)."""
 
-  def __init__(self, world_size, device, inexact=False):
+  def __init__(self, world_size, device, inexact=False, authoritative=False):
     super().__init__(world_size)
     self.dev = device
     self.inexact = inexact
+    self.authoritative = authoritative
     self.token = threading.Lock()
     self._holder = None
     self.mirrors = {}  # start of a registered host storage -> its mirror (+ padding + guard)
@@ -254,9 +274,10 @@ class MirrorWorld(dry_run.DryWorld):
           return f"rank {ops.rank} {name}", t.dtype
     return f"buffer at {start:#x}", torch.uint8
 
-  def compare(self, what, tol=None):
+  def compare(self, what, tol=None, skip=()):
     """Every mirror == its host buffer, every guard intact.  ``tol``: ulps allowed in float
-    buffers (fp32; 16-bit buffers: one ulp of their format)."""
+    buffers (fp32; 16-bit buffers: one ulp of their format); ``skip``: starts of storages whose
+    contents are not compared (their guards are)."""
     self.dev.synchronize()
     for start, end in self._storages():
       n = end - start
@@ -268,7 +289,7 @@ class MirrorWorld(dry_run.DryWorld):
         k = int(torch.nonzero(got[n:] != GUARD_BYTE)[0])
         raise AssertionError(f"{what}: store behind the end of {name} ({n} bytes): guard byte "
                              f"{k} is {int(got[n + k]):#x}")
-      if torch.equal(got[:n], want):
+      if start in skip or torch.equal(got[:n], want):
         continue
       name, dtype = self.describe(start)
       esz = torch.empty((), dtype=dtype).element_size()
@@ -296,6 +317,10 @@ class MirrorWorld(dry_run.DryWorld):
                            f"{b.tolist()}")
 
 
+def _native_dtype(code):
+  return {0: "fp32", 1: "bf16", 2: "fp16"}[int(code)]
+
+
 def _tag(name, a):
   """Kernel path of one op call (for the census)."""
   if name == "lookup_fwd":
@@ -311,13 +336,20 @@ def _tag(name, a):
             (", vec8" if a["vec8"] else "")]
   if name == "segment_update":
     if a["kind"] == _native.OPT_EMIT:
-      tags = ["segment_update, emit"]
-    elif a["scratch"] is not None and a["vec4"] and a["max_width"] <= 128:
-      tags = ["segment_update, balanced"]
+      return ["segment_update, emit"]
+    if a["scratch"] is not None and a["vec4"] and a["max_width"] <= 128:
+      route = "balanced"
     else:
-      tags = ["segment_update, per-row"]
+      route = "per-row " + ("vec4" if a["vec4"] else "vec1")
+    kind = BY_CODE[a["kind"]]
+    half_state = bool(a["state_dtype"]) and kind.elementwise_state
+    tdt = _native_dtype(a["table_dtype"])
+    tags = ["segment_update, " + route.split(" ")[0], f"segment_update, {route}, {kind.name}",
+            f"segment_update, {tdt} table, {'bf16' if half_state else 'fp32'} state"]
     if a["table_dtype"]:
-      tags.append("segment_update, 16-bit table")
+      tags += ["segment_update, 16-bit table", f"segment_update, {tdt} table, {kind.name}"]
+    if half_state:
+      tags.append(f"segment_update, bf16 state, {kind.name}")
     return tags
   return [name]
 
@@ -364,7 +396,11 @@ class MirrorOps(dry_run.DryOps):
       tol = OPT_ULPS
     if w.inexact and name in ("scatter_add_bwd", "segment_update"):
       tol = INEXACT_ULPS
-    w.compare(what, tol)
+    skip = set()
+    adopt = w.authoritative and name == "segment_update" and a["kind"] != _native.OPT_EMIT
+    if adopt:
+      skip = self._adopt_update(what, a)
+    w.compare(what, tol, skip)
     for k, host, dev in copies:
       self._compare_copy(what, name, a, k, host, dev.cpu())
     if name == "sort_items":
@@ -372,6 +408,60 @@ class MirrorOps(dry_run.DryOps):
     for t in _tag(name, a):
       REPLAYED[t] += 1
     return want
+
+  def _adopt_update(self, what, a):
+    """Kernel-authoritative ``segment_update`` (see the module doc): rows of the op's tables that
+    no key touched must be bit-identical in every weight and state buffer; the touched rows are
+    copied from the mirrors into the host buffers.  Returns the storages ``compare`` must skip:
+    these buffers, checked here."""
+    w = self.world
+    w.dev.synchronize()
+    T = np.frombuffer(a["tables"].numpy().tobytes(), dtype=TABLE_DESC)[:a["n_tables"]]
+    nu = int(a["n_unique"][0])
+    keys = a["keys"][a["seg"][:nu].long()].long().numpy()
+    opt = BY_CODE[a["kind"]]
+    half_state = bool(a["state_dtype"]) and opt.elementwise_state
+    skip = set()
+    # storage -> (offset, rows, row bytes, table, slot, key base) of every weight / state buffer
+    regions = collections.defaultdict(list)
+    for m, t in enumerate(T):
+      rows, width, base = int(t["rows"]), int(t["width"]), int(t["key_base"])
+      mine = keys[(keys >= base) & (keys < base + rows)] - base
+      slots = [("weight", t["weight"], width * (2 if a["table_dtype"] else 4))]
+      for k, s in enumerate(opt.slots):
+        slots.append((f"state{k}", t[f"state{k}"], 4 if s.per_row else
+                      width * (2 if half_state else 4)))
+      for label, ptr, row_bytes in slots:
+        start = w._find(int(ptr))
+        assert start is not None, f"{what}: table {m} {label} is not a registered buffer"
+        off = int(ptr) - start
+        regions[start].append((off, rows, row_bytes, m, label, base))
+        host = w.tensor(int(ptr), torch.uint8, rows * row_bytes).view(rows, row_bytes)
+        dev = w.mirrors[start][off:off + rows * row_bytes].view(rows, row_bytes)
+        idx = torch.as_tensor(mine, dtype=torch.long)
+        host[idx] = dev[idx.to(dev.device)].cpu()
+    for start, parts in regions.items():
+      skip.add(start)
+      n = w._ranges[start] - start
+      got = w.mirrors[start][:n].cpu()
+      want = w.tensor(start, torch.uint8, n)
+      if torch.equal(got, want):
+        continue
+      i = int(torch.nonzero(got != want)[0])
+      name, _ = w.describe(start)
+      for off, rows, row_bytes, m, label, base in parts:
+        if off <= i < off + rows * row_bytes:
+          row = (i - off) // row_bytes
+          raise AssertionError(f"{what}: {name}: row {row} of table {m} ({label}, key "
+                               f"{base + row}) changed, but no key of the op touched it")
+      raise AssertionError(f"{what}: {name} differs at byte {i}, outside every table's rows")
+    # a -0.0 weight (a 16-bit rounding or FTRL's closed form) pools to -0.0 through one id in the
+    # kernels but to +0.0 in the interpreter's sum: later ops see the zero weights as +0.0
+    tdt = {0: torch.float32, 1: torch.bfloat16, 2: torch.float16}[int(a["table_dtype"])]
+    for t in T:
+      wt = w.tensor(int(t["weight"]), tdt, int(t["rows"]) * int(t["width"]))
+      wt[wt == 0] = 0
+    return skip
 
   @staticmethod
   def _compare_copy(what, name, a, k, host, got):

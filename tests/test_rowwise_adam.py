@@ -26,7 +26,7 @@ from distributed_embeddings_b200.parallel.hybrid import SparseRowOptimizer
 import test_fused_optimizers as tfo  # pylint: disable=wrong-import-order
 import optim_reference  # pylint: disable=wrong-import-order
 from optim_reference import (TINY, U, _e_sum, _ulp32, f32,  # pylint: disable=wrong-import-order
-                             half_within, worst_table_ratio)
+                             worst_table_ratio)
 from test_dry_run import assemble  # pylint: disable=wrong-import-order
 from test_examples_smoke import run as run_example  # pylint: disable=wrong-import-order
 
@@ -123,141 +123,26 @@ def _initial_state(rows, width):
   return [np.zeros((rows, width), np.float32), np.zeros(rows, np.float32)]
 
 
-def _state_of(demb, t, rows, width):
-  st = demb.get_optimizer_state()
-  if st["tables"] is None:
+class _Spec(tfo.Spec):
+  """Row-wise Adam for the driver of ``test_fused_optimizers.py``: m element-wise, v per row (per
+  column slice: the mean over the slice's columns)."""
+
+  def initial(self, rows, width, sdt):
     return _initial_state(rows, width)
-  m, v = st["tables"][t]
-  assert m.shape == (rows, width) and v.shape == (rows, 1)
-  return [np.asarray(m, dtype=np.float32), np.asarray(v, dtype=np.float32)[:, 0]]
+
+  def model(self, case, before, state, occ, step, scale):
+    return table_step(KIND, before, state, occ[0], occ[1], scale, case["lrs"][step], step + 1,
+                      _cfg(case.get("wd", 0.0)))
 
 
-def _slices(demb, t, width):
-  """Column ranges of table ``t`` that keep their own row word (the whole row unless sliced)."""
-  st = demb.strategy
-  if t not in st.table_groups[1]:
-    return [(0, width)]
-  gt = st.table_groups[1].index(t)
-  return sorted({(s.col_start, s.col_end) for shards in st.shards for s in shards
-                 if s.table == gt})
+SPEC = _Spec(KIND)
+_slices = tfo._slices
 
 
-def _model(case, before, state, occ, step, scale, slices):
-  """The float64 step of one table, slice by slice; v is checked only for an unsliced table."""
-  rows, vals = occ
-  out, bound, touched = {"p": None, "s0": None}, {"p": None, "s0": None}, None
-  parts = []
-  for c0, c1 in slices:
-    o, b, touched = table_step(KIND, before[:, c0:c1], [state[0][:, c0:c1], state[1]], rows,
-                               vals[:, c0:c1], scale, case["lrs"][step], step + 1,
-                               _cfg(case.get("wd", 0.0)))
-    parts.append((o, b))
-  for k in ("p", "s0"):
-    out[k] = torch.cat([o[k] for o, _ in parts], 1)
-    bound[k] = torch.cat([b[k] for _, b in parts], 1)
-  if len(slices) == 1:
-    out["s1"], bound["s1"] = parts[0][0]["s1"], parts[0][1]["s1"]
-  return out, bound, touched
-
-
-def _check_step(case, out, bound, touched, after, state_after, slack, weights_only):
-  bound = {k: slack * b for k, b in bound.items()}
-  got = {"p": after}
-  if not weights_only:
-    got["s0"], got["s1"] = state_after
-  else:
-    out, bound = {"p": out["p"]}, {"p": bound["p"]}
-  tdt = case.get("table_dtype", torch.float32)
-  sdt = case.get("state_dtype", torch.float32)
-  idx = np.nonzero(touched)[0]
-  keys = idx + case.get("key_base", 0)
-  for k in out:
-    g = torch.as_tensor(np.asarray(got[k], dtype=np.float64))
-    dt = {"p": tdt, "s0": sdt, "s1": torch.float32}[k]
-    unt = ~torch.as_tensor(touched)
-    assert torch.equal(g[unt], out[k][unt]), f"untouched rows of {k} changed"
-    if dt == torch.float32:
-      r = worst_table_ratio({k: out[k][idx]}, {k: bound[k][idx]}, {k: g[idx].numpy()})
-      assert r <= 1.0, f"{k}: worst error / bound {r}"
-    else:
-      bad = half_within(g[idx], out[k][idx], bound[k][idx], dt, case["step"] + 1, keys,
-                        {"p": 0, "s0": 1}[k])
-      assert bad == 0, f"{k}: {bad} 16-bit values outside the rounding of the bound"
-
-
-def _run(case, world=1, dev=None, plan=None, route=None):
-  """``case`` for ``len(case['lrs'])`` steps (the driver of test_fused_optimizers.py), every step
-  checked; ``plan``: extra DistributedEmbedding arguments (slicing)."""
-  embs = [{"input_dim": r, "output_dim": w, "combiner": c} for r, w, c in case["tables"]]
-  kw = dict(input_table_map=list(case["imap"]), strategy="basic")
-  kw.update(plan or {})
-  if case.get("table_dtype", torch.float32) != torch.float32:
-    kw["table_dtype"] = case["table_dtype"]
-  if case.get("compute_dtype"):
-    kw["compute_dtype"] = case["compute_dtype"]
-  opt = {"weight_decay": case.get("wd", 0.0)}
-  if case.get("state_dtype", torch.float32) != torch.float32:
-    opt["state_dtype"] = case["state_dtype"]
-  cdt = case.get("compute_dtype", torch.float32)
-  torch.manual_seed(case.get("seed", 0))
-  if dev is None:
-    sim, des = dry_run.build_engines(embs, world, dp_input=True, **kw)
-  else:
-    sim, des = None, [de.DistributedEmbedding(embs, device=dev, backend="fused", world_size=1,
-                                              rank=0, **kw)]
-  gen = np.random.default_rng(case.get("seed", 0))
-  tables = [gen.standard_normal((r, w)).astype(np.float32) for r, w, _ in case["tables"]]
-  for d in des:
-    d.set_weights(tables)
-    d.set_optimizer(KIND, lr=case["lrs"][0], **opt)
-    assert d._fused_optimizer["eps"] == 1e-8
-    if any(h == "ragged" for h in case["hots"]):
-      d.ragged_capacity = 8
-  demb = des[0]
-  routes = []
-  assert world == 1 or len(case["lrs"]) == 1
-  for step, lr in enumerate(case["lrs"]):
-    if step and lr != case["lrs"][step - 1]:
-      for d in des:
-        d.set_learning_rate(lr)
-    ids, grad = tfo._draw(case, step)
-    grad = grad.to(cdt)
-    lb = case["batch"] // world
-    before = tfo._weights(des, world)
-    states = [_state_of(demb, t, r, w) if world == 1 else _initial_state(r, w)
-              for t, (r, w, _) in enumerate(case["tables"])]
-
-    def rank_fn(r):
-      d = des[r]
-      out = d(tfo._as_inputs(case, ids, d.device if dev is None else dev, r * lb, (r + 1) * lb),
-              concat=True)
-      eng = d._engine
-      if not isinstance(eng.ops, tfo._Counting):
-        eng.ops = tfo._Counting(eng.ops)
-      out.backward(grad[r * lb:(r + 1) * lb].to(out.device))
-      return eng.ops.routes
-    if dev is None:
-      routes = list(dry_run.run_ranks(sim, rank_fn)[0])
-    else:
-      routes = list(rank_fn(0))
-      torch.cuda.synchronize()
-    if case.get("edges"):
-      tfo._check_edge_layout(case, ids, des[0]._engine)
-    after = tfo._weights(des, world)
-    if world == 1:
-      assert demb.get_optimizer_state()["step"] == step + 1
-    for t, (r, w, _) in enumerate(case["tables"]):
-      occ = tfo._occurrences(case, ids, grad.float(), t)
-      out, bound, touched = _model(case, before[t], states[t], occ, step, 1.0 / world,
-                                   _slices(demb, t, w))
-      sa = _state_of(demb, t, r, w) if world == 1 else None
-      # the interpreter computes in torch fp32 ops without fma: three times the kernel's bounds
-      _check_step(dict(case, step=step), out, bound, touched, after[t], sa,
-                  slack=3.0 if dev is None else 1.0, weights_only=world > 1 or "s1" not in out)
-  want = route or tfo._expected_route(case, KIND)
-  assert routes and set(routes) <= ({want} if want != "any" else
-                                    {"balanced", "per_row_vec4", "per_row_vec1"}), (routes, want)
-  return des
+def _run(case, world=1, dev=None, plan=None, route=None, **kw):
+  """``case`` for ``len(case['lrs'])`` steps through the driver of test_fused_optimizers.py,
+  every step and every slot checked; ``plan``: extra DistributedEmbedding arguments (slicing)."""
+  return tfo._run(case, KIND, world, dev, plan, route, spec=SPEC, **kw)
 
 
 _case, _with = tfo._case, tfo._with
