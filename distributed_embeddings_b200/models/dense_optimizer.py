@@ -12,6 +12,13 @@ trainers do the same.  The math is that of the fused embedding update (``apply_u
   p -= lr * (m / (1 - b1^t)) / (sqrt(v / (1 - b2^t)) + eps)`` (``beta1=0.9``, ``beta2=0.999``,
   ``eps=1e-8``).
 
+Every kind takes ``weight_decay`` (lambda, default 0) and ``weight_decay_mode``: ``"l2"``
+(default) adds ``lambda * p`` to the gradient before the update; ``"decoupled"`` (AdamW-style)
+first scales ``p`` by the fp32 ``1 - lr * lambda`` and then applies the step of the undecayed
+gradient, ``p = (1 - lr * lambda) * p - lr * u``.  SGD's update is ``p -= lr * (g + lambda * p)``
+in both modes.  Unlike the lazy embedding optimizers, the decay applies to every dense element
+(MLP weights, biases, replicated tables) on every step; pad elements of the flat buffers stay 0.
+
 The learning rate is the trainer's device-resident ``lr_t`` word and Adam's step count ``t`` is a
 device-resident fp32 word advanced inside the step, so both follow a scheduler under CUDA-graph
 replay.
@@ -28,12 +35,15 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import torch
 from torch import nn
 
+from ..parallel.embedding_optimizers import WEIGHT_DECAY_MODE_CODE, WEIGHT_DECAY_MODES
+
 KINDS = ("sgd", "adagrad", "adam")
 _DEFAULTS = {
     "sgd": {},
     "adagrad": {"eps": 1e-7, "initial_accumulator_value": 0.1},
     "adam": {"beta1": 0.9, "beta2": 0.999, "eps": 1e-8},
 }
+_DECAY = {"weight_decay": 0.0, "weight_decay_mode": "l2"}  # every kind
 
 
 def dense_optimizer_config(kind: str, kwargs: Optional[dict] = None) -> dict:
@@ -41,13 +51,28 @@ def dense_optimizer_config(kind: str, kwargs: Optional[dict] = None) -> dict:
   kind = str(kind).lower()
   if kind not in KINDS:
     raise ValueError(f"dense_optimizer must be one of {', '.join(KINDS)}, got {kind!r}")
-  cfg = dict(_DEFAULTS[kind])
+  cfg = dict(_DEFAULTS[kind], **_DECAY)
   unknown = sorted(set(kwargs or {}) - set(cfg))
   if unknown:
     raise ValueError(f"dense optimizer {kind!r} takes no argument(s) {', '.join(unknown)}")
-  cfg.update({k: float(v) for k, v in (kwargs or {}).items()})
+  kwargs = dict(kwargs or {})
+  mode = kwargs.pop("weight_decay_mode", cfg["weight_decay_mode"])
+  if mode not in WEIGHT_DECAY_MODES:
+    raise ValueError(f"dense optimizer weight_decay_mode must be one of "
+                     f"{', '.join(WEIGHT_DECAY_MODES)}, got {mode!r}")
+  cfg.update({k: float(v) for k, v in kwargs.items()})
+  if not cfg["weight_decay"] >= 0.0:
+    raise ValueError(f"dense optimizer weight_decay must be >= 0, got {cfg['weight_decay']}")
+  cfg["weight_decay_mode"] = mode
   cfg["kind"] = kind
   return cfg
+
+
+def decay_args(cfg: dict) -> tuple:
+  """The trailing ``(weight_decay, weight_decay_mode)`` of the dense ops, empty without decay
+  (the launch then keeps the arguments and kernels of a run without decay)."""
+  wd = cfg["weight_decay"]
+  return (wd, WEIGHT_DECAY_MODE_CODE[cfg["weight_decay_mode"]]) if wd != 0.0 else ()
 
 
 def slot_init(cfg: dict) -> List[float]:
@@ -88,14 +113,15 @@ class FlatDenseOptimizer:
   def apply(self, ops, p16: torch.Tensor, g32: torch.Tensor, lr_t: torch.Tensor):
     """p32 update + ``p16 = bf16(p32)`` + ``g32 = 0``, one launch (Adam: plus the step word)."""
     c = self.cfg
+    decay = decay_args(c)
     if self.kind == "sgd":
-      ops.dense_sgd(self.p32, p16, g32, lr_t, 1.0)
+      ops.dense_sgd(self.p32, p16, g32, lr_t, 1.0, *decay)
     elif self.kind == "adagrad":
-      ops.dense_adagrad(self.p32, p16, g32, self.state[0], lr_t, c["eps"])
+      ops.dense_adagrad(self.p32, p16, g32, self.state[0], lr_t, c["eps"], *decay)
     else:
       self.step_t.add_(1.0)  # device counter: the bias corrections stay right under graph replay
       ops.dense_adam(self.p32, p16, g32, self.state[0], self.state[1], lr_t, self.step_t,
-                     c["beta1"], c["beta2"], c["eps"])
+                     c["beta1"], c["beta2"], c["eps"], *decay)
 
   def snapshot(self) -> List[torch.Tensor]:
     return [s.clone() for s in self.state] + ([self.step_t.clone()] if self.step_t is not None

@@ -32,7 +32,10 @@ class HybridTrainer:
     scheduler: optional :class:`LearningRateScheduler`.
     dense_optimizer: ``sgd`` | ``adagrad`` | ``adam`` for the dense parameters (MLPs and
       replicated tables), hyperparameters in ``dense_optimizer_kwargs`` (see
-      ``models/dense_optimizer.py``); ``momentum`` applies to ``sgd`` only.
+      ``models/dense_optimizer.py``), ``weight_decay`` / ``weight_decay_mode`` included;
+      ``momentum`` applies to ``sgd`` only.  Momentum SGD takes L2 decay as
+      ``torch.optim.SGD(weight_decay=...)`` does (into the gradient, before the momentum
+      buffer); ``weight_decay_mode="decoupled"`` with momentum raises ``ValueError``.
   """
 
   def __init__(self, model: nn.Module, lr: float = 24.0, embedding_optimizer: str = "sgd",
@@ -44,6 +47,10 @@ class HybridTrainer:
     self.dense_cfg = dense_optimizer_config(dense_optimizer, dense_optimizer_kwargs)
     if momentum != 0.0 and self.dense_cfg["kind"] != "sgd":
       raise ValueError("momentum applies to dense_optimizer='sgd' only")
+    if momentum != 0.0 and self.dense_cfg["weight_decay"] and \
+        self.dense_cfg["weight_decay_mode"] == "decoupled":
+      raise ValueError("momentum SGD takes weight_decay_mode='l2' only (torch.optim.SGD's "
+                       "weight decay); decoupled decay is for momentum=0")
     self.model = model
     self.emb = model.embedding
     self.emb.set_optimizer(embedding_optimizer, lr=lr, **(embedding_optimizer_kwargs or {}))
@@ -61,6 +68,7 @@ class HybridTrainer:
     self.bucket = GradBucket(self.dense_params, self.ctx if self.world > 1 else None)
     self.bucket.attach()
     self.opt = torch.optim.SGD(self.dense_params, lr=lr, momentum=momentum,
+                               weight_decay=self.dense_cfg["weight_decay"],
                                foreach=dev.type == "cuda")
     # plain SGD keeps its learning rate in device memory: a captured CUDA graph bakes host
     # scalars in, so a scheduler would otherwise leave the dense lr frozen at its capture-time
@@ -110,6 +118,9 @@ class HybridTrainer:
       return
     with torch.no_grad():
       grads = [p.grad for p in params]
+      wd = self.dense_cfg["weight_decay"]
+      if wd:  # p -= lr * (g + wd * p): SGD's update in both decay modes
+        grads = torch._foreach_add(grads, params, alpha=wd)
       if params[0].is_cuda:
         upd = torch._foreach_mul(grads, self.lr_t)  # device-resident lr (graph replay safe)
         torch._foreach_sub_(params, upd)
@@ -123,6 +134,11 @@ class HybridTrainer:
     if not params:
       return
     with torch.no_grad():
+      if c["weight_decay"] and c["weight_decay_mode"] == "decoupled":
+        # p = (1 - lr wd) p before the step of the undecayed gradient (device lr: graph safe)
+        torch._foreach_mul_(params, 1.0 - self.lr_t * c["weight_decay"])
+      elif c["weight_decay"]:
+        grads = torch._foreach_add(grads, params, alpha=c["weight_decay"])
       if c["kind"] == "adagrad":
         acc = self.dense_state[0]
         torch._foreach_addcmul_(acc, grads, grads)

@@ -358,10 +358,15 @@ void segment_update(const Tensor& descs, const Tensor& tables, int64_t n_tables,
                     bool vec4, const c10::optional<Tensor>& scratch, int64_t step_ptr,
                     int64_t table_dtype, int64_t state_dtype, double lr_power = -0.5,
                     double l1 = 0.0, double l2 = 0.0, double l2_shrinkage = 0.0,
-                    double ftrl_beta = 0.0) {
+                    double ftrl_beta = 0.0, int64_t weight_decay_mode = de::kWeightDecayL2) {
   c10::cuda::CUDAGuard guard(descs.device());
   TORCH_CHECK(table_dtype >= 0 && table_dtype <= 2, "table_dtype: 0 fp32, 1 bf16, 2 fp16");
   TORCH_CHECK(state_dtype == 0 || state_dtype == 1, "state_dtype: 0 fp32, 1 bf16");
+  TORCH_CHECK(weight_decay_mode == de::kWeightDecayL2 ||
+                  weight_decay_mode == de::kWeightDecayDecoupled,
+              "weight_decay_mode: 0 l2, 1 decoupled");
+  TORCH_CHECK(weight_decay_mode == de::kWeightDecayL2 || opt_kind != de::kOptFtrl,
+              "decoupled weight decay does not apply to FTRL");
   de::OptimizerArgs opt;
   opt.kind = static_cast<int32_t>(opt_kind);
   opt.lr = static_cast<float>(lr);
@@ -379,6 +384,7 @@ void segment_update(const Tensor& descs, const Tensor& tables, int64_t n_tables,
   opt.l2 = static_cast<float>(l2);
   opt.l2_shrinkage = static_cast<float>(l2_shrinkage);
   opt.ftrl_beta = static_cast<float>(ftrl_beta);
+  opt.weight_decay_mode = static_cast<int32_t>(weight_decay_mode);
   if (opt.kind == de::kOptEmit) TORCH_CHECK(emit_keys.has_value() && emit_rows.has_value());
   // occurrence-balanced path: immune to id skew (needs a zeroed scratch of >= n_items/32 rows)
   if (scratch.has_value() && vec4 && max_width <= 128 && opt.kind != de::kOptEmit) {
@@ -1102,14 +1108,24 @@ void head_eval(const Tensor& x, const Tensor& w, const Tensor& bias, const Tenso
   check_launch();
 }
 
-void dense_sgd(Tensor p32, Tensor p16, Tensor g32, const Tensor& lr, double grad_scale) {
+// weight_decay_mode of the dense ops: 0 L2, 1 decoupled (see OptimizerArgs)
+void check_decay_mode(int64_t weight_decay_mode) {
+  TORCH_CHECK(weight_decay_mode == de::kWeightDecayL2 ||
+                  weight_decay_mode == de::kWeightDecayDecoupled,
+              "weight_decay_mode: 0 l2, 1 decoupled");
+}
+
+// SGD's update is the same under both decay modes: p -= lr * (grad_scale * g + weight_decay * p)
+void dense_sgd(Tensor p32, Tensor p16, Tensor g32, const Tensor& lr, double grad_scale,
+               double weight_decay = 0.0, int64_t weight_decay_mode = de::kWeightDecayL2) {
+  check_decay_mode(weight_decay_mode);
   TORCH_CHECK(p32.is_cuda() && p32.scalar_type() == at::kFloat && g32.scalar_type() == at::kFloat &&
               p16.scalar_type() == at::kBFloat16 && lr.scalar_type() == at::kFloat);
   TORCH_CHECK(p32.numel() % 4 == 0 && p32.numel() == g32.numel() && p32.numel() == p16.numel());
   c10::cuda::CUDAGuard guard(p32.device());
   de::launch_sgd_update(p32.data_ptr<float>(), p16.data_ptr(), g32.data_ptr<float>(),
                         lr.data_ptr<float>(), static_cast<float>(grad_scale), p32.numel(),
-                        sm_count(), cur_stream());
+                        sm_count(), cur_stream(), static_cast<float>(weight_decay));
   check_launch();
 }
 
@@ -1143,25 +1159,31 @@ void check_dense_opt(const Tensor& p32, const Tensor& p16, const Tensor& g32,
   if (step != nullptr) word(*step, "step");
 }
 
-void dense_adagrad(Tensor p32, Tensor p16, Tensor g32, Tensor acc, const Tensor& lr, double eps) {
+void dense_adagrad(Tensor p32, Tensor p16, Tensor g32, Tensor acc, const Tensor& lr, double eps,
+                   double weight_decay = 0.0, int64_t weight_decay_mode = de::kWeightDecayL2) {
+  check_decay_mode(weight_decay_mode);
   check_dense_opt(p32, p16, g32, {{&acc, "acc"}}, lr, nullptr);
   c10::cuda::CUDAGuard guard(p32.device());
   de::launch_dense_opt(de::kOptAdagrad, p32.data_ptr<float>(), p16.data_ptr(),
                        g32.data_ptr<float>(), acc.data_ptr<float>(), nullptr,
                        lr.data_ptr<float>(), nullptr, 0.f, 0.f, static_cast<float>(eps),
-                       p32.numel(), sm_count(), cur_stream());
+                       p32.numel(), sm_count(), cur_stream(), static_cast<float>(weight_decay),
+                       static_cast<int>(weight_decay_mode));
   check_launch();
 }
 
 void dense_adam(Tensor p32, Tensor p16, Tensor g32, Tensor m, Tensor v, const Tensor& lr,
-                const Tensor& step, double beta1, double beta2, double eps) {
+                const Tensor& step, double beta1, double beta2, double eps,
+                double weight_decay = 0.0, int64_t weight_decay_mode = de::kWeightDecayL2) {
+  check_decay_mode(weight_decay_mode);
   check_dense_opt(p32, p16, g32, {{&m, "m"}, {&v, "v"}}, lr, &step);
   c10::cuda::CUDAGuard guard(p32.device());
   de::launch_dense_opt(de::kOptAdam, p32.data_ptr<float>(), p16.data_ptr(),
                        g32.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(),
                        lr.data_ptr<float>(), step.data_ptr<float>(), static_cast<float>(beta1),
                        static_cast<float>(beta2), static_cast<float>(eps), p32.numel(),
-                       sm_count(), cur_stream());
+                       sm_count(), cur_stream(), static_cast<float>(weight_decay),
+                       static_cast<int>(weight_decay_mode));
   check_launch();
 }
 
@@ -1457,7 +1479,7 @@ TORCH_LIBRARY(de_b200, m) {
       "Tensor? emit_keys, Tensor? emit_rows, int max_width, int act_dtype, bool vec4, "
       "Tensor? scratch, int step_ptr, int table_dtype=0, int state_dtype=0, "
       "float lr_power=-0.5, float l1=0., float l2=0., float l2_shrinkage=0., "
-      "float ftrl_beta=0.) -> ()",
+      "float ftrl_beta=0., int weight_decay_mode=0) -> ()",
       &segment_update);
   m.def(
       "embedding_lookup_fwd(Tensor param, Tensor values, Tensor? offsets, int hotness, int batch, "
@@ -1542,16 +1564,17 @@ TORCH_LIBRARY(de_b200, m) {
       "Tensor(b!) hist, Tensor(c!) loss_sum, Tensor(d!) count) -> ()",
       &head_eval);
   m.def(
-      "dense_sgd(Tensor(a!) p32, Tensor(b!) p16, Tensor(c!) g32, Tensor lr, float grad_scale) "
-      "-> ()",
+      "dense_sgd(Tensor(a!) p32, Tensor(b!) p16, Tensor(c!) g32, Tensor lr, float grad_scale, "
+      "float weight_decay=0., int weight_decay_mode=0) -> ()",
       &dense_sgd);
   m.def(
       "dense_adagrad(Tensor(a!) p32, Tensor(b!) p16, Tensor(c!) g32, Tensor(d!) acc, Tensor lr, "
-      "float eps) -> ()",
+      "float eps, float weight_decay=0., int weight_decay_mode=0) -> ()",
       &dense_adagrad);
   m.def(
       "dense_adam(Tensor(a!) p32, Tensor(b!) p16, Tensor(c!) g32, Tensor(d!) m, Tensor(e!) v, "
-      "Tensor lr, Tensor step, float beta1, float beta2, float eps) -> ()",
+      "Tensor lr, Tensor step, float beta1, float beta2, float eps, float weight_decay=0., "
+      "int weight_decay_mode=0) -> ()",
       &dense_adam);
   m.def("cast_pad(Tensor src, Tensor(a!) dst) -> ()", &cast_pad);
   m.def(

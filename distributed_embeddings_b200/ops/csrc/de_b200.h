@@ -116,7 +116,13 @@ struct OptimizerArgs {
   float l1, l2;
   float l2_shrinkage;
   float ftrl_beta;     // Keras's beta: adds beta / (2 lr) to l2
+  // kWeightDecayL2: weight_decay * w joins the gradient; kWeightDecayDecoupled (AdamW): the
+  // weight is scaled by 1 - lr * weight_decay and the step comes from the undecayed gradient
+  int32_t weight_decay_mode;
 };
+
+constexpr int kWeightDecayL2 = 0;
+constexpr int kWeightDecayDecoupled = 1;
 
 // ---- pooled lookup forward (+ optional fused push to peer output buffers) ------------------
 // ids come from src.p[g / src_batch] (peer mapped) or desc.ids; pooled rows are stored to
@@ -375,14 +381,17 @@ bool launch_head_loss(const void* x, int K, const void* w, const void* bias, con
 bool launch_head_eval(const void* x, int K, const void* w, const void* bias, const float* labels,
                       int64_t batch, const int64_t* n_valid, float* probs, int64_t* hist, int nb,
                       double* loss_sum, int64_t* count, int sm_count, cudaStream_t stream);
+// weight_decay != 0: p32 -= lr * (grad_scale * g32 + weight_decay * p32) (both decay modes)
 void launch_sgd_update(float* p32, void* p16, float* g32, const float* lr_ptr, float grad_scale,
-                       int64_t n, int sm_count, cudaStream_t stream);
+                       int64_t n, int sm_count, cudaStream_t stream, float weight_decay = 0.f);
 // Fused dense Adagrad (kind kOptAdagrad, s0 = accumulator) or Adam (kOptAdam, s0 / s1 = m / v,
 // *step_ptr = t after this step) + bf16 re-cast + gradient zeroing over n (multiple of 4) fp32
-// elements; false for another kind.
+// elements; false for another kind.  weight_decay with weight_decay_mode kWeightDecayL2 or
+// kWeightDecayDecoupled, as the embedding update applies it.
 bool launch_dense_opt(int kind, float* p32, void* p16, float* g32, float* s0, float* s1,
                       const float* lr_ptr, const float* step_ptr, float beta1, float beta2,
-                      float eps, int64_t n, int sm_count, cudaStream_t stream);
+                      float eps, int64_t n, int sm_count, cudaStream_t stream,
+                      float weight_decay = 0.f, int weight_decay_mode = kWeightDecayL2);
 void launch_cast_pad(const float* src, int src_cols, void* dst, int dst_cols, int64_t rows,
                      cudaStream_t stream);
 

@@ -896,19 +896,31 @@ head_eval_kernel(const bf16* __restrict__ x, const bf16* __restrict__ w,
 }
 
 // p32 -= lr * g32 ; p16 = bf16(p32) ; g32 = 0   (lr read from device memory: graph replay safe)
+// kDecay: p32 -= lr * (grad_scale * g32 + weight_decay * p32), SGD's update under either weight
+// decay mode
+template <bool kDecay>
 __global__ void __launch_bounds__(256)
 sgd_update_kernel(float* __restrict__ p32, bf16* __restrict__ p16, float* __restrict__ g32,
-                  const float* __restrict__ lr_ptr, float grad_scale, int64_t n_vec4) {
+                  const float* __restrict__ lr_ptr, float grad_scale, float weight_decay,
+                  int64_t n_vec4) {
   const float step = -(*lr_ptr) * grad_scale;
+  const float neg_lr = -(*lr_ptr);
   const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
   for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n_vec4;
        i += stride) {
     float4 p = reinterpret_cast<float4*>(p32)[i];
     const float4 g = reinterpret_cast<const float4*>(g32)[i];
-    p.x = fmaf(step, g.x, p.x);
-    p.y = fmaf(step, g.y, p.y);
-    p.z = fmaf(step, g.z, p.z);
-    p.w = fmaf(step, g.w, p.w);
+    if constexpr (kDecay) {
+      p.x = fmaf(neg_lr, fmaf(weight_decay, p.x, __fmul_rn(grad_scale, g.x)), p.x);
+      p.y = fmaf(neg_lr, fmaf(weight_decay, p.y, __fmul_rn(grad_scale, g.y)), p.y);
+      p.z = fmaf(neg_lr, fmaf(weight_decay, p.z, __fmul_rn(grad_scale, g.z)), p.z);
+      p.w = fmaf(neg_lr, fmaf(weight_decay, p.w, __fmul_rn(grad_scale, g.w)), p.w);
+    } else {
+      p.x = fmaf(step, g.x, p.x);
+      p.y = fmaf(step, g.y, p.y);
+      p.z = fmaf(step, g.z, p.z);
+      p.w = fmaf(step, g.w, p.w);
+    }
     reinterpret_cast<float4*>(p32)[i] = p;
     reinterpret_cast<float4*>(g32)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     __nv_bfloat162 a = __floats2bfloat162_rn(p.x, p.y), b = __floats2bfloat162_rn(p.z, p.w);
@@ -922,11 +934,18 @@ sgd_update_kernel(float* __restrict__ p32, bf16* __restrict__ p16, float* __rest
 // Adagrad / Adam over the flat dense buffers, element by element with the expressions of the
 // embedding update (apply_update in sparse_update_kernels.cu), then p16 = bf16(p32) and g32 = 0
 // (the next step's gradient kernels accumulate into g32).  lr and Adam's step count t are device
-// words: graph replay safe.  s0 = Adagrad accumulator or Adam m, s1 = Adam v.
-template <int KIND>
+// words: graph replay safe.  s0 = Adagrad accumulator or Adam m, s1 = Adam v.  DECAY: 0 none,
+// kDenseDecayL2 (g += weight_decay * p before the update), kDenseDecayDecoupled (p *= 1 - lr *
+// weight_decay before the step, which the undecayed g drives: torch.optim.AdamW's order).
+constexpr int kDenseDecayL2 = 1;
+constexpr int kDenseDecayDecoupled = 2;
+
+template <int KIND, int DECAY>
 __device__ __forceinline__ void dense_opt_elem(float& p, float& a, float& v, float g, float lr,
                                                float beta1, float beta2, float bias1, float bias2,
-                                               float eps) {
+                                               float eps, float weight_decay, float keep) {
+  if constexpr (DECAY == kDenseDecayL2) g = fmaf(weight_decay, p, g);
+  if constexpr (DECAY == kDenseDecayDecoupled) p = __fmul_rn(p, keep);
   if constexpr (KIND == kOptAdagrad) {
     a = fmaf(g, g, a);
     p -= lr * g / (sqrtf(a) + eps);
@@ -939,13 +958,14 @@ __device__ __forceinline__ void dense_opt_elem(float& p, float& a, float& v, flo
   }
 }
 
-template <int KIND>
+template <int KIND, int DECAY>
 __global__ void __launch_bounds__(256)
 dense_opt_kernel(float* __restrict__ p32, bf16* __restrict__ p16, float* __restrict__ g32,
                  float* __restrict__ s0, float* __restrict__ s1, const float* __restrict__ lr_ptr,
                  const float* __restrict__ step_ptr, float beta1, float beta2, float eps,
-                 int64_t n_vec4) {
+                 float weight_decay, int64_t n_vec4) {
   const float lr = *lr_ptr;
+  const float keep = fmaf(-lr, weight_decay, 1.f);  // decoupled decay only
   float bias1 = 1.f, bias2 = 1.f;
   if constexpr (KIND == kOptAdam) {  // bias corrections as resolve_step computes them
     const float t = *step_ptr;
@@ -960,10 +980,14 @@ dense_opt_kernel(float* __restrict__ p32, bf16* __restrict__ p16, float* __restr
     float4 a = reinterpret_cast<float4*>(s0)[i];
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
     if constexpr (KIND == kOptAdam) v = reinterpret_cast<float4*>(s1)[i];
-    dense_opt_elem<KIND>(p.x, a.x, v.x, g.x, lr, beta1, beta2, bias1, bias2, eps);
-    dense_opt_elem<KIND>(p.y, a.y, v.y, g.y, lr, beta1, beta2, bias1, bias2, eps);
-    dense_opt_elem<KIND>(p.z, a.z, v.z, g.z, lr, beta1, beta2, bias1, bias2, eps);
-    dense_opt_elem<KIND>(p.w, a.w, v.w, g.w, lr, beta1, beta2, bias1, bias2, eps);
+    dense_opt_elem<KIND, DECAY>(p.x, a.x, v.x, g.x, lr, beta1, beta2, bias1, bias2, eps,
+                                weight_decay, keep);
+    dense_opt_elem<KIND, DECAY>(p.y, a.y, v.y, g.y, lr, beta1, beta2, bias1, bias2, eps,
+                                weight_decay, keep);
+    dense_opt_elem<KIND, DECAY>(p.z, a.z, v.z, g.z, lr, beta1, beta2, bias1, bias2, eps,
+                                weight_decay, keep);
+    dense_opt_elem<KIND, DECAY>(p.w, a.w, v.w, g.w, lr, beta1, beta2, bias1, bias2, eps,
+                                weight_decay, keep);
     reinterpret_cast<float4*>(p32)[i] = p;
     reinterpret_cast<float4*>(s0)[i] = a;
     if constexpr (KIND == kOptAdam) reinterpret_cast<float4*>(s1)[i] = v;
@@ -1274,31 +1298,48 @@ bool launch_head_eval(const void* x, int K, const void* w, const void* bias, con
 }
 
 void launch_sgd_update(float* p32, void* p16, float* g32, const float* lr_ptr, float grad_scale,
-                       int64_t n, int sm_count, cudaStream_t stream) {
+                       int64_t n, int sm_count, cudaStream_t stream, float weight_decay) {
   const int64_t n_vec4 = n / 4;  // buffers are padded to 16 bytes
   if (n_vec4 <= 0) return;
   int64_t blocks = (n_vec4 + 255) / 256;
   if (blocks > sm_count * 8) blocks = sm_count * 8;
-  sgd_update_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
-      p32, reinterpret_cast<bf16*>(p16), g32, lr_ptr, grad_scale, n_vec4);
+  auto launch = [&](auto kernel) {
+    kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
+        p32, reinterpret_cast<bf16*>(p16), g32, lr_ptr, grad_scale, weight_decay, n_vec4);
+  };
+  if (weight_decay != 0.f) launch(sgd_update_kernel<true>);
+  else launch(sgd_update_kernel<false>);
 }
 
 bool launch_dense_opt(int kind, float* p32, void* p16, float* g32, float* s0, float* s1,
                       const float* lr_ptr, const float* step_ptr, float beta1, float beta2,
-                      float eps, int64_t n, int sm_count, cudaStream_t stream) {
+                      float eps, int64_t n, int sm_count, cudaStream_t stream, float weight_decay,
+                      int weight_decay_mode) {
   if (kind != kOptAdagrad && kind != kOptAdam) return false;
   const int64_t n_vec4 = n / 4;  // buffers are padded to 16 bytes
   if (n_vec4 <= 0) return true;
   int64_t blocks = (n_vec4 + 255) / 256;
   if (blocks > sm_count * 8) blocks = sm_count * 8;
-  if (kind == kOptAdagrad)
-    dense_opt_kernel<kOptAdagrad><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
-        p32, reinterpret_cast<bf16*>(p16), g32, s0, nullptr, lr_ptr, nullptr, 0.f, 0.f, eps,
-        n_vec4);
-  else
-    dense_opt_kernel<kOptAdam><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
-        p32, reinterpret_cast<bf16*>(p16), g32, s0, s1, lr_ptr, step_ptr, beta1, beta2, eps,
-        n_vec4);
+  const int decay = weight_decay == 0.f ? 0
+                    : weight_decay_mode == kWeightDecayDecoupled ? kDenseDecayDecoupled
+                                                                 : kDenseDecayL2;
+  auto launch = [&](auto kind_c, auto decay_c) {
+    constexpr int K = decltype(kind_c)::value, D = decltype(decay_c)::value;
+    dense_opt_kernel<K, D><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
+        p32, reinterpret_cast<bf16*>(p16), g32, s0, K == kOptAdam ? s1 : nullptr, lr_ptr,
+        K == kOptAdam ? step_ptr : nullptr, K == kOptAdam ? beta1 : 0.f,
+        K == kOptAdam ? beta2 : 0.f, eps, weight_decay, n_vec4);
+  };
+  auto with_decay = [&](auto kind_c) {
+    if (decay == kDenseDecayDecoupled)
+      launch(kind_c, std::integral_constant<int, kDenseDecayDecoupled>{});
+    else if (decay == kDenseDecayL2)
+      launch(kind_c, std::integral_constant<int, kDenseDecayL2>{});
+    else
+      launch(kind_c, std::integral_constant<int, 0>{});
+  };
+  if (kind == kOptAdagrad) with_decay(std::integral_constant<int, kOptAdagrad>{});
+  else with_decay(std::integral_constant<int, kOptAdam>{});
   return true;
 }
 

@@ -88,6 +88,10 @@ __global__ void finish_segments_kernel(int64_t* seg_start, const int64_t* n_uniq
 constexpr int kRowDecay = 1;  // weight decay on: the row pass reads the weights (s * g + wd * w)
 constexpr int kRowAdam = 2;   // row-wise Adam (kind kOptRowwiseAdam)
 constexpr int kRowFtrl = 4;   // FTRL-Proximal (kind kOptFtrl): no row pass, its own apply_update
+// decoupled (AdamW-style) weight decay: apply_update scales the weight by 1 - lr * weight_decay
+// before the step, and the gradient, the state and the row pass never see the decay (the row pass
+// reads no weights)
+constexpr int kRowDecoupled = 8;
 
 // Adam bias corrections from a device-resident step count (the host scalars baked into a captured
 // CUDA graph would freeze at their capture-time values).
@@ -138,7 +142,15 @@ __device__ __forceinline__ void apply_update(const TableDesc& T, const Optimizer
   TabT* w = reinterpret_cast<TabT*>(T.weight) + row * T.width + col;
   FVec<VEC> wv = ld_tab_rw<TabT, VEC>(w);
   FVec<VEC> gv = g;
-  if (opt.weight_decay != 0.f) gv.fma(opt.weight_decay, wv);
+  if constexpr ((kRow & kRowDecoupled) != 0) {
+    // w = (1 - lr wd) w, then the kind's step from the undecayed g: torch.optim.AdamW's order.
+    // fmaf and __fmul_rn fix the roundings (no contraction into the step's subtraction).
+    const float keep = fmaf(-opt.lr, opt.weight_decay, 1.f);
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) wv.v[i] = __fmul_rn(wv.v[i], keep);
+  } else {
+    if (opt.weight_decay != 0.f) gv.fma(opt.weight_decay, wv);
+  }
   if constexpr ((kRow & kRowFtrl) != 0) {
     if (opt.lr == 0.f) return;
     StateT* n = reinterpret_cast<StateT*>(T.state0) + row * T.width + col;
@@ -636,13 +648,27 @@ int grid_cap(int64_t work_warps, int sm_count, int per_sm) {
 // kRow).  Only Adagrad, Adam, row-wise Adam and FTRL read element-wise state, so every other
 // optimizer takes the fp32-state kernels; row-wise Adam (kRowAdam) and FTRL (kRowFtrl) have
 // kernels of their own; only the row-wise optimizers with weight decay read the weights in their
-// row pass (kRowDecay); the emit path never touches the table, so one fp32-table instantiation
-// serves every storage type.
+// row pass (kRowDecay); decoupled decay of the stateful kinds takes kRowDecoupled (SGD's
+// decoupled update is its L2 update, so it stays on the plain kernels); the emit path never
+// touches the table, so one fp32-table instantiation serves every storage type.
 template <typename F>
 void with_update_types(const OptimizerArgs& opt, int table_dtype, int state_dtype, F&& f) {
   using Plain = std::integral_constant<int, 0>;
+  const bool decoupled = opt.weight_decay_mode == kWeightDecayDecoupled &&
+                         opt.weight_decay != 0.f && opt.kind != kOptSGD &&
+                         opt.kind != kOptEmit && opt.kind != kOptFtrl;
   with_dtype(opt.kind == kOptEmit ? 0 : table_dtype, [&](auto tab) {
-    if (opt.kind == kOptFtrl) {
+    if (decoupled) {
+      // Adagrad / Adam with fp32 or bf16 state; row-wise Adagrad and row-wise Adam (fp32 or bf16
+      // m) without a weight read in their row pass
+      const bool half = state_dtype == 1 && opt.kind != kOptRowwiseAdagrad;
+      with_type_if<__nv_bfloat16, float>(half, [&](auto state) {
+        if (opt.kind == kOptRowwiseAdam)
+          f(tab, state, std::integral_constant<int, kRowAdam | kRowDecoupled>{});
+        else
+          f(tab, state, std::integral_constant<int, kRowDecoupled>{});
+      });
+    } else if (opt.kind == kOptFtrl) {
       with_type_if<__nv_bfloat16, float>(state_dtype == 1, [&](auto state) {
         f(tab, state, std::integral_constant<int, kRowFtrl>{});
       });

@@ -29,7 +29,7 @@ from ..ops import embedding_lookup_ops as elo
 from ..ops.ragged import RaggedIds, SparseIds
 from ..utils import initializers
 from .comm import dist_ready
-from .embedding_optimizers import OPTIMIZERS, check_state_dtype
+from .embedding_optimizers import OPTIMIZERS, check_state_dtype, check_weight_decay_mode
 from .strategy import DistEmbeddingStrategy, STRATEGIES, suggest_column_slice_threshold
 
 
@@ -626,6 +626,11 @@ class DistributedEmbedding(nn.Module):
       least one id of the step touched (a row whose ids carry only zero gradients included).  The
       optimizers are lazy: rows no id touched, and their state, do not move.  Row-wise Adagrad
       accumulates, and row-wise Adam averages into v, the mean square of this decayed gradient.
+    - ``weight_decay_mode``: ``"l2"`` (default, the above) or ``"decoupled"`` (AdamW-style): the
+      gradient and the optimizer state never see the decay; each touched row is scaled by
+      ``1 - lr * weight_decay`` once per step and then takes the optimizer's step,
+      ``w = (1 - lr * weight_decay) * w - lr * u``.  The same for SGD as ``"l2"``; FTRL
+      rejects it (use its ``l2`` / ``l2_shrinkage``).
     - ``deterministic``: SGD only (default False).  False sends SGD without weight decay through
       one atomic scatter of the gradient rows into the tables; True, or any weight decay, takes
       the sorted update, which sums each row's gradient before it applies it.
@@ -643,13 +648,15 @@ class DistributedEmbedding(nn.Module):
       raise ValueError("state_dtype=torch.bfloat16 is not supported with offload_cache_size: the "
                        "HBM row cache keeps optimizer state rows as fp32 words")
     cfg = {"kind": kind, "lr": float(lr), "eps": entry.eps,
-           "beta1": 0.9, "beta2": 0.999, "weight_decay": 0.0, "initial_accumulator_value": 0.1,
+           "beta1": 0.9, "beta2": 0.999, "weight_decay": 0.0, "weight_decay_mode": "l2",
+           "initial_accumulator_value": 0.1,
            "deterministic": kind != "sgd", "step": 0, "state_dtype": state_dtype, **entry.hyper}
     unknown = sorted(set(kwargs) - set(cfg))
     if unknown:
       raise ValueError(f"unknown fused optimizer argument(s) {unknown}; the known ones are "
                        f"{sorted(set(cfg) - {'kind', 'lr'})}")
     cfg.update(kwargs)
+    check_weight_decay_mode(kind, cfg["weight_decay_mode"])
     if entry.check is not None:
       entry.check(cfg)
     self._fused_optimizer = cfg

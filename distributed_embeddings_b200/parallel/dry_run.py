@@ -35,7 +35,7 @@ from ..ops._native import (GRAD_ROUTE, INPUT_DESC, MAX_PEERS, OPT_ADAGRAD, OPT_A
                            OPT_FTRL, OPT_ROWWISE_ADAGRAD, OPT_ROWWISE_ADAM, OPT_SGD, TABLE_DESC)
 from ..ops.stochastic_rounding import STREAM_STATE0, STREAM_STATE1, stochastic_round
 from . import fused as _fused
-from .embedding_optimizers import BY_CODE
+from .embedding_optimizers import BY_CODE, decay_keep
 
 
 class DryWorld:
@@ -505,8 +505,15 @@ class DryOps:
                      keys, items, seg, n_unique, kind, lr, eps, beta1, beta2, bias1, bias2,
                      grad_scale, weight_decay, lr_ptr, emit_keys, emit_rows, max_width, act_dtype,
                      vec4, scratch, step_ptr, table_dtype=0, state_dtype=0, lr_power=-0.5,
-                     l1=0.0, l2=0.0, l2_shrinkage=0.0, ftrl_beta=0.0):
+                     l1=0.0, l2=0.0, l2_shrinkage=0.0, ftrl_beta=0.0, weight_decay_mode=0):
     self._count("segment_update")
+    # decoupled decay (weight_decay_mode 1, never SGD or FTRL): the row is scaled by the kernels'
+    # fp32 1 - lr * weight_decay first, and the gradient, the state and the row words never see
+    # the decay (SGD's decoupled update is its L2 update: it launches in mode 0)
+    assert int(weight_decay_mode) in (0, 1), weight_decay_mode
+    decoupled = int(weight_decay_mode) == 1 and weight_decay != 0 and \
+        kind not in (OPT_SGD, OPT_EMIT)
+    assert not (decoupled and kind == OPT_FTRL), "decoupled weight decay does not apply to FTRL"
     tdt = self._ADT[int(table_dtype)]
     tsz = 4 if int(table_dtype) == 0 else 2
     # Adagrad / Adam / FTRL state and row-wise Adam's m in bf16: widened to fp32 for the update,
@@ -575,7 +582,9 @@ class DryOps:
       if tsz == 2:
         # 16-bit table: fp32 math on an fp32 copy of the row, stochastic rounding back
         w16, wt = wt, wt.float()
-      if weight_decay:
+      if decoupled:
+        wt.mul_(decay_keep(lr, weight_decay))  # one fp32 rounding, before the step
+      elif weight_decay:
         g = g + weight_decay * wt
       if kind == OPT_SGD:
         wt -= lr * g

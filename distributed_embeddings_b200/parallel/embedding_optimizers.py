@@ -9,6 +9,7 @@ from __future__ import annotations
 
 from typing import Any, Callable, Dict, List, Mapping, NamedTuple, Optional, Tuple
 
+import numpy as np
 import torch
 
 from ..ops import _native
@@ -68,6 +69,43 @@ OPTIMIZERS: Dict[str, EmbeddingOptimizer] = {o.name: o for o in (
 )}
 NAMES = tuple(OPTIMIZERS)
 BY_CODE = {o.code: o for o in OPTIMIZERS.values()}
+
+
+# How ``weight_decay`` (lambda) applies, with ``weight_decay_mode``:
+# - "l2": lambda * w joins the summed, scaled gradient of a touched row before the optimizer sees
+#   it, so Adagrad and Adam divide it by their adaptive denominators;
+# - "decoupled" (AdamW-style, FBGEMM's WeightDecayMode.DECOUPLE): the gradient and the state never
+#   see it; a touched row is first scaled by 1 - lr * lambda, then the kind's step is applied:
+#   w = (1 - lr * lambda) * w - lr * u.  SGD's update is the same in both modes.  FTRL has no
+#   decoupled mode: its weight is a closed form of z (use its l2 / l2_shrinkage).
+WEIGHT_DECAY_MODES = ("l2", "decoupled")
+WEIGHT_DECAY_MODE_CODE = {"l2": 0, "decoupled": 1}  # weight_decay_mode of the native ops
+
+
+def check_weight_decay_mode(kind: str, mode: Any) -> str:
+  """Validate ``weight_decay_mode`` for optimizer ``kind`` ("sgd" ... "ftrl"); returns it."""
+  if mode not in WEIGHT_DECAY_MODES:
+    raise ValueError(f"weight_decay_mode must be one of {', '.join(WEIGHT_DECAY_MODES)}, "
+                     f"got {mode!r}")
+  if mode == "decoupled" and kind == "ftrl":
+    raise ValueError("weight_decay_mode='decoupled' does not apply to ftrl: its weight is a closed "
+                     "form of z; use its l2 / l2_shrinkage (or weight_decay_mode='l2')")
+  return mode
+
+
+def decoupled_decay(kind: str, cfg: Mapping[str, Any]) -> bool:
+  """Whether an update of ``kind`` with ``cfg`` runs the decoupled kernels: decoupled mode, a
+  nonzero decay, and a kind other than SGD (whose decoupled update is its L2 update)."""
+  return cfg.get("weight_decay_mode", "l2") == "decoupled" and \
+      float(cfg.get("weight_decay", 0.0)) != 0.0 and kind != "sgd"
+
+
+def decay_keep(lr: float, weight_decay: float) -> float:
+  """The factor 1 - lr * weight_decay of a decoupled update as the kernels form it, one fp32 fma
+  of the fp32 lr and decay: the product is exact in float64, and the difference is rounded to
+  float64 and then to fp32 (the fma's result unless the float64 value is an exact fp32 tie)."""
+  lr32, wd32 = np.float32(lr), np.float32(weight_decay)
+  return float(np.float32(1.0 - float(lr32) * float(wd32)))
 
 
 def check_state_dtype(kind: str, state_dtype: torch.dtype) -> torch.dtype:

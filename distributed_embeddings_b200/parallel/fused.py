@@ -46,7 +46,8 @@ from ..ops._native import DTYPE_CODE, GRAD_ROUTE, INPUT_DESC, TABLE_DESC
 from ..ops.ragged import RaggedIds
 from ..utils import nvtx
 from .comm import CH_BARRIER0, CH_CONSUMED, CH_GRAD, CH_IDS, CH_OUT, CommContext
-from .embedding_optimizers import OPTIMIZERS, state_slots
+from .embedding_optimizers import (OPTIMIZERS, WEIGHT_DECAY_MODE_CODE, decoupled_decay,
+                                   state_slots)
 from .offload_cache import OffloadCache, split_budget
 
 _COMB = {None: 0, "sum": 0, "mean": 1}
@@ -1159,8 +1160,9 @@ class FusedEngine:
 
   def _atomic_sgd(self) -> bool:
     """The SGD update is one atomic scatter of the gradient rows into the tables.  Not with
-    weight decay: the scatter adds each id's gradient on its own, so with duplicate ids it could
-    not apply the decay exactly once per row; SGD with decay takes the sorted update."""
+    weight decay in either mode: the scatter adds each id's gradient on its own, so with
+    duplicate ids it could not apply the decay exactly once per row; SGD with decay takes the
+    sorted update."""
     opt = self.de._fused_optimizer
     return opt is not None and opt["kind"] == "sgd" and not opt.get("deterministic", False) and \
         opt.get("weight_decay", 0.0) == 0.0 and not self.has_offload and self.tab == 0
@@ -1266,6 +1268,10 @@ class FusedEngine:
       # a dry update has no decay either: weight_decay * w would move the weights and feed the
       # Adagrad accumulators on every warm-up pass
       wd = 0.0 if self._dry_updates else opt["weight_decay"]
+      # decoupled decay (AdamW-style) takes kernels of its own; the default L2 launch keeps its
+      # arguments.  SGD's decoupled update is its L2 update.
+      mode = {"weight_decay_mode": WEIGHT_DECAY_MODE_CODE["decoupled"]} \
+          if wd and decoupled_decay(entry.name, opt) else {}
       ops.segment_update(self.mpdesc, self.tdesc, n_mp, B, B, self.recv_width, self.recv_ptr,
                          keys, items, seg, n_unique, entry.code, opt["lr"],
                          opt["eps"], opt["beta1"], opt["beta2"], 1.0, 1.0, gscale,
@@ -1274,7 +1280,7 @@ class FusedEngine:
                          self.tab, DTYPE_CODE[self.state_dtype],
                          # FTRL's hyperparameters trail the op's arguments (the other kinds
                          # launch without them)
-                         *(opt[k] for k in entry.hyper))
+                         *(opt[k] for k in entry.hyper), **mode)
       if multi:
         ops.sync_only(self._sync(signal=CH_CONSUMED))
       return [None] * n_mp

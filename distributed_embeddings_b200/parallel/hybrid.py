@@ -22,7 +22,8 @@ from ..ops.stochastic_rounding import (HALF_DTYPES, STREAM_STATE0, STREAM_STATE1
                                        stochastic_round)
 from .comm import CommContext, dist_ready
 from .dist_model_parallel import _is_mp, broadcast_variables
-from .embedding_optimizers import OPTIMIZERS, check_state_dtype, state_slots
+from .embedding_optimizers import (OPTIMIZERS, check_state_dtype, check_weight_decay_mode,
+                                   decay_keep, state_slots)
 
 
 def _world(group=None) -> int:
@@ -271,15 +272,21 @@ class SparseRowOptimizer:
   ``state_dtype=torch.bfloat16`` stores the Adagrad accumulator / Adam moments / row-wise Adam's
   m / FTRL's n and z in bf16 like the fused back end: the touched rows' state is widened to fp32,
   the update runs in fp32 with the unrounded new state, and the state is stored with stochastic
-  rounding (streams 1 and 2).  Row-wise state (one word per row) stays fp32."""
+  rounding (streams 1 and 2).  Row-wise state (one word per row) stays fp32.
+
+  ``weight_decay_mode``: ``"l2"`` (default) adds ``weight_decay * w`` to the gradient;
+  ``"decoupled"`` scales each touched row by the fp32 ``1 - lr * weight_decay`` first and applies
+  the step of the undecayed gradient, as :meth:`DistributedEmbedding.set_optimizer` describes."""
 
   def __init__(self, params: Sequence[nn.Parameter], kind: str = "sgd", lr: float = 0.01,
                eps: Optional[float] = None, beta1: float = 0.9, beta2: float = 0.999,
                initial_accumulator_value: float = 0.1, weight_decay: float = 0.0,
-               state_dtype: torch.dtype = torch.float32, **ftrl):
+               state_dtype: torch.dtype = torch.float32, weight_decay_mode: str = "l2",
+               **ftrl):
     kind = kind.lower()
     if kind not in OPTIMIZERS:
       raise ValueError(f"Unsupported optimizer {kind}")
+    self.weight_decay_mode = check_weight_decay_mode(kind, weight_decay_mode)
     entry = OPTIMIZERS[kind]
     unknown = sorted(set(ftrl) - set(entry.hyper))
     if unknown:
@@ -323,7 +330,10 @@ class SparseRowOptimizer:
         continue  # rows and state keep their bits
       cdt = torch.promote_types(p.dtype, torch.float32)
       w, val = p[idx].to(cdt), val.to(cdt)
-      if self.weight_decay:
+      if self.weight_decay and self.weight_decay_mode == "decoupled" and self.kind != "sgd":
+        # (1 - lr wd) w in one rounding of the compute dtype, then the undecayed step
+        w = w * torch.tensor(decay_keep(self.lr, self.weight_decay), dtype=cdt)
+      elif self.weight_decay:
         val = val + self.weight_decay * w
       w, new_state = self._update(w, val, [s[idx].to(cdt) for s in st])
       self._store(p, idx, w, STREAM_WEIGHT)

@@ -78,6 +78,12 @@ def parse():
   p.add_argument("--optimizer_state_dtype", default="fp32", choices=["fp32", "bf16"],
                  help="storage of the Adagrad / Adam / FTRL state (row-wise Adam: its m) of the "
                       "model-parallel tables (bf16: half the memory, stochastically rounded)")
+  p.add_argument("--weight_decay", type=float, default=0.0,
+                 help="weight decay of the embedding and the dense optimizer (rows a step "
+                      "touched / every dense parameter)")
+  p.add_argument("--weight_decay_mode", default="l2", choices=["l2", "decoupled"],
+                 help="l2: added to the gradient; decoupled: AdamW-style, the weights are scaled "
+                      "by 1 - lr * weight_decay before the step (not with ftrl)")
   p.add_argument("--warmup_steps", type=int, default=8000)
   p.add_argument("--decay_start_step", type=int, default=48000)
   p.add_argument("--decay_steps", type=int, default=24000)
@@ -148,6 +154,11 @@ def main():
   de.broadcast_variables(model)
   fast = args.fast and cuda and args.dp_input
   opt_kwargs = {"state_dtype": STATE_DTYPES[args.optimizer_state_dtype]}
+  dense_kwargs = {}
+  if args.weight_decay:
+    decay = {"weight_decay": args.weight_decay, "weight_decay_mode": args.weight_decay_mode}
+    opt_kwargs.update(decay)
+    dense_kwargs.update(decay)
   if args.eval_interval > 0 and not fast:
     raise SystemExit("--eval_interval needs the hand-scheduled step: --fast with --dp_input on "
                      "a GPU")
@@ -155,7 +166,8 @@ def main():
     from distributed_embeddings_b200.models.dlrm_fast import DLRMTrainStep
     trainer = DLRMTrainStep(model, lr=args.learning_rate, scheduler=sched,
                             embedding_optimizer=args.embedding_optimizer,
-                            embedding_optimizer_kwargs=opt_kwargs)
+                            embedding_optimizer_kwargs=opt_kwargs,
+                            dense_optimizer_kwargs=dense_kwargs)
     if args.interaction == "dcnv2":  # list of [b, h_f] ids
       step = lambda n, c, l: trainer.step(n, [x.to(torch.int32) for x in c], l)
     else:
@@ -163,7 +175,8 @@ def main():
   else:
     trainer = HybridTrainer(model, lr=args.learning_rate, scheduler=sched,
                             embedding_optimizer=args.embedding_optimizer,
-                            embedding_optimizer_kwargs=opt_kwargs)
+                            embedding_optimizer_kwargs=opt_kwargs,
+                            dense_optimizer_kwargs=dense_kwargs)
     step = trainer.step
 
   def batches():
