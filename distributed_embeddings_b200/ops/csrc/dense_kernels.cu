@@ -49,10 +49,10 @@ __device__ __forceinline__ void mma_bf16(float (&c)[4], const uint32_t (&a)[4], 
 
 constexpr int kMaxFeat = 32;     // rows of F incl. the bottom-MLP vector, padded to 32
 constexpr int kWarps = 4;        // samples in flight per block
-
-__host__ __device__ constexpr int fwd_warp_bytes(int d) {
-  return (kMaxFeat * (d + 8) * 2 > kMaxFeat * 33 * 4) ? kMaxFeat * (d + 8) * 2 : kMaxFeat * 33 * 4;
-}
+// Samples in flight per block of interact_bwd_apply_kernel (one 139.8 KB block per SM at n_emb
+// 26).  At the step's shapes with 10 applied tables it beats 3 blocks x 4 warps and 5 x 2 per SM
+// (DESIGN §8); the backward without the update is fastest at kWarps.
+constexpr int kApplyWarps = 8;
 
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)),
@@ -63,9 +63,9 @@ __device__ __forceinline__ void cp_async_wait_all() {
   asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
 }
 
-// Stage F = [bottom ; emb_0 .. emb_{n-1}] (each D bf16) of one sample into smem [32][LD] with
+// Stage F = [bottom ; emb_0 .. emb_{n-1}] (each D bf16) of one sample into rows 0..n_emb of sF with
 // cp.async (LDGSTS): every 16-byte chunk of the sample is in flight before the first wait.
-// Pad rows (> n_emb) are zeroed once by the caller.
+// Rows past n_emb are not touched: v1 zeroes them once, the forward reads a zero row instead.
 template <int D>
 __device__ __forceinline__ void stage_features(bf16* sF, int LD, const bf16* bottom,
                                                const bf16* emb, int n_emb, int lane) {
@@ -89,6 +89,18 @@ __device__ __forceinline__ void zero_pad_rows(bf16* sF, int LD, int n_emb, int l
   }
 }
 
+// Shared memory of the forward: the triangle table (C offset i * 33 + j of every z column
+// idx = i (i - 1) / 2 + j < n_inter), the zero row, then per warp the nf staged rows of F.  After
+// the MMAs, C = F F^T ([32][33] fp32) overwrites F from row 1 on; row 0, the bottom vector that
+// z also carries, stays.
+constexpr int kFwdTriBytes = kMaxFeat * (kMaxFeat - 1) / 2 * 2;  // 496 uint16, 16-byte multiple
+__host__ __device__ constexpr int fwd_head_bytes(int d) { return kFwdTriBytes + (d + 8) * 2; }
+__host__ __device__ constexpr int fwd_warp_bytes(int d, int n_emb) {
+  return ((n_emb + 1) * (d + 8) * 2 > (d + 8) * 2 + kMaxFeat * 33 * 4)
+             ? (n_emb + 1) * (d + 8) * 2
+             : (d + 8) * 2 + kMaxFeat * 33 * 4;
+}
+
 // z[s] = [ tril(F F^T, -1) (row major) | bottom | 0 pad ]
 template <int D>
 __global__ void __launch_bounds__(kWarps * 32)
@@ -98,31 +110,53 @@ interact_fwd_kernel(const bf16* __restrict__ bottom, int64_t bottom_stride,
                     const __grid_constant__ SyncArgs sync) {
   sync_head(sync);  // every owner's pooled rows have landed in this rank's embedding output
   constexpr int LD = D + 8;
-  constexpr int kWarpBytes = fwd_warp_bytes(D);
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  bf16* sF = reinterpret_cast<bf16*>(smem_raw + warp * kWarpBytes);
-  float* sC = reinterpret_cast<float*>(sF);  // reused after the MMAs: [32][33] fp32 (4.2 KB)
   const int nf = n_emb + 1;
   const int n_inter = nf * (nf - 1) / 2;
+  uint16_t* sTri = reinterpret_cast<uint16_t*>(smem_raw);
+  bf16* sZero = reinterpret_cast<bf16*>(smem_raw + kFwdTriBytes);
+  bf16* sF = reinterpret_cast<bf16*>(smem_raw + fwd_head_bytes(D) +
+                                     warp * fwd_warp_bytes(D, n_emb));
+  float* sC = reinterpret_cast<float*>(sF + LD);  // C after the MMAs, behind row 0
+  for (int idx = threadIdx.x; idx < n_inter; idx += blockDim.x) {
+    int i = static_cast<int>((1.0f + sqrtf(1.0f + 8.0f * idx)) * 0.5f);
+    while (i * (i - 1) / 2 > idx) --i;
+    while ((i + 1) * i / 2 <= idx) ++i;
+    sTri[idx] = static_cast<uint16_t>(i * 33 + idx - i * (i - 1) / 2);
+  }
+  for (int c = threadIdx.x; c < LD; c += blockDim.x) sZero[c] = __float2bfloat16_rn(0.f);
+  __syncthreads();
+  // operand rows >= nf read the zero row
+  const int arow = lane & 15, brow = (lane & 7) + ((lane >> 4) << 3);
+  const bf16* pa0 = arow < nf ? sF + arow * LD : sZero;
+  const bf16* pa1 = 16 + arow < nf ? sF + (16 + arow) * LD : sZero;
+  const bf16* pb0 = brow < nf ? sF + brow * LD : sZero;
+  const bf16* pb1 = 16 + brow < nf ? sF + (16 + brow) * LD : sZero;
+  // element e of a z row: triangle, bottom (row 0 of F), zero pad
+  auto z_elem = [&](int e) -> bf16 {
+    if (e < n_inter) return __float2bfloat16_rn(sC[sTri[e]]);
+    if (e < n_inter + D) return sF[e - n_inter];
+    return __float2bfloat16_rn(0.f);
+  };
+  const bool vec = ((reinterpret_cast<uintptr_t>(z) & 15) | (z_stride & 7)) == 0;
+  const int n_vec = vec ? z_width >> 3 : 0;  // 16-byte chunks per row; the rest is stored scalar
 
   for (int64_t s = static_cast<int64_t>(blockIdx.x) * kWarps + warp; s < batch;
        s += static_cast<int64_t>(gridDim.x) * kWarps) {
-    const bf16* bp = bottom + s * bottom_stride;
-    zero_pad_rows<D>(sF, LD, n_emb, lane);  // the C staging below may alias the pad rows
-    stage_features<D>(sF, LD, bp, emb + s * emb_stride, n_emb, lane);
+    stage_features<D>(sF, LD, bottom + s * bottom_stride, emb + s * emb_stride, n_emb, lane);
     __syncwarp();
     // lower triangle tiles: m-tile 0 x n-tiles {0,1}; m-tile 1 x n-tiles {0..3}
     float acc0[2][4] = {}, acc1[4][4] = {};
 #pragma unroll
     for (int k = 0; k < D; k += 16) {
       uint32_t a0[4], a1[4], b01[4], b23[4];
-      const int arow = lane & 15, acol = k + ((lane >> 4) << 3);
-      ldmatrix_x4(a0, smem_u32(sF + arow * LD + acol));
-      ldmatrix_x4(a1, smem_u32(sF + (16 + arow) * LD + acol));
-      const int brow = (lane & 7) + ((lane >> 4) << 3), bcol = k + (((lane >> 3) & 1) << 3);
-      ldmatrix_x4(b01, smem_u32(sF + brow * LD + bcol));         // n-tiles 0,1 (rows 0..15)
-      ldmatrix_x4(b23, smem_u32(sF + (16 + brow) * LD + bcol));  // n-tiles 2,3 (rows 16..31)
+      const int acol = k + ((lane >> 4) << 3);
+      ldmatrix_x4(a0, smem_u32(pa0 + acol));
+      ldmatrix_x4(a1, smem_u32(pa1 + acol));
+      const int bcol = k + (((lane >> 3) & 1) << 3);
+      ldmatrix_x4(b01, smem_u32(pb0 + bcol));  // n-tiles 0,1 (rows 0..15)
+      ldmatrix_x4(b23, smem_u32(pb1 + bcol));  // n-tiles 2,3 (rows 16..31)
       mma_bf16(acc0[0], a0, b01[0], b01[1]);
       mma_bf16(acc0[1], a0, b01[2], b01[3]);
       mma_bf16(acc1[0], a1, b01[0], b01[1]);
@@ -148,16 +182,15 @@ interact_fwd_kernel(const bf16* __restrict__ bottom, int64_t bottom_stride,
     }
     __syncwarp();
     bf16* zp = z + s * z_stride;
-    // strict lower triangle in row-major order: idx = i*(i-1)/2 + j
-    for (int idx = lane; idx < n_inter; idx += 32) {
-      int i = static_cast<int>((1.0f + sqrtf(1.0f + 8.0f * idx)) * 0.5f);
-      while (i * (i - 1) / 2 > idx) --i;
-      while ((i + 1) * i / 2 <= idx) ++i;
-      const int j = idx - i * (i - 1) / 2;
-      zp[idx] = __float2bfloat16_rn(sC[i * 33 + j]);
+    for (int c = lane; c < n_vec; c += 32) {
+      uint32_t w[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        w[k] = static_cast<uint32_t>(__bfloat16_as_ushort(z_elem(c * 8 + 2 * k))) |
+               (static_cast<uint32_t>(__bfloat16_as_ushort(z_elem(c * 8 + 2 * k + 1))) << 16);
+      *reinterpret_cast<uint4*>(zp + c * 8) = make_uint4(w[0], w[1], w[2], w[3]);
     }
-    for (int c = lane; c < D; c += 32) zp[n_inter + c] = bp[c];
-    for (int c = n_inter + D + lane; c < z_width; c += 32) zp[c] = __float2bfloat16_rn(0.f);
+    for (int e = n_vec * 8 + lane; e < z_width; e += 32) zp[e] = z_elem(e);
     __syncwarp();
   }
   sync_tail(sync);
@@ -259,7 +292,10 @@ interact_bwd_kernel(const bf16* __restrict__ bottom, int64_t bottom_stride,
 // warps active - a warp loads a sample, waits, computes, stores, and only then touches the next
 // sample.  v2 keeps the *next* sample's features and dz row in flight (cp.async into a second
 // buffer) while the current one is multiplied and stored, and reads dz from shared memory
-// (16-byte chunks) instead of 351 scalar global loads.  8 warps/SM x 8 KB in flight each.
+// (16-byte chunks) instead of 351 scalar global loads.  Only the nf = n_emb + 1 rows of F are
+// staged; the MMA operand rows >= nf read one shared zero row, and the G fragments are gathered
+// straight from the staged dz through a per-block offset table, so a warp holds ~16.4 KB at
+// n_emb 26, dim 128: three 4-warp blocks of v2 fit on an SM.
 __device__ __forceinline__ void cp_async_commit() {
   asm volatile("cp.async.commit_group;" ::: "memory");
 }
@@ -268,7 +304,21 @@ __device__ __forceinline__ void cp_async_wait_group() {
   asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
 
-constexpr int kDzMax = 512;  // staged dz elements per sample (n_inter + D <= 512)
+constexpr int kDzMax = 512;        // staged dz elements per sample (n_inter + D <= 512)
+constexpr int kDzBuf = kDzMax + 8;  // + one zero chunk: element kDzMax reads as 0 (G's sentinel)
+
+// Shared memory of the v2 backward, in this order: the G offset table (4 x 32 uint4: 8 dz
+// offsets per lane per entry), the zero row, the applied / routed feature lists, the per-warp
+// double buffers (2 x [nf][D + 8] F rows, 2 x kDzBuf dz), the chunk routing table.
+constexpr int kBwdGOffBytes = 4 * 32 * 16;
+constexpr int kBwdListBytes = 64;
+__host__ __device__ constexpr int bwd_zero_row_bytes(int d) { return (d + 8) * 2; }
+__host__ __device__ constexpr int bwd_head_bytes(int d) {
+  return kBwdGOffBytes + bwd_zero_row_bytes(d) + kBwdListBytes;
+}
+__host__ __device__ constexpr int bwd_warp_bytes(int d, int n_emb) {
+  return (2 * (n_emb + 1) * (d + 8) + 2 * kDzBuf) * 2;
+}
 
 template <int D>
 __device__ __forceinline__ void issue_sample(bf16* sF, int LD, bf16* sDz, const bf16* bottom,
@@ -299,7 +349,7 @@ __device__ __forceinline__ void prefetch_l2(const void* p) {
 
 // APPLY: rows of F flagged in `apply.mask` are reduced into their table rows (SGD) instead of
 // being stored through the routes; the routed rows are unchanged.
-template <int D, bool APPLY>
+template <int D, int W, bool APPLY>
 __device__ __forceinline__ void
 interact_bwd_v2_body(const bf16* __restrict__ bottom, int64_t bottom_stride,
                      const bf16* __restrict__ emb, int64_t emb_stride, int n_emb,
@@ -309,23 +359,24 @@ interact_bwd_v2_body(const bf16* __restrict__ bottom, int64_t bottom_stride,
                      int n_routes, const SyncArgs& sync, uint32_t* __restrict__ done_counters,
                      int chunk_rows, const InteractApply& apply) {
   constexpr int LD = D + 8;
-  constexpr int LDG = 40;
-  constexpr int kWarpElems = 2 * kMaxFeat * LD + 2 * kDzMax + kMaxFeat * LDG;
   constexpr int kRowChunks = D / 8;  // 16-byte chunks per feature row
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  bf16* base = reinterpret_cast<bf16*>(smem_raw) + warp * kWarpElems;
-  bf16* sDz0 = base + 2 * kMaxFeat * LD;
-  bf16* sG = sDz0 + 2 * kDzMax;
-  ChunkDst* sDst = reinterpret_cast<ChunkDst*>(reinterpret_cast<bf16*>(smem_raw) +
-                                               kWarps * kWarpElems);
   const int nf = n_emb + 1;
   const int n_inter = nf * (nf - 1) / 2;
   const int dz_chunks = (n_inter + D + 7) >> 3;
-  const int n_chunks = n_emb * kRowChunks;
+  uint4* sGOff = reinterpret_cast<uint4*>(smem_raw);  // [4][32]
+  bf16* sZero = reinterpret_cast<bf16*>(smem_raw + kBwdGOffBytes);
+  uint8_t* sRouted = smem_raw + kBwdGOffBytes + bwd_zero_row_bytes(D);  // [32]
+  uint8_t* sApplied = sRouted + 32;                                      // [32]
+  const int warp_elems = bwd_warp_bytes(D, n_emb) / 2;
+  bf16* base = reinterpret_cast<bf16*>(smem_raw + bwd_head_bytes(D)) + warp * warp_elems;
+  bf16* sDz0 = base + 2 * nf * LD;
+  ChunkDst* sDst = reinterpret_cast<ChunkDst*>(smem_raw + bwd_head_bytes(D) +
+                                               W * bwd_warp_bytes(D, n_emb));
   // chunk routing table (all chunks are covered: the host checks that the pieces tile the row)
   if (routes == nullptr) {
-    for (int c = threadIdx.x; c < n_chunks; c += blockDim.x) {
+    for (int c = threadIdx.x; c < n_emb * kRowChunks; c += blockDim.x) {
       sDst[c].base = reinterpret_cast<unsigned long long>(demb + c * 8);
       sDst[c].stride = demb_stride * 2;
     }
@@ -340,96 +391,120 @@ interact_bwd_v2_body(const bf16* __restrict__ bottom, int64_t bottom_stride,
       }
     }
   }
-  zero_pad_rows<D>(base, LD, n_emb, lane);
-  zero_pad_rows<D>(base + kMaxFeat * LD, LD, n_emb, lane);
+  // G offset table: A fragment register r (m-tile mt, k-step ks, 8x8 matrix q) of lane l holds
+  // G[i][j], G[i][j + 1] with i = 16 mt + 8 (q & 1) + l / 4, j = 16 ks + 8 (q >> 1) + 2 (l % 4),
+  // the layout ldmatrix_x4 produces.  G_ij = dz[idx(max, min)]; diagonal and pad entries point at
+  // the zero element kDzMax of the dz buffer.
+  for (int e = threadIdx.x; e < 4 * 32 * 8; e += blockDim.x) {
+    const int l = e & 31, slot = e >> 5;  // slot = 2 * r + h, r = (mt * 2 + ks) * 4 + q
+    const int h = slot & 1, r = slot >> 1, q = r & 3, ks = (r >> 2) & 1, mt = r >> 3;
+    const int i = mt * 16 + (q & 1) * 8 + (l >> 2);
+    const int j = ks * 16 + (q >> 1) * 8 + 2 * (l & 3) + h;
+    const int hi = i > j ? i : j, lo = i > j ? j : i;
+    const int off = (i == j || hi >= nf) ? kDzMax : hi * (hi - 1) / 2 + lo;
+    reinterpret_cast<uint16_t*>(sGOff)[((slot >> 3) * 32 + l) * 8 + (slot & 7)] =
+        static_cast<uint16_t>(off);
+  }
+  for (int c = threadIdx.x; c < LD; c += blockDim.x) sZero[c] = __float2bfloat16_rn(0.f);
+  if (threadIdx.x == 0) {
+    int na = 0, nr = 0;
+    for (int f = 0; f < n_emb; ++f) {
+      if (APPLY && ((apply.mask >> f) & 1u)) sApplied[na++] = static_cast<uint8_t>(f);
+      else sRouted[nr++] = static_cast<uint8_t>(f);
+    }
+  }
+  if (lane < 2)  // the zero chunk behind each of the warp's two dz buffers
+    *reinterpret_cast<uint4*>(sDz0 + lane * kDzBuf + kDzMax) = make_uint4(0, 0, 0, 0);
   __syncthreads();
+  const int n_applied = APPLY ? __popc(apply.mask) : 0;
+  const int n_routed_chunks = (n_emb - n_applied) * kRowChunks;
 
-  // APPLY: lane f holds the table row id of feature f for the current / next sample (-1: not
-  // applied or out of range)
+  // APPLY: lane f holds the fp32 table row that feature f of the current / next sample reduces
+  // into (0: not applied or id out of range)
   float apply_scale = 0.f;
-  long long id_cur = -1, id_next = -1;
+  unsigned long long row_cur = 0, row_next = 0;
   if constexpr (APPLY) {
     apply_scale = apply.scale;
     if (apply.scale_ptr != nullptr) apply_scale *= *apply.scale_ptr;
   }
-  auto load_id = [&](int64_t smp) -> long long {
+  auto load_row = [&](int64_t smp) -> unsigned long long {
     if (lane < n_emb && ((apply.mask >> lane) & 1u)) {
       const long long raw = apply.ids64 ? static_cast<const int64_t*>(apply.ids[lane])[smp]
                                         : static_cast<const int32_t*>(apply.ids[lane])[smp];
       const long long id = raw + apply.id_shift[lane];
       if (static_cast<unsigned long long>(id) < static_cast<unsigned long long>(apply.sub_rows[lane]))
-        return id;
+        return reinterpret_cast<unsigned long long>(apply.table[lane] +
+                                                    (apply.row_base[lane] + id) * D);
     }
-    return -1;
+    return 0;
   };
   // the row this lane's feature reduces into: have it resident in L2 when the REDs arrive
-  auto prefetch_row = [&](long long id) {
-    if (id >= 0) {
-      const char* row = reinterpret_cast<const char*>(apply.table[lane] +
-                                                      (apply.row_base[lane] + id) * D);
+  auto prefetch_row = [&](unsigned long long row) {
+    if (row != 0) {
 #pragma unroll
-      for (int l = 0; l < D * 4 / 128; ++l) prefetch_l2(row + (l << 7));
+      for (int l = 0; l < D * 4 / 128; ++l)
+        prefetch_l2(reinterpret_cast<const char*>(row) + (l << 7));
     }
   };
 
-  const int64_t stride = static_cast<int64_t>(gridDim.x) * kWarps;
-  int64_t s = static_cast<int64_t>(blockIdx.x) * kWarps + warp;
+  const int64_t stride = static_cast<int64_t>(gridDim.x) * W;
+  int64_t s = static_cast<int64_t>(blockIdx.x) * W + warp;
   int cur = 0;
   if (s < batch) {
     issue_sample<D>(base, LD, sDz0, bottom + s * bottom_stride, emb + s * emb_stride,
                     dz + s * dz_stride, n_emb, dz_chunks, lane);
     if constexpr (APPLY) {
-      id_cur = load_id(s);
-      prefetch_row(id_cur);
+      row_cur = load_row(s);
+      prefetch_row(row_cur);
     }
   }
   cp_async_commit();
   for (; s < batch; s += stride, cur ^= 1) {
     const int64_t nxt = s + stride;
     if (nxt < batch) {
-      issue_sample<D>(base + (cur ^ 1) * (kMaxFeat * LD), LD, sDz0 + (cur ^ 1) * kDzMax,
+      issue_sample<D>(base + (cur ^ 1) * (nf * LD), LD, sDz0 + (cur ^ 1) * kDzBuf,
                       bottom + nxt * bottom_stride, emb + nxt * emb_stride, dz + nxt * dz_stride,
                       n_emb, dz_chunks, lane);
-      if constexpr (APPLY) id_next = load_id(nxt);  // consumed after this sample's MMAs
+      if constexpr (APPLY) row_next = load_row(nxt);  // consumed after this sample's MMAs
     } else if constexpr (APPLY) {
-      id_next = -1;
+      row_next = 0;
     }
     cp_async_commit();        // possibly empty: keeps the group arithmetic uniform
     cp_async_wait_group<1>();  // everything but the prefetch just issued has landed
     __syncwarp();
-    bf16* sF = base + cur * (kMaxFeat * LD);
-    const bf16* sDz = sDz0 + cur * kDzMax;
-    for (int c = lane; c < kMaxFeat * LDG / 8; c += 32)
-      reinterpret_cast<uint4*>(sG)[c] = make_uint4(0, 0, 0, 0);
-    __syncwarp();
-    for (int idx = lane; idx < n_inter; idx += 32) {
-      int i = static_cast<int>((1.0f + sqrtf(1.0f + 8.0f * idx)) * 0.5f);
-      while (i * (i - 1) / 2 > idx) --i;
-      while ((i + 1) * i / 2 <= idx) ++i;
-      const int j = idx - i * (i - 1) / 2;
-      const bf16 v = sDz[idx];
-      sG[i * LDG + j] = v;
-      sG[j * LDG + i] = v;
-    }
-    __syncwarp();
+    bf16* sF = base + cur * (nf * LD);
+    const bf16* sDz = sDz0 + cur * kDzBuf;
+    // A = G (32x32): 2 m-tiles x 2 k-steps, gathered from dz
     uint32_t ga[2][2][4];
 #pragma unroll
-    for (int mt = 0; mt < 2; ++mt)
+    for (int g = 0; g < 4; ++g) {
+      const uint4 o = sGOff[g * 32 + lane];
+      const uint32_t w[4] = {o.x, o.y, o.z, o.w};
 #pragma unroll
-      for (int ks = 0; ks < 2; ++ks)
-        ldmatrix_x4(ga[mt][ks],
-                    smem_u32(sG + (mt * 16 + (lane & 15)) * LDG + ks * 16 + ((lane >> 4) << 3)));
+      for (int k = 0; k < 4; ++k) {
+        const int r = g * 4 + k;
+        const uint32_t lo = reinterpret_cast<const uint16_t*>(sDz)[w[k] & 0xffffu];
+        const uint32_t hi = reinterpret_cast<const uint16_t*>(sDz)[w[k] >> 16];
+        ga[r >> 3][(r >> 2) & 1][r & 3] = lo | (hi << 16);
+      }
+    }
     const int cr = lane >> 2, cc = (lane & 3) << 1;
+    // B = F as K x N row major -> transposed loads; K rows >= nf read the zero row
+    const bf16* brow[2];
+#pragma unroll
+    for (int ks = 0; ks < 2; ++ks) {
+      const int krow = ks * 16 + (lane & 7) + (((lane >> 3) & 1) << 3);
+      brow[ks] = krow < nf ? sF + krow * LD : sZero;
+    }
 #pragma unroll 1
     for (int n0 = 0; n0 < D; n0 += 32) {
       float acc[2][4][4] = {};
 #pragma unroll
       for (int ks = 0; ks < 2; ++ks) {
         uint32_t b01[4], b23[4];
-        const int krow = ks * 16 + (lane & 7) + (((lane >> 3) & 1) << 3);
         const int ncol = n0 + ((lane >> 4) << 3);
-        ldmatrix_x4_trans(b01, smem_u32(sF + krow * LD + ncol));
-        ldmatrix_x4_trans(b23, smem_u32(sF + krow * LD + ncol + 16));
+        ldmatrix_x4_trans(b01, smem_u32(brow[ks] + ncol));
+        ldmatrix_x4_trans(b23, smem_u32(brow[ks] + ncol + 16));
 #pragma unroll
         for (int mt = 0; mt < 2; ++mt) {
           mma_bf16(acc[mt][0], ga[mt][ks], b01[0], b01[1]);
@@ -464,50 +539,38 @@ interact_bwd_v2_body(const bf16* __restrict__ bottom, int64_t bottom_stride,
       }
     }
     __syncwarp();
-    if constexpr (APPLY) prefetch_row(id_next);
-    // coalesced 16-byte copy-out: row 0 -> bottom-MLP gradient, rows 1.. -> the chunk's owner
+    if constexpr (APPLY) prefetch_row(row_next);
+    // coalesced 16-byte copy-out: row 0 -> bottom-MLP gradient, routed rows -> the chunk's owner
     // (local buffer, or a peer's receive buffer over NVLink: 128-256 contiguous bytes per piece)
     if (lane < kRowChunks)
       *reinterpret_cast<uint4*>(dbottom + s * dbottom_stride + lane * 8) =
           *reinterpret_cast<const uint4*>(sF + lane * 8);
+    for (int c = lane; c < n_routed_chunks; c += 32) {
+      const int f = sRouted[c / kRowChunks], ch = c % kRowChunks;
+      const ChunkDst d = sDst[f * kRowChunks + ch];
+      *reinterpret_cast<uint4*>(d.base + static_cast<unsigned long long>(s * d.stride)) =
+          *reinterpret_cast<const uint4*>(sF + (f + 1) * LD + ch * 8);
+    }
     if constexpr (APPLY) {
-      // applied rows: the bf16 gradient the routed store would write, widened and scaled like
-      // the scatter's (bf16 -> fp32, * scale), reduced into the table row
-      for (int c0 = 0; c0 < n_chunks; c0 += 32) {
-        const int c = c0 + lane;
-        const int f = c / kRowChunks, ch = c - f * kRowChunks;
-        const long long id = __shfl_sync(0xffffffffu, id_cur, f & 31);
-        if (c >= n_chunks) continue;
-        const uint4 v = *reinterpret_cast<const uint4*>(sF + (f + 1) * LD + ch * 8);
-        if ((apply.mask >> f) & 1u) {
-          if (id >= 0) {
-            const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&v);
-            FVec<4> lo, hi;
-#pragma unroll
-            for (int k = 0; k < 2; ++k) {
-              const float2 a = __bfloat1622float2(h[k]), b = __bfloat1622float2(h[k + 2]);
-              lo.v[2 * k] = a.x * apply_scale;
-              lo.v[2 * k + 1] = a.y * apply_scale;
-              hi.v[2 * k] = b.x * apply_scale;
-              hi.v[2 * k + 1] = b.y * apply_scale;
-            }
-            float* dst = apply.table[f] + (apply.row_base[f] + id) * D + ch * 8;
-            red_add_f32<4>(dst, lo);
-            red_add_f32<4>(dst + 4, hi);
-          }
-        } else {
-          const ChunkDst d = sDst[c];
-          *reinterpret_cast<uint4*>(d.base + static_cast<unsigned long long>(s * d.stride)) = v;
-        }
+      // applied rows, one warp instruction per row: lane l reduces floats [4l, 4l + 4) of the bf16
+      // gradient the routed store would write, widened and scaled like the scatter's
+      // (bf16 -> fp32, * scale), so every 32-byte sector of the table row gets one request
+      static_assert(D == 128, "one red.v4 per lane covers a 128-wide row");
+      for (int k = 0; k < n_applied; ++k) {
+        const int f = sApplied[k];
+        const unsigned long long row = __shfl_sync(0xffffffffu, row_cur, f);
+        if (row == 0) continue;
+        const uint2 v = *reinterpret_cast<const uint2*>(sF + (f + 1) * LD + lane * 4);
+        const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&v.x));
+        const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&v.y));
+        FVec<4> x;
+        x.v[0] = a.x * apply_scale;
+        x.v[1] = a.y * apply_scale;
+        x.v[2] = b.x * apply_scale;
+        x.v[3] = b.y * apply_scale;
+        red_add_f32<4>(reinterpret_cast<float*>(row) + lane * 4, x);
       }
-      id_cur = id_next;
-    } else {
-      for (int c = lane; c < n_chunks; c += 32) {
-        const int row = 1 + c / kRowChunks, ch = c - (row - 1) * kRowChunks;
-        const ChunkDst d = sDst[c];
-        *reinterpret_cast<uint4*>(d.base + static_cast<unsigned long long>(s * d.stride)) =
-            *reinterpret_cast<const uint4*>(sF + row * LD + ch * 8);
-      }
+      row_cur = row_next;
     }
     __syncwarp();  // all lanes are done with buffer `cur` before the next iteration refills it
     if (done_counters != nullptr && lane == 0) {
@@ -530,7 +593,7 @@ interact_bwd_v2_kernel(const bf16* __restrict__ bottom, int64_t bottom_stride,
                        const GradRoute* __restrict__ routes, int n_routes,
                        const __grid_constant__ SyncArgs sync, uint32_t* __restrict__ done_counters,
                        int chunk_rows) {
-  interact_bwd_v2_body<D, false>(bottom, bottom_stride, emb, emb_stride, n_emb, dz, dz_stride,
+  interact_bwd_v2_body<D, kWarps, false>(bottom, bottom_stride, emb, emb_stride, n_emb, dz, dz_stride,
                                  dbottom, dbottom_stride, demb, demb_stride, emb_grad_scale, batch,
                                  routes, n_routes, sync, done_counters, chunk_rows,
                                  InteractApply{});
@@ -538,7 +601,7 @@ interact_bwd_v2_kernel(const bf16* __restrict__ bottom, int64_t bottom_stride,
 
 // v2 with the table update of the features in `apply` (single-GPU SGD step)
 template <int D>
-__global__ void __launch_bounds__(kWarps * 32)
+__global__ void __launch_bounds__(kApplyWarps * 32)
 interact_bwd_apply_kernel(const bf16* __restrict__ bottom, int64_t bottom_stride,
                           const bf16* __restrict__ emb, int64_t emb_stride, int n_emb,
                           const bf16* __restrict__ dz, int64_t dz_stride,
@@ -547,7 +610,7 @@ interact_bwd_apply_kernel(const bf16* __restrict__ bottom, int64_t bottom_stride
                           int64_t batch, const GradRoute* __restrict__ routes, int n_routes,
                           const __grid_constant__ SyncArgs sync,
                           const __grid_constant__ InteractApply apply) {
-  interact_bwd_v2_body<D, true>(bottom, bottom_stride, emb, emb_stride, n_emb, dz, dz_stride,
+  interact_bwd_v2_body<D, kApplyWarps, true>(bottom, bottom_stride, emb, emb_stride, n_emb, dz, dz_stride,
                                 dbottom, dbottom_stride, demb, demb_stride, emb_grad_scale, batch,
                                 routes, n_routes, sync, nullptr, 0, apply);
 }
@@ -1080,14 +1143,17 @@ bool launch_interact_fwd(const void* bottom, int64_t bottom_stride, const void* 
                          int z_width, int64_t batch, int sm_count, cudaStream_t stream,
                          const SyncArgs& sync) {
   if (n_emb + 1 > kMaxFeat || batch <= 0) return false;
-  int64_t blocks = (batch + kWarps - 1) / kWarps;
-  const int64_t cap = static_cast<int64_t>(sm_count) * 8;
-  if (blocks > cap) blocks = cap;
 #define DE_IFWD(DD)                                                                              \
   {                                                                                              \
-    const size_t smem = kWarps * fwd_warp_bytes(DD);                                             \
+    const int smem = fwd_head_bytes(DD) + kWarps * fwd_warp_bytes(DD, n_emb);                   \
     cudaFuncSetAttribute(interact_fwd_kernel<DD>, cudaFuncAttributeMaxDynamicSharedMemorySize,   \
-                         static_cast<int>(smem));                                                \
+                         smem);                                                                  \
+    int per_sm = 0;                                                                              \
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, interact_fwd_kernel<DD>, kWarps * 32, \
+                                                  smem);                                         \
+    int64_t blocks = (batch + kWarps - 1) / kWarps;                                              \
+    const int64_t cap = static_cast<int64_t>(sm_count) * (per_sm > 0 ? per_sm : 1);              \
+    if (blocks > cap) blocks = cap;                                                              \
     interact_fwd_kernel<DD><<<static_cast<unsigned>(blocks), kWarps * 32, smem, stream>>>(       \
         reinterpret_cast<const bf16*>(bottom), bottom_stride, reinterpret_cast<const bf16*>(emb), \
         emb_stride, n_emb, reinterpret_cast<bf16*>(z), z_stride, z_width, batch, sync);          \
@@ -1132,26 +1198,28 @@ bool launch_interact_bwd(const void* bottom, int64_t bottom_stride, const void* 
   const bool has_sync = sync.state != nullptr && (sync.wait_ch >= 0 || sync.signal_ch >= 0);
   if (v2_ok &&
       (!force_v1 || routes != nullptr || has_sync || done_counters != nullptr || applied)) {
-    // two resident blocks per SM, each warp streams its samples through a double buffer
-    int64_t blocks2 = (batch + kWarps - 1) / kWarps;
-    if (blocks2 > static_cast<int64_t>(sm_count) * 2) blocks2 = static_cast<int64_t>(sm_count) * 2;
-#define DE_IBWD2(KERNEL, DD, ...)                                                                \
+    // as many resident blocks per SM as the shared memory of n_emb allows, each warp streams its
+    // samples through a double buffer
+#define DE_IBWD2(KERNEL, DD, W, ...)                                                             \
   {                                                                                              \
-    const size_t smem =                                                                          \
-        kWarps * (2 * kMaxFeat * (DD + 8) + 2 * kDzMax + kMaxFeat * 40) * sizeof(bf16) +         \
-        static_cast<size_t>(n_emb) * (DD / 8) * sizeof(ChunkDst);                                \
-    cudaFuncSetAttribute(KERNEL<DD>, cudaFuncAttributeMaxDynamicSharedMemorySize,                \
-                         static_cast<int>(smem));                                                \
-    KERNEL<DD><<<static_cast<unsigned>(blocks2), kWarps * 32, smem, stream>>>(                   \
+    const int smem = bwd_head_bytes(DD) + W * bwd_warp_bytes(DD, n_emb) +                        \
+                     n_emb * (DD / 8) * static_cast<int>(sizeof(ChunkDst));                      \
+    cudaFuncSetAttribute(KERNEL<DD>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);         \
+    int per_sm = 0;                                                                              \
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, KERNEL<DD>, W * 32, smem);            \
+    int64_t blocks2 = (batch + W - 1) / W;                                                       \
+    const int64_t cap2 = static_cast<int64_t>(sm_count) * (per_sm > 0 ? per_sm : 1);             \
+    if (blocks2 > cap2) blocks2 = cap2;                                                          \
+    KERNEL<DD><<<static_cast<unsigned>(blocks2), W * 32, smem, stream>>>(                        \
         reinterpret_cast<const bf16*>(bottom), bottom_stride, reinterpret_cast<const bf16*>(emb), \
         emb_stride, n_emb, reinterpret_cast<const bf16*>(dz), dz_stride,                         \
         reinterpret_cast<bf16*>(dbottom), dbottom_stride, reinterpret_cast<bf16*>(demb),         \
         demb_stride, emb_grad_scale, batch, routes, n_routes, sync, __VA_ARGS__);                \
     return true;                                                                                 \
   }
-    if (applied) DE_IBWD2(interact_bwd_apply_kernel, 128, *apply)
-    if (dim == 128) DE_IBWD2(interact_bwd_v2_kernel, 128, done_counters, chunk_rows)
-    if (dim == 64) DE_IBWD2(interact_bwd_v2_kernel, 64, done_counters, chunk_rows)
+    if (applied) DE_IBWD2(interact_bwd_apply_kernel, 128, kApplyWarps, *apply)
+    if (dim == 128) DE_IBWD2(interact_bwd_v2_kernel, 128, kWarps, done_counters, chunk_rows)
+    if (dim == 64) DE_IBWD2(interact_bwd_v2_kernel, 64, kWarps, done_counters, chunk_rows)
 #undef DE_IBWD2
   }
   if (has_sync) return false;
