@@ -1,5 +1,5 @@
-"""Dense optimizer of the trainers: SGD, Adagrad or Adam on the data-parallel parameters (the MLPs
-and any replicated embedding tables).
+"""Dense optimizer of the trainers: SGD, Adagrad, Adam or momentum SGD on the data-parallel
+parameters (the MLPs and any replicated embedding tables).
 
 The reference applies one optimizer to every trainable variable; ``dense_optimizer`` lets the
 trainers do the same.  The math is that of the fused embedding update (``apply_update`` in
@@ -10,14 +10,19 @@ trainers do the same.  The math is that of the fused embedding update (``apply_u
   ``initial_accumulator_value=0.1``);
 * Adam: ``m = b1 m + (1 - b1) g; v = b2 v + (1 - b2) g^2;
   p -= lr * (m / (1 - b1^t)) / (sqrt(v / (1 - b2^t)) + eps)`` (``beta1=0.9``, ``beta2=0.999``,
-  ``eps=1e-8``).
+  ``eps=1e-8``);
+* momentum SGD (``torch.optim.SGD``, dampening 0): ``b = mu b + g; p -= lr * b``, or with
+  ``nesterov`` ``p -= lr * (mu b + g)`` (``momentum=0.9``, ``nesterov=False``), each step one
+  fp32 fma in this order.
 
 Every kind takes ``weight_decay`` (lambda, default 0) and ``weight_decay_mode``: ``"l2"``
 (default) adds ``lambda * p`` to the gradient before the update; ``"decoupled"`` (AdamW-style)
 first scales ``p`` by the fp32 ``1 - lr * lambda`` and then applies the step of the undecayed
-gradient, ``p = (1 - lr * lambda) * p - lr * u``.  SGD's update is ``p -= lr * (g + lambda * p)``
-in both modes.  Unlike the lazy embedding optimizers, the decay applies to every dense element
-(MLP weights, biases, replicated tables) on every step; pad elements of the flat buffers stay 0.
+gradient, ``p = (1 - lr * lambda) * p - lr * u`` (momentum SGD's L2 decay passes through the
+buffer, as ``torch.optim.SGD``'s ``weight_decay`` does).  SGD's update is
+``p -= lr * (g + lambda * p)`` in both modes.  Unlike the lazy embedding optimizers, the decay
+applies to every dense element (MLP weights, biases, replicated tables) on every step; pad elements
+of the flat buffers stay 0.
 
 The learning rate is the trainer's device-resident ``lr_t`` word and Adam's step count ``t`` is a
 device-resident fp32 word advanced inside the step, so both follow a scheduler under CUDA-graph
@@ -25,8 +30,8 @@ replay.
 
 Checkpoints have one format for every trainer: ``{"kind", "step", "slots"}`` where ``slots`` maps
 each dense parameter name (``model.named_parameters()``) to its state tensors shaped like the
-parameter (Adagrad ``[acc]``, Adam ``[m, v]``, SGD none) and ``step`` is Adam's ``t`` (0 for the
-kinds that keep no step count).
+parameter (Adagrad ``[acc]``, Adam ``[m, v]``, momentum ``[b]``, SGD none) and ``step`` is Adam's
+``t`` (0 for the kinds that keep no step count).
 """
 from __future__ import annotations
 
@@ -35,13 +40,15 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import torch
 from torch import nn
 
-from ..parallel.embedding_optimizers import WEIGHT_DECAY_MODE_CODE, WEIGHT_DECAY_MODES
+from ..parallel.embedding_optimizers import (MOMENTUM_DEFAULTS, WEIGHT_DECAY_MODE_CODE,
+                                              WEIGHT_DECAY_MODES, check_momentum_args)
 
-KINDS = ("sgd", "adagrad", "adam")
+KINDS = ("sgd", "adagrad", "adam", "momentum")
 _DEFAULTS = {
     "sgd": {},
     "adagrad": {"eps": 1e-7, "initial_accumulator_value": 0.1},
     "adam": {"beta1": 0.9, "beta2": 0.999, "eps": 1e-8},
+    "momentum": dict(MOMENTUM_DEFAULTS),
 }
 _DECAY = {"weight_decay": 0.0, "weight_decay_mode": "l2"}  # every kind
 
@@ -60,7 +67,10 @@ def dense_optimizer_config(kind: str, kwargs: Optional[dict] = None) -> dict:
   if mode not in WEIGHT_DECAY_MODES:
     raise ValueError(f"dense optimizer weight_decay_mode must be one of "
                      f"{', '.join(WEIGHT_DECAY_MODES)}, got {mode!r}")
-  cfg.update({k: float(v) for k, v in kwargs.items()})
+  # nesterov stays a bool; every other hyperparameter is a number
+  cfg.update({k: v if k == "nesterov" else float(v) for k, v in kwargs.items()})
+  if kind == "momentum":
+    check_momentum_args(cfg)
   if not cfg["weight_decay"] >= 0.0:
     raise ValueError(f"dense optimizer weight_decay must be >= 0, got {cfg['weight_decay']}")
   cfg["weight_decay_mode"] = mode
@@ -76,9 +86,10 @@ def decay_args(cfg: dict) -> tuple:
 
 
 def slot_init(cfg: dict) -> List[float]:
-  """Initial value of each state slot: Adagrad ``[acc]``, Adam ``[m, v]``, SGD none."""
+  """Initial value of each state slot: Adagrad ``[acc]``, Adam ``[m, v]``, momentum ``[b]``, SGD
+  none."""
   return {"sgd": [], "adagrad": [cfg.get("initial_accumulator_value")],
-          "adam": [0.0, 0.0]}[cfg["kind"]]
+          "adam": [0.0, 0.0], "momentum": [0.0]}[cfg["kind"]]
 
 
 def dense_named_parameters(model: nn.Module) -> List[Tuple[str, nn.Parameter]]:
@@ -97,10 +108,10 @@ def check_state(cfg: dict, state: dict, names: Sequence[str]):
 
 
 class FlatDenseOptimizer:
-  """Adagrad / Adam state laid out like a trainer's flat fp32 master buffer ``p32`` and the fused
-  update over it (``dense_adagrad`` / ``dense_adam``); SGD keeps no state and launches
-  ``dense_sgd``.  Pad elements keep ``g = 0``, so they stay at ``p = 0`` and their state at its
-  initial value."""
+  """Adagrad / Adam / momentum state laid out like a trainer's flat fp32 master buffer ``p32`` and
+  the fused update over it (``dense_adagrad`` / ``dense_adam`` / ``dense_momentum``); SGD keeps no
+  state and launches ``dense_sgd``.  Pad elements keep ``g = 0``, so they stay at ``p = 0`` and
+  their state at its initial value."""
 
   def __init__(self, cfg: dict, p32: torch.Tensor):
     self.cfg = cfg
@@ -118,6 +129,9 @@ class FlatDenseOptimizer:
       ops.dense_sgd(self.p32, p16, g32, lr_t, 1.0, *decay)
     elif self.kind == "adagrad":
       ops.dense_adagrad(self.p32, p16, g32, self.state[0], lr_t, c["eps"], *decay)
+    elif self.kind == "momentum":
+      ops.dense_momentum(self.p32, p16, g32, self.state[0], lr_t, c["momentum"], c["nesterov"],
+                         *decay)
     else:
       self.step_t.add_(1.0)  # device counter: the bias corrections stay right under graph replay
       ops.dense_adam(self.p32, p16, g32, self.state[0], self.state[1], lr_t, self.step_t,

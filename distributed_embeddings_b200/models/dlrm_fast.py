@@ -87,7 +87,7 @@ class _Layer:
 class DLRMTrainStep:
   """Static-schedule training step for :class:`DLRM` on the fused embedding back end.
 
-  ``dense_optimizer`` (``sgd`` | ``adagrad`` | ``adam``, hyperparameters in
+  ``dense_optimizer`` (``sgd`` | ``adagrad`` | ``adam`` | ``momentum``, hyperparameters in
   ``dense_optimizer_kwargs``) updates the MLPs and any replicated tables with the shared
   learning rate.  Replicated tables (``data_parallel_threshold``) need
   ``dense_optimizer == embedding_optimizer``, so the row-wise optimizers and ``ftrl`` need a model
@@ -207,7 +207,7 @@ class DLRMTrainStep:
               "data_parallel_threshold=None (no replicated tables)")
         raise ValueError("replicated tables in the fast step are updated by the dense optimizer "
                          "kernel: use the same embedding_optimizer and dense_optimizer ('sgd', "
-                         "'adagrad' or 'adam') or data_parallel_threshold=None")
+                         "'adagrad', 'adam' or 'momentum') or data_parallel_threshold=None")
       for layer in self.emb.dp_layers:
         w = layer.embeddings
         self._dp_slots.append((pos, tuple(w.shape)))

@@ -43,11 +43,11 @@ from .synthetic import SyntheticModel
 class SyntheticTrainStep:
   """Static-schedule training step for :class:`SyntheticModel` on the fused embedding back end.
 
-  ``dense_optimizer`` (``sgd`` | ``adagrad`` | ``adam``, hyperparameters in
+  ``dense_optimizer`` (``sgd`` | ``adagrad`` | ``adam`` | ``momentum``, hyperparameters in
   ``dense_optimizer_kwargs``) updates the MLP with the shared learning rate; the reference's
   configuration is ``embedding_optimizer="adagrad", dense_optimizer="adagrad"``.
-  ``embedding_optimizer`` is any kind of ``DistributedEmbedding.set_optimizer`` (``ftrl``
-  included), with its hyperparameters in ``embedding_optimizer_kwargs``."""
+  ``embedding_optimizer`` is any kind of ``DistributedEmbedding.set_optimizer`` (``ftrl`` and
+  ``momentum`` included), with its hyperparameters in ``embedding_optimizer_kwargs``."""
 
   def __init__(self, model: SyntheticModel, lr: float = 0.001, embedding_optimizer: str = "adagrad",
                use_cuda_graph: bool = True, embedding_optimizer_kwargs: Optional[dict] = None,

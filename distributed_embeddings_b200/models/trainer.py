@@ -27,15 +27,19 @@ class HybridTrainer:
       (DistributedEmbedding) and ``dense_parameters()``.
     lr: learning rate (dense SGD and fused embedding optimizer share it like the reference).
     embedding_optimizer: ``sgd`` | ``adagrad`` | ``rowwise_adagrad`` | ``adam`` | ``rowwise_adam``
-      | ``ftrl``; its hyperparameters in ``embedding_optimizer_kwargs`` go to both the fused
-      optimizer and the torch back end's :class:`SparseRowOptimizer`.
+      | ``ftrl`` | ``momentum``; its hyperparameters in ``embedding_optimizer_kwargs`` go to both
+      the fused optimizer and the torch back end's :class:`SparseRowOptimizer`.
     scheduler: optional :class:`LearningRateScheduler`.
-    dense_optimizer: ``sgd`` | ``adagrad`` | ``adam`` for the dense parameters (MLPs and
-      replicated tables), hyperparameters in ``dense_optimizer_kwargs`` (see
-      ``models/dense_optimizer.py``), ``weight_decay`` / ``weight_decay_mode`` included;
-      ``momentum`` applies to ``sgd`` only.  Momentum SGD takes L2 decay as
+    dense_optimizer: ``sgd`` | ``adagrad`` | ``adam`` | ``momentum`` for the dense parameters
+      (MLPs and replicated tables), hyperparameters in ``dense_optimizer_kwargs`` (see
+      ``models/dense_optimizer.py``), ``weight_decay`` / ``weight_decay_mode`` included.
+      ``dense_optimizer="momentum"`` (``momentum`` / ``nesterov`` in ``dense_optimizer_kwargs``)
+      is the embedding kind's update on device words, so it follows a scheduler inside a
+      captured CUDA graph, and takes both decay modes.
+    momentum: applies to ``dense_optimizer="sgd"`` only, through ``torch.optim.SGD`` (learning
+      rate on the host: no scheduler inside a captured graph).  It takes L2 decay as
       ``torch.optim.SGD(weight_decay=...)`` does (into the gradient, before the momentum
-      buffer); ``weight_decay_mode="decoupled"`` with momentum raises ``ValueError``.
+      buffer); ``weight_decay_mode="decoupled"`` with it raises ``ValueError``.
   """
 
   def __init__(self, model: nn.Module, lr: float = 24.0, embedding_optimizer: str = "sgd",
@@ -129,7 +133,8 @@ class HybridTrainer:
           p.sub_(g * self.lr_t)
 
   def _adaptive_dense_step(self):
-    """Dense Adagrad / Adam with the expressions of the fused kernels, on device words."""
+    """Dense Adagrad / Adam / momentum with the expressions of the fused kernels, on device
+    words."""
     c, params, grads = self.dense_cfg, self.bucket.params, self.bucket.views
     if not params:
       return
@@ -139,6 +144,14 @@ class HybridTrainer:
         torch._foreach_mul_(params, 1.0 - self.lr_t * c["weight_decay"])
       elif c["weight_decay"]:
         grads = torch._foreach_add(grads, params, alpha=c["weight_decay"])
+      if c["kind"] == "momentum":
+        buf = self.dense_state[0]
+        torch._foreach_mul_(buf, c["momentum"])
+        torch._foreach_add_(buf, grads)
+        step = torch._foreach_add(torch._foreach_mul(buf, c["momentum"]), grads) \
+            if c["nesterov"] else buf
+        torch._foreach_sub_(params, torch._foreach_mul(step, self.lr_t))
+        return
       if c["kind"] == "adagrad":
         acc = self.dense_state[0]
         torch._foreach_addcmul_(acc, grads, grads)

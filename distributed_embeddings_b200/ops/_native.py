@@ -66,6 +66,7 @@ DTYPE_CODE = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
 OPT_SGD, OPT_ADAGRAD, OPT_ROWWISE_ADAGRAD, OPT_ADAM, OPT_EMIT = 0, 1, 2, 3, 4
 OPT_ROWWISE_ADAM = 5
 OPT_FTRL = 6
+OPT_MOMENTUM = 7
 MAX_PEERS = 16
 
 
@@ -111,7 +112,7 @@ _KERNELS_PER_OP = {
     "embedding_lookup_fwd": 1, "embedding_scatter_add": 1, "embedding_lookup_grad": 14,
     "row_to_split": 1, "hash_init": 1, "integer_lookup": 1, "barrier": 1, "allreduce": 1,
     "gather_segments": 1, "gather_ragged": 1, "copy_cast_2d": 1, "dense_sgd": 1, "interact_fwd": 1, "interact_bwd": 1,
-    "dense_adagrad": 1, "dense_adam": 1, "cross_fwd": 1, "cross_bwd": 1, "cross_dx0": 1,
+    "dense_adagrad": 1, "dense_adam": 1, "dense_momentum": 1, "cross_fwd": 1, "cross_bwd": 1, "cross_dx0": 1,
     "relu_bwd_bias": 1, "head_loss": 1, "head_eval": 1, "select_copy": 1, "cast_pad": 1, "gemm_tn_bias_act": 1, "gemm_dgrad_relu_bias": 1,
 }
 _launches = 0

@@ -358,7 +358,8 @@ void segment_update(const Tensor& descs, const Tensor& tables, int64_t n_tables,
                     bool vec4, const c10::optional<Tensor>& scratch, int64_t step_ptr,
                     int64_t table_dtype, int64_t state_dtype, double lr_power = -0.5,
                     double l1 = 0.0, double l2 = 0.0, double l2_shrinkage = 0.0,
-                    double ftrl_beta = 0.0, int64_t weight_decay_mode = de::kWeightDecayL2) {
+                    double ftrl_beta = 0.0, int64_t weight_decay_mode = de::kWeightDecayL2,
+                    double momentum = 0.0, bool nesterov = false) {
   c10::cuda::CUDAGuard guard(descs.device());
   TORCH_CHECK(table_dtype >= 0 && table_dtype <= 2, "table_dtype: 0 fp32, 1 bf16, 2 fp16");
   TORCH_CHECK(state_dtype == 0 || state_dtype == 1, "state_dtype: 0 fp32, 1 bf16");
@@ -385,6 +386,8 @@ void segment_update(const Tensor& descs, const Tensor& tables, int64_t n_tables,
   opt.l2_shrinkage = static_cast<float>(l2_shrinkage);
   opt.ftrl_beta = static_cast<float>(ftrl_beta);
   opt.weight_decay_mode = static_cast<int32_t>(weight_decay_mode);
+  opt.momentum = static_cast<float>(momentum);
+  opt.nesterov = nesterov ? 1 : 0;
   if (opt.kind == de::kOptEmit) TORCH_CHECK(emit_keys.has_value() && emit_rows.has_value());
   // occurrence-balanced path: immune to id skew (needs a zeroed scratch of >= n_items/32 rows)
   if (scratch.has_value() && vec4 && max_width <= 128 && opt.kind != de::kOptEmit) {
@@ -1187,6 +1190,21 @@ void dense_adam(Tensor p32, Tensor p16, Tensor g32, Tensor m, Tensor v, const Te
   check_launch();
 }
 
+// Momentum SGD with buffer b (torch.optim.SGD, dampening 0), the embedding kernels' update
+void dense_momentum(Tensor p32, Tensor p16, Tensor g32, Tensor b, const Tensor& lr,
+                    double momentum, bool nesterov, double weight_decay = 0.0,
+                    int64_t weight_decay_mode = de::kWeightDecayL2) {
+  check_decay_mode(weight_decay_mode);
+  check_dense_opt(p32, p16, g32, {{&b, "b"}}, lr, nullptr);
+  c10::cuda::CUDAGuard guard(p32.device());
+  de::launch_dense_momentum(p32.data_ptr<float>(), p16.data_ptr(), g32.data_ptr<float>(),
+                            b.data_ptr<float>(), lr.data_ptr<float>(),
+                            static_cast<float>(momentum), nesterov, p32.numel(), sm_count(),
+                            cur_stream(), static_cast<float>(weight_decay),
+                            static_cast<int>(weight_decay_mode));
+  check_launch();
+}
+
 void cast_pad(const Tensor& src, Tensor dst) {
   TORCH_CHECK(src.is_cuda() && src.scalar_type() == at::kFloat && src.is_contiguous());
   TORCH_CHECK(dst.scalar_type() == at::kBFloat16 && dst.is_contiguous() &&
@@ -1479,7 +1497,7 @@ TORCH_LIBRARY(de_b200, m) {
       "Tensor? emit_keys, Tensor? emit_rows, int max_width, int act_dtype, bool vec4, "
       "Tensor? scratch, int step_ptr, int table_dtype=0, int state_dtype=0, "
       "float lr_power=-0.5, float l1=0., float l2=0., float l2_shrinkage=0., "
-      "float ftrl_beta=0., int weight_decay_mode=0) -> ()",
+      "float ftrl_beta=0., int weight_decay_mode=0, float momentum=0., bool nesterov=False) -> ()",
       &segment_update);
   m.def(
       "embedding_lookup_fwd(Tensor param, Tensor values, Tensor? offsets, int hotness, int batch, "
@@ -1576,6 +1594,10 @@ TORCH_LIBRARY(de_b200, m) {
       "Tensor lr, Tensor step, float beta1, float beta2, float eps, float weight_decay=0., "
       "int weight_decay_mode=0) -> ()",
       &dense_adam);
+  m.def(
+      "dense_momentum(Tensor(a!) p32, Tensor(b!) p16, Tensor(c!) g32, Tensor(d!) b, Tensor lr, "
+      "float momentum, bool nesterov, float weight_decay=0., int weight_decay_mode=0) -> ()",
+      &dense_momentum);
   m.def("cast_pad(Tensor src, Tensor(a!) dst) -> ()", &cast_pad);
   m.def(
       "gemm_tn_bias_act(Tensor a, Tensor b, Tensor? bias, Tensor(a!) out, bool relu, int block_n) "

@@ -84,13 +84,14 @@ enum OptimizerKind : int32_t {
   kOptEmit = 4,
   kOptRowwiseAdam = 5,  // Adam with element-wise m (state0) and one fp32 v word per row (state1)
   kOptFtrl = 6,         // FTRL-Proximal: accumulator n (state0) and linear term z (state1)
+  kOptMomentum = 7,     // momentum SGD: element-wise momentum buffer b (state0)
 };
 
 // One entry per (fused) local table, used by the sorted/deduplicated update path.
 struct alignas(16) TableDesc {
   void* weight;       // [rows, width]; fp32, bf16 or fp16 (`table_dtype` of the launch)
   void* state0;       // Adagrad accumulator [rows,width] / row-wise [rows] / Adam m / row-wise
-                      // Adam m / FTRL n
+                      // Adam m / FTRL n / momentum b
   void* state1;       // Adam v / row-wise Adam v [rows] / FTRL z  (element-wise state: fp32 or bf16,
                       // `state_dtype` of the launch; row-wise state is always fp32)
   int64_t rows;
@@ -119,6 +120,11 @@ struct OptimizerArgs {
   // kWeightDecayL2: weight_decay * w joins the gradient; kWeightDecayDecoupled (AdamW): the
   // weight is scaled by 1 - lr * weight_decay and the step comes from the undecayed gradient
   int32_t weight_decay_mode;
+  // momentum SGD (kind kOptMomentum; the other kinds ignore them), torch.optim.SGD's buffer:
+  // b = momentum * b + g, then w -= lr * b, or with nesterov w -= lr * (momentum * b + g).
+  // Appended so that the offsets of the fields above stay put.
+  float momentum;
+  int32_t nesterov;
 };
 
 constexpr int kWeightDecayL2 = 0;
@@ -392,6 +398,12 @@ bool launch_dense_opt(int kind, float* p32, void* p16, float* g32, float* s0, fl
                       const float* lr_ptr, const float* step_ptr, float beta1, float beta2,
                       float eps, int64_t n, int sm_count, cudaStream_t stream,
                       float weight_decay = 0.f, int weight_decay_mode = kWeightDecayL2);
+// Fused dense momentum SGD (torch.optim.SGD, dampening 0) with buffer b over n (multiple of 4) fp32
+// elements + bf16 re-cast + gradient zeroing; the update of kOptMomentum in the embedding kernels,
+// with weight_decay in either mode.
+void launch_dense_momentum(float* p32, void* p16, float* g32, float* b, const float* lr_ptr,
+                           float momentum, bool nesterov, int64_t n, int sm_count,
+                           cudaStream_t stream, float weight_decay, int weight_decay_mode);
 void launch_cast_pad(const float* src, int src_cols, void* dst, int dst_cols, int64_t rows,
                      cudaStream_t stream);
 

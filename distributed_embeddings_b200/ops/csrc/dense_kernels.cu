@@ -1063,6 +1063,46 @@ dense_opt_kernel(float* __restrict__ p32, bf16* __restrict__ p16, float* __restr
   }
 }
 
+// Momentum SGD over the flat dense buffers with the expressions of the embedding update
+// (kOptMomentum in apply_update): b = fmaf(mu, b, g), p = fmaf(-lr, b, p) or, NESTEROV,
+// p = fmaf(-lr, fmaf(mu, b, g), p); then p16 = bf16(p32) and g32 = 0.  DECAY as dense_opt_kernel.
+template <int DECAY, bool NESTEROV>
+__device__ __forceinline__ void dense_momentum_elem(float& p, float& b, float g, float neg_lr,
+                                                    float mu, float weight_decay, float keep) {
+  if constexpr (DECAY == kDenseDecayL2) g = fmaf(weight_decay, p, g);
+  if constexpr (DECAY == kDenseDecayDecoupled) p = __fmul_rn(p, keep);
+  b = fmaf(mu, b, g);
+  p = fmaf(neg_lr, NESTEROV ? fmaf(mu, b, g) : b, p);
+}
+
+template <int DECAY, bool NESTEROV>
+__global__ void __launch_bounds__(256)
+dense_momentum_kernel(float* __restrict__ p32, bf16* __restrict__ p16, float* __restrict__ g32,
+                      float* __restrict__ buf, const float* __restrict__ lr_ptr, float mu,
+                      float weight_decay, int64_t n_vec4) {
+  const float lr = *lr_ptr;
+  const float keep = fmaf(-lr, weight_decay, 1.f);  // decoupled decay only
+  const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n_vec4;
+       i += stride) {
+    float4 p = reinterpret_cast<float4*>(p32)[i];
+    const float4 g = reinterpret_cast<const float4*>(g32)[i];
+    float4 b = reinterpret_cast<float4*>(buf)[i];
+    dense_momentum_elem<DECAY, NESTEROV>(p.x, b.x, g.x, -lr, mu, weight_decay, keep);
+    dense_momentum_elem<DECAY, NESTEROV>(p.y, b.y, g.y, -lr, mu, weight_decay, keep);
+    dense_momentum_elem<DECAY, NESTEROV>(p.z, b.z, g.z, -lr, mu, weight_decay, keep);
+    dense_momentum_elem<DECAY, NESTEROV>(p.w, b.w, g.w, -lr, mu, weight_decay, keep);
+    reinterpret_cast<float4*>(p32)[i] = p;
+    reinterpret_cast<float4*>(buf)[i] = b;
+    reinterpret_cast<float4*>(g32)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    __nv_bfloat162 lo = __floats2bfloat162_rn(p.x, p.y), hi = __floats2bfloat162_rn(p.z, p.w);
+    uint2 o;
+    o.x = *reinterpret_cast<uint32_t*>(&lo);
+    o.y = *reinterpret_cast<uint32_t*>(&hi);
+    reinterpret_cast<uint2*>(p16)[i] = o;
+  }
+}
+
 // dst[r, 0:dst_cols] = bf16(src[r, 0:src_cols]) zero padded
 __global__ void cast_pad_kernel(const float* __restrict__ src, int src_cols, bf16* __restrict__ dst,
                                 int dst_cols, int64_t rows) {
@@ -1409,6 +1449,33 @@ bool launch_dense_opt(int kind, float* p32, void* p16, float* g32, float* s0, fl
   if (kind == kOptAdagrad) with_decay(std::integral_constant<int, kOptAdagrad>{});
   else with_decay(std::integral_constant<int, kOptAdam>{});
   return true;
+}
+
+void launch_dense_momentum(float* p32, void* p16, float* g32, float* b, const float* lr_ptr,
+                           float momentum, bool nesterov, int64_t n, int sm_count,
+                           cudaStream_t stream, float weight_decay, int weight_decay_mode) {
+  const int64_t n_vec4 = n / 4;  // buffers are padded to 16 bytes
+  if (n_vec4 <= 0) return;
+  int64_t blocks = (n_vec4 + 255) / 256;
+  if (blocks > sm_count * 8) blocks = sm_count * 8;
+  const int decay = weight_decay == 0.f ? 0
+                    : weight_decay_mode == kWeightDecayDecoupled ? kDenseDecayDecoupled
+                                                                 : kDenseDecayL2;
+  auto launch = [&](auto decay_c, auto nesterov_c) {
+    dense_momentum_kernel<decltype(decay_c)::value, decltype(nesterov_c)::value>
+        <<<static_cast<unsigned>(blocks), 256, 0, stream>>>(
+            p32, reinterpret_cast<bf16*>(p16), g32, b, lr_ptr, momentum, weight_decay, n_vec4);
+  };
+  auto with_nesterov = [&](auto decay_c) {
+    if (nesterov) launch(decay_c, std::true_type{});
+    else launch(decay_c, std::false_type{});
+  };
+  if (decay == kDenseDecayDecoupled)
+    with_nesterov(std::integral_constant<int, kDenseDecayDecoupled>{});
+  else if (decay == kDenseDecayL2)
+    with_nesterov(std::integral_constant<int, kDenseDecayL2>{});
+  else
+    with_nesterov(std::integral_constant<int, 0>{});
 }
 
 void launch_cast_pad(const float* src, int src_cols, void* dst, int dst_cols, int64_t rows,

@@ -92,6 +92,8 @@ constexpr int kRowFtrl = 4;   // FTRL-Proximal (kind kOptFtrl): no row pass, its
 // before the step, and the gradient, the state and the row pass never see the decay (the row pass
 // reads no weights)
 constexpr int kRowDecoupled = 8;
+// momentum SGD (kind kOptMomentum): no row pass, its own apply_update
+constexpr int kRowMomentum = 16;
 
 // Adam bias corrections from a device-resident step count (the host scalars baked into a captured
 // CUDA graph would freeze at their capture-time values).
@@ -135,6 +137,11 @@ __device__ __forceinline__ float ftrl_pow(float n, float lr_power) {
 //   n' = n + g^2,  sigma = (P(n') - P(n)) / lr,  z += g + 2 l2_shrinkage w - sigma w,
 //   w = |z| > l1 ? (sign(z) l1 - z) / ((beta + P(n')) / lr + 2 l2) : 0,  n = n'.
 // At lr = 0 the row, n and z keep their bits (sigma would divide by zero).
+//
+// Momentum SGD (torch.optim.SGD, dampening 0), g the decayed gradient, b the buffer (state0):
+//   b = fmaf(momentum, b, g);  w = fmaf(-lr, b, w),
+//   nesterov: w = fmaf(-lr, fmaf(momentum, b, g), w).
+// At momentum 0 both give SGD's fmaf(-lr, g, w) bit for bit.
 template <typename TabT, int VEC, typename StateT = float, int kRow = 0>
 __device__ __forceinline__ void apply_update(const TableDesc& T, const OptimizerArgs& opt,
                                              int64_t row, int col, const FVec<VEC>& g,
@@ -168,6 +175,16 @@ __device__ __forceinline__ void apply_update(const TableDesc& T, const Optimizer
     }
     st_tab<StateT, VEC>(n, nv, step, T.key_base + row, col, kStreamState0);
     st_tab<StateT, VEC>(z, zv, step, T.key_base + row, col, kStreamState1);
+  } else if constexpr ((kRow & kRowMomentum) != 0) {
+    StateT* b = reinterpret_cast<StateT*>(T.state0) + row * T.width + col;
+    FVec<VEC> bv = ld_tab_rw<StateT, VEC>(b);
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) {
+      bv.v[i] = fmaf(opt.momentum, bv.v[i], gv.v[i]);
+      const float u = opt.nesterov ? fmaf(opt.momentum, bv.v[i], gv.v[i]) : bv.v[i];
+      wv.v[i] = fmaf(-opt.lr, u, wv.v[i]);
+    }
+    st_tab<StateT, VEC>(b, bv, step, T.key_base + row, col, kStreamState0);
   } else if constexpr ((kRow & kRowAdam) != 0) {
     // row-wise Adam: m element-wise; row_sumsq_mean carries the row's new v (the caller advanced
     // state1[row])
@@ -312,7 +329,8 @@ __device__ __forceinline__ void segment_update_body(
     const int nvec = (W + VEC - 1) / VEC;
 
     float row_state = 0.f;
-    if (!(kRow & kRowFtrl) && ((kRow & kRowAdam) || opt.kind == kOptRowwiseAdagrad)) {
+    if (!(kRow & (kRowFtrl | kRowMomentum)) &&
+        ((kRow & kRowAdam) || opt.kind == kOptRowwiseAdagrad)) {
       // pass 1: mean of squared (scaled) gradient over the whole row
       float ss = 0.f;
       if (valid) {
@@ -441,14 +459,16 @@ __device__ __forceinline__ int find_table(const TableDesc* __restrict__ tables, 
 }
 
 // Apply the optimizer to one row given the complete (scaled) gradient fragment of this lane.
-// kRow: the row pass of row-wise Adagrad / row-wise Adam, or FTRL (see segment_update_body).
+// kRow: the row pass of row-wise Adagrad / row-wise Adam, or FTRL / momentum (see
+// segment_update_body).
 template <typename TabT, typename StateT, int kRow = 0>
 __device__ __forceinline__ void apply_row(const TableDesc& T, const OptimizerArgs& opt,
                                           int64_t row, int col, FVec<4> g, int lpr,
                                           unsigned group_mask, uint32_t step) {
   const bool col_ok = col < T.width;
   float row_state = 0.f;
-  if (!(kRow & kRowFtrl) && ((kRow & kRowAdam) || opt.kind == kOptRowwiseAdagrad)) {
+  if (!(kRow & (kRowFtrl | kRowMomentum)) &&
+      ((kRow & kRowAdam) || opt.kind == kOptRowwiseAdagrad)) {
     float ss = 0.f;
     if (col_ok) {
       if constexpr ((kRow & kRowDecay) != 0) {
@@ -649,8 +669,9 @@ int grid_cap(int64_t work_warps, int sm_count, int per_sm) {
 // optimizer takes the fp32-state kernels; row-wise Adam (kRowAdam) and FTRL (kRowFtrl) have
 // kernels of their own; only the row-wise optimizers with weight decay read the weights in their
 // row pass (kRowDecay); decoupled decay of the stateful kinds takes kRowDecoupled (SGD's
-// decoupled update is its L2 update, so it stays on the plain kernels); the emit path never
-// touches the table, so one fp32-table instantiation serves every storage type.
+// decoupled update is its L2 update, so it stays on the plain kernels); momentum (kRowMomentum,
+// fp32 or bf16 b, plain or decoupled) has kernels of its own, so the kinds above keep theirs; the
+// emit path never touches the table, so one fp32-table instantiation serves every storage type.
 template <typename F>
 void with_update_types(const OptimizerArgs& opt, int table_dtype, int state_dtype, F&& f) {
   using Plain = std::integral_constant<int, 0>;
@@ -658,7 +679,14 @@ void with_update_types(const OptimizerArgs& opt, int table_dtype, int state_dtyp
                          opt.weight_decay != 0.f && opt.kind != kOptSGD &&
                          opt.kind != kOptEmit && opt.kind != kOptFtrl;
   with_dtype(opt.kind == kOptEmit ? 0 : table_dtype, [&](auto tab) {
-    if (decoupled) {
+    if (opt.kind == kOptMomentum) {
+      with_type_if<__nv_bfloat16, float>(state_dtype == 1, [&](auto state) {
+        if (decoupled)
+          f(tab, state, std::integral_constant<int, kRowMomentum | kRowDecoupled>{});
+        else
+          f(tab, state, std::integral_constant<int, kRowMomentum>{});
+      });
+    } else if (decoupled) {
       // Adagrad / Adam with fp32 or bf16 state; row-wise Adagrad and row-wise Adam (fp32 or bf16
       // m) without a weight read in their row pass
       const bool half = state_dtype == 1 && opt.kind != kOptRowwiseAdagrad;

@@ -596,8 +596,8 @@ class DistributedEmbedding(nn.Module):
   def set_optimizer(self, kind: str = "sgd", lr: float = 0.01, **kwargs):
     """Attach an optimizer that is applied to the model-parallel tables *inside* the backward
     kernels (no sparse gradient is materialised).  ``kind``: ``sgd`` | ``adagrad`` |
-    ``rowwise_adagrad`` | ``adam`` | ``rowwise_adam`` | ``ftrl``.  Only the fused back end
-    consumes it.
+    ``rowwise_adagrad`` | ``adam`` | ``rowwise_adam`` | ``ftrl`` | ``momentum``.  Only the fused
+    back end consumes it.
 
     ``rowwise_adam`` is Adam with an element-wise first moment m and one fp32 second-moment word
     per row: ``v_row = beta2 * v_row + (1 - beta2) * mean_j(g_j^2)``, ``m = beta1 * m +
@@ -612,6 +612,17 @@ class DistributedEmbedding(nn.Module):
     ``n = n'``.  The L1 term sets the rows it applies to exactly to zero.  At ``lr == 0`` (the
     first step of a warm-up schedule) rows and state do not move.
 
+    ``momentum`` is momentum SGD as ``torch.optim.SGD(momentum=mu, nesterov=..., dampening=0)``
+    computes it, with an element-wise buffer b that starts at 0.  For a touched row with gradient
+    g (L2 decay included): ``b = mu * b + g``, then ``w -= lr * b``, or with ``nesterov``
+    ``w -= lr * (mu * b + g)``.  Keras's ``SGD(momentum=mu)`` keeps a velocity ``v = mu * v -
+    lr * g`` instead; at a constant learning rate the two give the same weights (``v = -lr * b``),
+    under a schedule they differ.  The torch form is used because the learning rate is a device
+    word that schedulers change, and because its buffer does not depend on the learning rate, so
+    the state keeps its meaning across checkpoints and learning-rate changes.  Like the other
+    kinds the update is lazy: a row no id touched keeps its weights and buffer.  At
+    ``momentum=0`` the update is SGD's, bit for bit.
+
     Keyword arguments (any other raises ``ValueError``):
 
     - ``eps``: added to the square root in the denominator (default 1e-7, Adam and row-wise Adam 1e-8).
@@ -621,6 +632,7 @@ class DistributedEmbedding(nn.Module):
     - ``lr_power`` (-0.5, at most 0), ``l1``, ``l2``, ``l2_shrinkage``, ``beta`` (0, at least 0):
       FTRL only, Keras's ``learning_rate_power``, ``l1_regularization_strength``,
       ``l2_regularization_strength``, ``l2_shrinkage_regularization_strength`` and ``beta``.
+    - ``momentum`` (0.9, in [0, 1)), ``nesterov`` (False, a bool): ``momentum`` only.
     - ``weight_decay``: L2 decay (default 0).  ``weight_decay * w`` is added to the summed,
       scaled gradient of a row before the optimizer sees it, once per step for every row that at
       least one id of the step touched (a row whose ids carry only zero gradients included).  The
@@ -629,16 +641,18 @@ class DistributedEmbedding(nn.Module):
     - ``weight_decay_mode``: ``"l2"`` (default, the above) or ``"decoupled"`` (AdamW-style): the
       gradient and the optimizer state never see the decay; each touched row is scaled by
       ``1 - lr * weight_decay`` once per step and then takes the optimizer's step,
-      ``w = (1 - lr * weight_decay) * w - lr * u``.  The same for SGD as ``"l2"``; FTRL
-      rejects it (use its ``l2`` / ``l2_shrinkage``).
+      ``w = (1 - lr * weight_decay) * w - lr * u``.  The same for SGD as ``"l2"`` (not for
+      ``momentum``, whose L2 decay passes through the buffer); FTRL rejects it (use its ``l2`` /
+      ``l2_shrinkage``).
     - ``deterministic``: SGD only (default False).  False sends SGD without weight decay through
       one atomic scatter of the gradient rows into the tables; True, or any weight decay, takes
       the sorted update, which sums each row's gradient before it applies it.
     - ``step``: the Adam / row-wise Adam step count to resume from (0).
     - ``state_dtype``: storage of the Adagrad accumulator / Adam moments / row-wise Adam's m
-      (its v stays one fp32 word per row) / FTRL's n and z, ``torch.float32``
-      (default) or ``torch.bfloat16`` (half the bytes; the update runs in fp32 and stores the
-      state with stochastic rounding, see the user guide, "Half-precision optimizer state")."""
+      (its v stays one fp32 word per row) / FTRL's n and z / the momentum buffer,
+      ``torch.float32`` (default) or ``torch.bfloat16`` (half the bytes; the update runs in fp32
+      and stores the state with stochastic rounding, see the user guide, "Half-precision optimizer
+      state")."""
     kind = kind.lower()
     if kind not in OPTIMIZERS:
       raise ValueError(f"Unsupported fused optimizer {kind}")

@@ -32,7 +32,8 @@ import numpy as np
 import torch
 
 from ..ops._native import (GRAD_ROUTE, INPUT_DESC, MAX_PEERS, OPT_ADAGRAD, OPT_ADAM, OPT_EMIT,
-                           OPT_FTRL, OPT_ROWWISE_ADAGRAD, OPT_ROWWISE_ADAM, OPT_SGD, TABLE_DESC)
+                           OPT_FTRL, OPT_MOMENTUM, OPT_ROWWISE_ADAGRAD, OPT_ROWWISE_ADAM, OPT_SGD,
+                           TABLE_DESC)
 from ..ops.stochastic_rounding import STREAM_STATE0, STREAM_STATE1, stochastic_round
 from . import fused as _fused
 from .embedding_optimizers import BY_CODE, decay_keep
@@ -505,7 +506,8 @@ class DryOps:
                      keys, items, seg, n_unique, kind, lr, eps, beta1, beta2, bias1, bias2,
                      grad_scale, weight_decay, lr_ptr, emit_keys, emit_rows, max_width, act_dtype,
                      vec4, scratch, step_ptr, table_dtype=0, state_dtype=0, lr_power=-0.5,
-                     l1=0.0, l2=0.0, l2_shrinkage=0.0, ftrl_beta=0.0, weight_decay_mode=0):
+                     l1=0.0, l2=0.0, l2_shrinkage=0.0, ftrl_beta=0.0, weight_decay_mode=0,
+                     momentum=0.0, nesterov=False):
     self._count("segment_update")
     # decoupled decay (weight_decay_mode 1, never SGD or FTRL): the row is scaled by the kernels'
     # fp32 1 - lr * weight_decay first, and the gradient, the state and the row words never see
@@ -516,9 +518,9 @@ class DryOps:
     assert not (decoupled and kind == OPT_FTRL), "decoupled weight decay does not apply to FTRL"
     tdt = self._ADT[int(table_dtype)]
     tsz = 4 if int(table_dtype) == 0 else 2
-    # Adagrad / Adam / FTRL state and row-wise Adam's m in bf16: widened to fp32 for the update,
-    # stored with stochastic rounding (streams 1 and 2); the other optimizers ignore the code, like
-    # the kernels
+    # Adagrad / Adam / FTRL / momentum state and row-wise Adam's m in bf16: widened to fp32 for the
+    # update, stored with stochastic rounding (streams 1 and 2); the other optimizers ignore the
+    # code, like the kernels
     half_state = int(state_dtype) == 1 and kind in BY_CODE and BY_CODE[kind].elementwise_state
     sdt, ssz = (torch.bfloat16, 2) if half_state else (torch.float32, 4)
 
@@ -632,6 +634,17 @@ class DryOps:
         if half_state:
           n16.copy_(stochastic_round(n, sdt, step, key, stream=STREAM_STATE0))
           z16.copy_(stochastic_round(z, sdt, step, key, stream=STREAM_STATE1))
+      elif kind == OPT_MOMENTUM:
+        # the kernels' fmaf order, each fma one fp32 rounding of the exact float64 value
+        b16, b = state(t["state0"], row, width, "momentum b")
+        mu = torch.tensor(float(np.float32(momentum)), dtype=torch.float64)
+        neg_lr = torch.tensor(-float(np.float32(lr)), dtype=torch.float64)
+        g64 = g.double()
+        b.copy_((mu * b.double() + g64).float())
+        u = (mu * b.double() + g64).float() if nesterov else b
+        wt.copy_((neg_lr * u.double() + wt.double()).float())
+        if half_state:
+          b16.copy_(stochastic_round(b, sdt, step, key, stream=STREAM_STATE0))
       else:
         raise ValueError(f"optimizer kind {kind}")
       if tsz == 2:

@@ -7,6 +7,7 @@ update kernels), its state slots, its defaults, and whether a zero gradient stil
 """
 from __future__ import annotations
 
+import numbers
 from typing import Any, Callable, Dict, List, Mapping, NamedTuple, Optional, Tuple
 
 import numpy as np
@@ -30,6 +31,20 @@ def check_ftrl_args(cfg: Mapping[str, Any]):
       raise ValueError(f"ftrl: {k} must be >= 0, got {cfg[k]}")
 
 
+# Momentum SGD's hyperparameters and their defaults (torch.optim.SGD's ``momentum`` and
+# ``nesterov``, dampening 0), the ``segment_update`` op's arguments of the same names
+MOMENTUM_DEFAULTS = {"momentum": 0.9, "nesterov": False}
+
+
+def check_momentum_args(cfg: Mapping[str, Any]):
+  """``momentum`` in [0, 1) and ``nesterov`` a bool."""
+  mu = cfg["momentum"]
+  if isinstance(mu, bool) or not isinstance(mu, numbers.Real) or not 0.0 <= float(mu) < 1.0:
+    raise ValueError(f"momentum: momentum must be a number in [0, 1), got {mu!r}")
+  if not isinstance(cfg["nesterov"], bool):
+    raise ValueError(f"momentum: nesterov must be a bool, got {cfg['nesterov']!r}")
+
+
 class Slot(NamedTuple):
   """One state slot: one fp32 word per row (``per_row``), else element-wise ``[rows, width]`` in
   the state dtype; it starts at ``initial_accumulator_value`` (``accumulator``) or at 0."""
@@ -42,7 +57,7 @@ class EmbeddingOptimizer(NamedTuple):
   code: int                                 # _native.OPT_*
   slots: Tuple[Slot, ...] = ()              # state0, state1 of the kernels' TableDesc
   eps: float = 1e-7
-  hyper: Mapping[str, float] = {}           # keyword arguments of this kind only, with defaults
+  hyper: Mapping[str, Any] = {}             # keyword arguments of this kind only, with defaults
   check: Optional[Callable[[Mapping[str, Any]], None]] = None  # validates them
   moves_on_zero_grad: bool = False          # a dry (warm-up) update must not run it
 
@@ -66,6 +81,9 @@ OPTIMIZERS: Dict[str, EmbeddingOptimizer] = {o.name: o for o in (
     # accumulator n, linear term z; on a zero gradient the closed form of z sets the weights
     EmbeddingOptimizer("ftrl", _native.OPT_FTRL, (Slot(accumulator=True), Slot()),
                        hyper=FTRL_DEFAULTS, check=check_ftrl_args, moves_on_zero_grad=True),
+    # momentum buffer b; a zero gradient still moves a row by -lr * momentum * b
+    EmbeddingOptimizer("momentum", _native.OPT_MOMENTUM, (Slot(),), hyper=MOMENTUM_DEFAULTS,
+                       check=check_momentum_args, moves_on_zero_grad=True),
 )}
 NAMES = tuple(OPTIMIZERS)
 BY_CODE = {o.code: o for o in OPTIMIZERS.values()}
@@ -76,14 +94,15 @@ BY_CODE = {o.code: o for o in OPTIMIZERS.values()}
 #   it, so Adagrad and Adam divide it by their adaptive denominators;
 # - "decoupled" (AdamW-style, FBGEMM's WeightDecayMode.DECOUPLE): the gradient and the state never
 #   see it; a touched row is first scaled by 1 - lr * lambda, then the kind's step is applied:
-#   w = (1 - lr * lambda) * w - lr * u.  SGD's update is the same in both modes.  FTRL has no
-#   decoupled mode: its weight is a closed form of z (use its l2 / l2_shrinkage).
+#   w = (1 - lr * lambda) * w - lr * u.  SGD's update is the same in both modes (momentum SGD's is
+#   not: its L2 decay passes through the buffer).  FTRL has no decoupled mode: its weight is a
+#   closed form of z (use its l2 / l2_shrinkage).
 WEIGHT_DECAY_MODES = ("l2", "decoupled")
 WEIGHT_DECAY_MODE_CODE = {"l2": 0, "decoupled": 1}  # weight_decay_mode of the native ops
 
 
 def check_weight_decay_mode(kind: str, mode: Any) -> str:
-  """Validate ``weight_decay_mode`` for optimizer ``kind`` ("sgd" ... "ftrl"); returns it."""
+  """Validate ``weight_decay_mode`` for optimizer ``kind`` ("sgd" ... "momentum"); returns it."""
   if mode not in WEIGHT_DECAY_MODES:
     raise ValueError(f"weight_decay_mode must be one of {', '.join(WEIGHT_DECAY_MODES)}, "
                      f"got {mode!r}")

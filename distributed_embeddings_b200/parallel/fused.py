@@ -1278,9 +1278,10 @@ class FusedEngine:
                          wd, self.lr_t.data_ptr(), None, None, self.max_width,
                          self.act, self.vec4, self._balanced_scratch(), self.step_t.data_ptr(),
                          self.tab, DTYPE_CODE[self.state_dtype],
-                         # FTRL's hyperparameters trail the op's arguments (the other kinds
-                         # launch without them)
-                         *(opt[k] for k in entry.hyper), **mode)
+                         # FTRL's and momentum's hyperparameters trail the op's arguments (the
+                         # other kinds launch without them); FTRL's beta is the op's ftrl_beta
+                         **{("ftrl_beta" if k == "beta" else k): opt[k] for k in entry.hyper},
+                         **mode)
       if multi:
         ops.sync_only(self._sync(signal=CH_CONSUMED))
       return [None] * n_mp

@@ -14,6 +14,7 @@ from __future__ import annotations
 
 from typing import Iterable, List, Optional, Sequence
 
+import numpy as np
 import torch
 import torch.distributed as dist
 from torch import nn
@@ -260,9 +261,10 @@ class SparseRowOptimizer:
   tensors - the ``torch`` back end of :class:`DistributedEmbedding`, i.e. the NCCL-collectives
   baseline, which has no fused update.  Same math as the fused kernels
   (``ops/csrc/sparse_update_kernels.cu``): ``sgd`` | ``adagrad`` | ``rowwise_adagrad`` | ``adam``
-  | ``rowwise_adam`` | ``ftrl`` (lazy: only the touched rows advance).  ``ftrl`` takes the
-  keyword arguments of ``DistributedEmbedding.set_optimizer("ftrl")`` (``lr_power``, ``l1``,
-  ``l2``, ``l2_shrinkage``, ``beta``); the other kinds reject them.  Counterpart of the Keras
+  | ``rowwise_adam`` | ``ftrl`` | ``momentum`` (lazy: only the touched rows advance).  ``ftrl``
+  and ``momentum`` take the keyword arguments of their kind in
+  ``DistributedEmbedding.set_optimizer`` (``lr_power``, ``l1``, ``l2``, ``l2_shrinkage``,
+  ``beta``; ``momentum``, ``nesterov``); the other kinds reject them.  Counterpart of the Keras
   sparse-apply kernels the reference relies on (examples/benchmarks/synthetic_models/main.py:96-101).
 
   bf16 / fp16 parameters keep fp32 state; their touched rows are updated in fp32 and written
@@ -270,9 +272,9 @@ class SparseRowOptimizer:
   (``ops/stochastic_rounding.py``).
 
   ``state_dtype=torch.bfloat16`` stores the Adagrad accumulator / Adam moments / row-wise Adam's
-  m / FTRL's n and z in bf16 like the fused back end: the touched rows' state is widened to fp32,
-  the update runs in fp32 with the unrounded new state, and the state is stored with stochastic
-  rounding (streams 1 and 2).  Row-wise state (one word per row) stays fp32.
+  m / FTRL's n and z / the momentum buffer in bf16 like the fused back end: the touched rows'
+  state is widened to fp32, the update runs in fp32 with the unrounded new state, and the state
+  is stored with stochastic rounding (streams 1 and 2).  Row-wise state (one word per row) stays fp32.
 
   ``weight_decay_mode``: ``"l2"`` (default) adds ``weight_decay * w`` to the gradient;
   ``"decoupled"`` scales each touched row by the fp32 ``1 - lr * weight_decay`` first and applies
@@ -282,18 +284,19 @@ class SparseRowOptimizer:
                eps: Optional[float] = None, beta1: float = 0.9, beta2: float = 0.999,
                initial_accumulator_value: float = 0.1, weight_decay: float = 0.0,
                state_dtype: torch.dtype = torch.float32, weight_decay_mode: str = "l2",
-               **ftrl):
+               **hyper):
     kind = kind.lower()
     if kind not in OPTIMIZERS:
       raise ValueError(f"Unsupported optimizer {kind}")
     self.weight_decay_mode = check_weight_decay_mode(kind, weight_decay_mode)
     entry = OPTIMIZERS[kind]
-    unknown = sorted(set(ftrl) - set(entry.hyper))
+    unknown = sorted(set(hyper) - set(entry.hyper))
     if unknown:
       raise ValueError(f"unknown fused optimizer argument(s) {unknown} for {kind}")
-    self.ftrl = dict(entry.hyper, initial_accumulator_value=initial_accumulator_value, **ftrl)
+    # the kind's own hyperparameters (FTRL's, momentum's), defaults filled in
+    self.hyper = dict(entry.hyper, initial_accumulator_value=initial_accumulator_value, **hyper)
     if entry.check is not None:
-      entry.check(self.ftrl)
+      entry.check(self.hyper)
     self.state_dtype = check_state_dtype(kind, state_dtype)
     self.params = [p for p in params if p.requires_grad]
     self.kind, self.lr = kind, float(lr)
@@ -361,13 +364,15 @@ class SparseRowOptimizer:
       m = self.beta1 * state[0] + (1 - self.beta1) * g
       v = self.beta2 * state[1] + (1 - self.beta2) * (g * g).mean(dim=1)
       return w - self.lr * (m / b1) / ((v / b2).sqrt().unsqueeze(1) + self.eps), [m, v]
+    if self.kind == "momentum":
+      return self._momentum(w, g, state[0])
     w, n, z = self._ftrl(w, g, state[0], state[1])
     return w, [n, z]
 
   def _ftrl(self, w, g, n, z):
     """FTRL-Proximal on rows ``w`` with decayed gradient ``g``, accumulator ``n`` and linear term
     ``z`` (lr != 0); returns the new (w, n, z)."""
-    c = self.ftrl
+    c = self.hyper
     pw = (lambda x: x.sqrt()) if c["lr_power"] == -0.5 else (lambda x: x.pow(-c["lr_power"]))
     n_new = n + g * g
     p_new = pw(n_new)
@@ -375,6 +380,17 @@ class SparseRowOptimizer:
     q = (c["beta"] + p_new) / self.lr + 2 * c["l2"]
     w = torch.where(z.abs() > c["l1"], (torch.sign(z) * c["l1"] - z) / q, torch.zeros_like(z))
     return w, n_new, z
+
+  def _momentum(self, w, g, b):
+    """Momentum SGD on rows ``w`` with decayed gradient ``g`` and buffer ``b``, in the kernels'
+    fmaf order (each fma one rounding of its float64 value); returns (w, [b])."""
+    cdt = w.dtype
+    mu = float(np.float32(self.hyper["momentum"]))
+    neg_lr = -float(np.float32(self.lr))
+    fma = lambda a, x, y: (a * x.double() + y.double()).to(cdt)
+    b = fma(mu, b, g)
+    u = fma(mu, b, g) if self.hyper["nesterov"] else b
+    return fma(neg_lr, u, w), [b]
 
   def _store(self, dst, idx, x, stream):
     """Store rows ``x`` at ``idx`` of a table or state slot: as is, or stochastically rounded

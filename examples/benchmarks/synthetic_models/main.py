@@ -26,6 +26,7 @@ import distributed_embeddings_b200 as de
 from distributed_embeddings_b200.models.configs import scaled, summary, synthetic_models_v3
 from distributed_embeddings_b200.models.synthetic import (InputGenerator, SyntheticModel,
                                                            SyntheticModelNative)
+from distributed_embeddings_b200.models.dense_optimizer import KINDS as DENSE_OPTIMIZERS
 from distributed_embeddings_b200.models.trainer import HybridTrainer
 from distributed_embeddings_b200.parallel.embedding_optimizers import NAMES as EMBEDDING_OPTIMIZERS
 
@@ -39,8 +40,12 @@ def main():
   p.add_argument("--dp_input", action="store_true")
   p.add_argument("--model", default="tiny", choices=sorted(synthetic_models_v3))
   p.add_argument("--optimizer", default="sgd", choices=EMBEDDING_OPTIMIZERS)
-  p.add_argument("--dense_optimizer", default="sgd", choices=["sgd", "adagrad", "adam"],
+  p.add_argument("--dense_optimizer", default="sgd", choices=list(DENSE_OPTIMIZERS),
                  help="optimizer of the MLP (--embedding_api de); the reference uses --optimizer's")
+  p.add_argument("--momentum", type=float, default=0.9,
+                 help="momentum of the 'momentum' optimizers (torch.optim.SGD's, dampening 0)")
+  p.add_argument("--nesterov", action="store_true",
+                 help="Nesterov momentum for the 'momentum' optimizers")
   p.add_argument("--column_slice_threshold", type=int, default=None)
   p.add_argument("--row_slice_threshold", type=int, default=None)
   p.add_argument("--data_parallel_threshold", type=int, default=None)
@@ -103,9 +108,13 @@ def main():
 
   if args.embedding_api == "de":
     lr = {"sgd": 0.03, "adagrad": 0.001, "rowwise_adagrad": 0.001, "adam": 0.001,
-          "rowwise_adam": 0.001, "ftrl": 0.01}[args.optimizer]
+          "rowwise_adam": 0.001, "ftrl": 0.01, "momentum": 0.01}[args.optimizer]
     opt_kwargs = {"state_dtype": {"fp32": torch.float32,
                                   "bf16": torch.bfloat16}[args.optimizer_state_dtype]}
+    momentum = {"momentum": args.momentum, "nesterov": args.nesterov}
+    if args.optimizer == "momentum":
+      opt_kwargs.update(momentum)
+    dense_kwargs = momentum if args.dense_optimizer == "momentum" else None
     from distributed_embeddings_b200.models.synthetic_fast import SyntheticTrainStep
     why = SyntheticTrainStep.unsupported_reason(model) if use_cuda else "needs CUDA"
     if args.trainer == "fast" and why:
@@ -114,12 +123,14 @@ def main():
       trainer = SyntheticTrainStep(model, lr=lr, embedding_optimizer=args.optimizer,
                                    use_cuda_graph=bool(args.cuda_graph),
                                    dense_optimizer=args.dense_optimizer,
+                                   dense_optimizer_kwargs=dense_kwargs,
                                    embedding_optimizer_kwargs=opt_kwargs)
       trainer_kind = "fast"
     else:
       trainer = HybridTrainer(model, lr=lr, embedding_optimizer=args.optimizer,
                               use_cuda_graph=bool(args.cuda_graph) and use_cuda,
                               dense_optimizer=args.dense_optimizer,
+                              dense_optimizer_kwargs=dense_kwargs,
                               embedding_optimizer_kwargs=opt_kwargs)
       trainer_kind = "autograd"
     step = lambda num, cat, lab: trainer.step(num, cat, lab)

@@ -23,6 +23,7 @@ import torch
 import torch.distributed as dist
 
 import distributed_embeddings_b200 as de
+from distributed_embeddings_b200.models.dense_optimizer import KINDS as DENSE_OPTIMIZERS
 from distributed_embeddings_b200.models.dlrm import DLRM, MLPERF_DCNV2_MULTI_HOT_SIZES
 from distributed_embeddings_b200.models.trainer import HybridTrainer
 from distributed_embeddings_b200.parallel.embedding_optimizers import NAMES as EMBEDDING_OPTIMIZERS
@@ -75,9 +76,17 @@ def parse():
   p.add_argument("--embedding_optimizer", default="sgd",
                  choices=EMBEDDING_OPTIMIZERS,
                  help="fused optimizer of the model-parallel tables")
+  p.add_argument("--dense_optimizer", default="sgd", choices=list(DENSE_OPTIMIZERS),
+                 help="optimizer of the MLPs (and of replicated tables, which need the embedding "
+                      "optimizer's kind)")
+  p.add_argument("--momentum", type=float, default=0.9,
+                 help="momentum of the 'momentum' optimizers (torch.optim.SGD's, dampening 0)")
+  p.add_argument("--nesterov", action="store_true",
+                 help="Nesterov momentum for the 'momentum' optimizers")
   p.add_argument("--optimizer_state_dtype", default="fp32", choices=["fp32", "bf16"],
-                 help="storage of the Adagrad / Adam / FTRL state (row-wise Adam: its m) of the "
-                      "model-parallel tables (bf16: half the memory, stochastically rounded)")
+                 help="storage of the Adagrad / Adam / FTRL / momentum state (row-wise Adam: its "
+                      "m) of the model-parallel tables (bf16: half the memory, stochastically "
+                      "rounded)")
   p.add_argument("--weight_decay", type=float, default=0.0,
                  help="weight decay of the embedding and the dense optimizer (rows a step "
                       "touched / every dense parameter)")
@@ -155,6 +164,11 @@ def main():
   fast = args.fast and cuda and args.dp_input
   opt_kwargs = {"state_dtype": STATE_DTYPES[args.optimizer_state_dtype]}
   dense_kwargs = {}
+  momentum = {"momentum": args.momentum, "nesterov": args.nesterov}
+  if args.embedding_optimizer == "momentum":
+    opt_kwargs.update(momentum)
+  if args.dense_optimizer == "momentum":
+    dense_kwargs.update(momentum)
   if args.weight_decay:
     decay = {"weight_decay": args.weight_decay, "weight_decay_mode": args.weight_decay_mode}
     opt_kwargs.update(decay)
@@ -167,6 +181,7 @@ def main():
     trainer = DLRMTrainStep(model, lr=args.learning_rate, scheduler=sched,
                             embedding_optimizer=args.embedding_optimizer,
                             embedding_optimizer_kwargs=opt_kwargs,
+                            dense_optimizer=args.dense_optimizer,
                             dense_optimizer_kwargs=dense_kwargs)
     if args.interaction == "dcnv2":  # list of [b, h_f] ids
       step = lambda n, c, l: trainer.step(n, [x.to(torch.int32) for x in c], l)
@@ -176,6 +191,7 @@ def main():
     trainer = HybridTrainer(model, lr=args.learning_rate, scheduler=sched,
                             embedding_optimizer=args.embedding_optimizer,
                             embedding_optimizer_kwargs=opt_kwargs,
+                            dense_optimizer=args.dense_optimizer,
                             dense_optimizer_kwargs=dense_kwargs)
     step = trainer.step
 

@@ -1,9 +1,10 @@
 #!/usr/bin/env python
 """fp32 versus bf16 optimizer state (Adagrad accumulator, Adam moments, row-wise Adam's m, FTRL's
-n and z) in the single-GPU DLRM training step.
+n and z, the momentum buffer) in the single-GPU DLRM training step.
 
   python tools/bench_state_dtype.py [--steps 30] [--warmup 5] [--repeats 3] [--loss-steps 40]
-                                    [--profile] [--optimizers adagrad,adam,rowwise_adam,ftrl]
+                                    [--profile]
+                                    [--optimizers sgd,adagrad,adam,rowwise_adam,ftrl,momentum]
 
 One invocation, one GPU, the MLPerf tables capped at ``--max-rows`` (default 20M:
 ``dlrm-mlperf-20m`` of ``bench.py``, whose id generator this uses), ``DLRMTrainStep`` (CUDA graph,
@@ -12,7 +13,9 @@ configurations fit one 80 GB card; ``--max-rows 5000000`` fits all of them:
 
 1. ``--optimizers`` (default Adagrad and Adam; ``rowwise_adam`` adds row-wise Adam, whose bf16
    state is its m: v stays one fp32 word per row; ``ftrl`` adds FTRL, two element-wise slots
-   like Adam) x {fp32, bf16} tables x {fp32, bf16} state,
+   like Adam; ``momentum`` adds momentum SGD, one element-wise slot like Adagrad; ``sgd`` adds
+   deterministic SGD, the sorted update without state, fp32 state only) x {fp32, bf16} tables x
+   {fp32, bf16} state,
    alternating, ``--repeats`` times
    each: device-timed ms per step (CUDA events around ``--steps`` graph replays; median and spread
    over the repeats), samples/s and ``torch.cuda.max_memory_allocated``.  A configuration whose
@@ -45,9 +48,12 @@ from bench import gen_ids  # noqa: E402
 from distributed_embeddings_b200.models.dlrm import mlperf_table_sizes  # noqa: E402
 
 _DTYPES = {"fp32": torch.float32, "bf16": torch.bfloat16}
-_SLOTS = {"adagrad": 1, "adam": 2, "rowwise_adam": 1, "ftrl": 2}   # element-wise state slots
-_ROW_SLOTS = {"adagrad": 0, "adam": 0, "rowwise_adam": 1, "ftrl": 0}  # fp32 words per row
-_LR = {"adagrad": 0.01, "adam": 0.0001, "rowwise_adam": 0.0001, "ftrl": 0.01}
+# element-wise state slots
+_SLOTS = {"sgd": 0, "adagrad": 1, "adam": 2, "rowwise_adam": 1, "ftrl": 2, "momentum": 1}
+# fp32 words per row
+_ROW_SLOTS = {"sgd": 0, "adagrad": 0, "adam": 0, "rowwise_adam": 1, "ftrl": 0, "momentum": 0}
+_LR = {"sgd": 0.1, "adagrad": 0.01, "adam": 0.0001, "rowwise_adam": 0.0001, "ftrl": 0.01,
+       "momentum": 0.01}
 _UPDATE_KERNELS = ("segment_update", "balanced_update", "finalize_crossing")
 DIM = 128
 
@@ -99,8 +105,10 @@ def run(cfg, args, pool, steps, mode="time"):
     torch.manual_seed(1234)
     model = DLRM(mlperf_table_sizes(args.max_rows), device=dev, compute_dtype=torch.bfloat16,
                  backend="fused", table_dtype=_DTYPES[tdt])
+    # SGD keeps no state: the sorted, deterministic update instead of the atomic scatter
+    kw = {"state_dtype": _DTYPES[sdt]} if _SLOTS[kind] else {"deterministic": True}
     trainer = DLRMTrainStep(model, lr=_LR[kind], embedding_optimizer=kind, use_cuda_graph=True,
-                            embedding_optimizer_kwargs={"state_dtype": _DTYPES[sdt]})
+                            embedding_optimizer_kwargs=kw)
     batches = [tuple(x.to(dev) for x in p) for p in pool]
     if mode == "loss":
       loss = None
@@ -154,7 +162,7 @@ def main():
   ap.add_argument("--max-rows", type=int, default=20_000_000)
   ap.add_argument("--profile", action="store_true")
   ap.add_argument("--optimizers", default="adagrad,adam",
-                  help="comma-separated subset of adagrad, adam, rowwise_adam, ftrl")
+                  help="comma-separated subset of " + ", ".join(_SLOTS))
   args = ap.parse_args()
   kinds = [k for k in args.optimizers.split(",") if k]
   if not kinds or any(k not in _SLOTS for k in kinds):
@@ -167,7 +175,8 @@ def main():
   out = {"gpu": gpu_info(), "max_rows": args.max_rows, "rows": sum(sizes),
          "global_batch": args.global_batch, "steps": args.steps, "card_gib": round(card_gib, 1)}
   pool = make_pool(sizes, args.global_batch)
-  cfgs = [(k, t, s) for k in kinds for t in ("fp32", "bf16") for s in ("fp32", "bf16")]
+  cfgs = [(k, t, s) for k in kinds for t in ("fp32", "bf16")
+          for s in (("fp32", "bf16") if _SLOTS[k] else ("fp32",))]
   planned = {c: planned_gib(sizes, *c) for c in cfgs}
   # tables and state alone must leave room for the step's buffers (a few GiB at batch 65536)
   runnable = [c for c in cfgs if planned[c] < card_gib - 6.0]
