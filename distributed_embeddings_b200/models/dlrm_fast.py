@@ -29,6 +29,7 @@ Same model/optimizer as the reference example (examples/dlrm/main.py:76-209): SG
 """
 from __future__ import annotations
 
+import copy
 import os
 from typing import Optional
 
@@ -40,7 +41,7 @@ from ..parallel.comm import CommContext
 from ..parallel.fused import FusedEngine
 from ..utils import nvtx
 from ..utils.lr_schedule import LearningRateScheduler
-from ..utils.metrics import BinnedAUC, auc_from_histogram
+from ..utils.metrics import BinnedAUC, ExactAUC, auc_from_counts, auc_from_histogram
 from .dense_optimizer import FlatDenseOptimizer, dense_optimizer_config
 from .dlrm import DLRM
 
@@ -117,7 +118,13 @@ class DLRMTrainStep:
                embedding_optimizer_kwargs: Optional[dict] = None, overlap: bool = True,
                gemm: str = "cublas", eval_thresholds: int = 8000, dense_optimizer: str = "sgd",
                dense_optimizer_kwargs: Optional[dict] = None, fused_table_update: bool = True,
-               fused_update_min_rows: int = FUSED_UPDATE_MIN_ROWS):
+               fused_update_min_rows: int = FUSED_UPDATE_MIN_ROWS, eval_auc: str = "binned",
+               eval_capacity: Optional[int] = None):
+    if eval_auc not in ("binned", "exact"):
+      raise ValueError("eval_auc must be 'binned' or 'exact'")
+    if eval_auc == "exact" and (eval_capacity is None or int(eval_capacity) < 1):
+      raise ValueError("eval_auc='exact' needs eval_capacity: the number of samples one rank "
+                       "evaluates between resets (4 bytes each)")
     if gemm not in ("cublas", "fused_dgrad", "tcgen05", "tcgen05_pair"):
       raise ValueError("gemm must be cublas | fused_dgrad | tcgen05 | tcgen05_pair")
     # Every value runs the data gradients below a ReLU on the first-party wgmma kernel with the
@@ -290,6 +297,9 @@ class DLRMTrainStep:
     self.eval_auc = BinnedAUC(eval_thresholds, device=dev)
     self._eval_loss = torch.zeros(1, dtype=torch.float64, device=dev)
     self._eval_count = torch.zeros(1, dtype=torch.int64, device=dev)
+    # eval_auc="exact": every evaluated sample's key, appended by auc_append in the eval graph
+    self.eval_auc_mode = eval_auc
+    self.exact_auc = ExactAUC(eval_capacity, device=dev) if eval_auc == "exact" else None
     self._eval_graph = None
 
   def _refresh_transposes(self):
@@ -732,6 +742,9 @@ class DLRMTrainStep:
       H = self.head
       self.ops.head_eval(self.top[-1].y, H.w16.view(-1), H.b16, self.lab_in, self._n_valid,
                          self._probs, self.eval_auc.hist, self._eval_loss, self._eval_count)
+      if self.exact_auc is not None:
+        self.ops.auc_append(self._probs, self.lab_in, self._n_valid, self.exact_auc.keys,
+                            self.exact_auc.state)
 
   def _eval_ready(self):
     if self._batch is None:
@@ -798,7 +811,8 @@ class DLRMTrainStep:
         out[s:s + m].copy_(self._probs[:m])
 
   def evaluate(self, numerical, categorical, labels):
-    """Accumulate the evaluation metrics (binned ROC AUC, log loss) over ``n >= 1`` local
+    """Accumulate the evaluation metrics (binned ROC AUC, log loss; with ``eval_auc="exact"``
+    also every sample's exact-AUC key, at most ``eval_capacity`` per rank) over ``n >= 1`` local
     samples: ``numerical [n, 13]``, ``categorical`` ``[n_features, n]`` or a list of ``[n]``
     (dcnv2 model: a list of ``[n, h_f]``), ``labels [n]``.  Nothing is copied to the host; read
     the result with :meth:`eval_metrics`."""
@@ -814,7 +828,12 @@ class DLRMTrainStep:
   def eval_metrics(self, reset: bool = True) -> dict:
     """``{"auc", "tie_bound", "log_loss", "samples"}`` over everything :meth:`evaluate` saw since
     the last reset, summed over all ranks (collective at world size > 1: one all-reduce).
-    ``tie_bound`` bounds ``|auc - exact AUC|`` (see ``utils.metrics.BinnedAUC``)."""
+    ``tie_bound`` bounds ``|auc - exact AUC|`` (see ``utils.metrics.BinnedAUC``).
+
+    ``eval_auc="exact"``: ``{"auc", "binned_auc", "tie_bound", "log_loss", "samples"}`` with the
+    exact ROC AUC of every rank's samples (``utils.metrics.ExactAUC``; at world size > 1 the keys
+    are all-gathered, so every rank returns the same value) and the binned one beside it.  Raises
+    when a rank evaluated more than ``eval_capacity`` samples or saw a NaN probability."""
     hist = self.eval_auc.hist.view(-1)
     packed = torch.cat([hist.double(), self._eval_loss, self._eval_count.double()])
     if self.world > 1:
@@ -824,9 +843,21 @@ class DLRMTrainStep:
     nb = hist.numel()
     res = auc_from_histogram(packed[:nb].round().long().view(2, -1))
     loss, count = float(packed[nb]), int(round(float(packed[nb + 1])))
+    exact = None
+    if self.exact_auc is not None:
+      m = self.exact_auc
+      if self.world > 1:
+        m = copy.copy(m)  # all_gather replaces the copy's buffers, not the graph's
+        m.all_gather(self.emb.group)
+      exact = auc_from_counts(*m.counts())
     if reset:
       self.eval_auc.reset()
       self._eval_loss.zero_()
       self._eval_count.zero_()
-    return {"auc": res.auc, "tie_bound": res.tie_bound,
-            "log_loss": loss / count if count else float("nan"), "samples": count}
+      if self.exact_auc is not None:
+        self.exact_auc.reset()
+    log_loss = loss / count if count else float("nan")
+    if exact is not None:
+      return {"auc": exact, "binned_auc": res.auc, "tie_bound": res.tie_bound,
+              "log_loss": log_loss, "samples": count}
+    return {"auc": res.auc, "tie_bound": res.tie_bound, "log_loss": log_loss, "samples": count}

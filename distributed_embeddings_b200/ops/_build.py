@@ -25,7 +25,7 @@ SO_PATH = os.path.join(PKG_DIR, "_C.so")
 
 CU_SOURCES = ["lookup_kernels.cu", "sparse_update_kernels.cu", "misc_kernels.cu", "comm_kernels.cu",
               "dense_kernels.cu", "gemm_wgmma.cu", "radix_sort.cu",
-              "offload_cache.cu"]
+              "offload_cache.cu", "eval_auc.cu"]
 CPP_SOURCES = ["bindings.cpp"]
 
 ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]

@@ -114,6 +114,7 @@ _KERNELS_PER_OP = {
     "gather_segments": 1, "gather_ragged": 1, "copy_cast_2d": 1, "dense_sgd": 1, "interact_fwd": 1, "interact_bwd": 1,
     "dense_adagrad": 1, "dense_adam": 1, "dense_momentum": 1, "cross_fwd": 1, "cross_bwd": 1, "cross_dx0": 1,
     "relu_bwd_bias": 1, "head_loss": 1, "head_eval": 1, "select_copy": 1, "cast_pad": 1, "gemm_tn_bias_act": 1, "gemm_dgrad_relu_bias": 1,
+    "auc_append": 1, "radix_sort_keys32": 12, "auc_count": 3,
 }
 _launches = 0
 

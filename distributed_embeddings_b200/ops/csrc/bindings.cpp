@@ -237,6 +237,29 @@ std::tuple<Tensor, Tensor> radix_sort_pairs32(const Tensor& keys, const Tensor& 
   return {out, where == 0 ? ia : ib};
 }
 
+// Sorts the first n int32 keys (read as unsigned, every key < 2^end_bit) in place; the ping-pong
+// buffer and the histograms are temporaries.
+void radix_sort_keys32(Tensor keys, int64_t n, int64_t end_bit) {
+  TORCH_CHECK(keys.is_cuda() && keys.scalar_type() == at::kInt && keys.is_contiguous(),
+              "keys must be a contiguous int32 CUDA tensor");
+  TORCH_CHECK(n >= 0 && n <= keys.numel(), "n must be in [0, keys.numel()]");
+  TORCH_CHECK(n < (int64_t(1) << 31), "own radix sort: too many items");
+  TORCH_CHECK(end_bit >= 1 && end_bit <= 32, "end_bit must be in [1, 32]");
+  if (n == 0) return;
+  c10::cuda::CUDAGuard guard(keys.device());
+  Tensor alt = at::empty({n}, keys.options());
+  Tensor temp = at::empty({static_cast<int64_t>(de::radix_sort_temp_bytes(n))},
+                          at::TensorOptions().device(keys.device()).dtype(at::kByte));
+  uint32_t* a = reinterpret_cast<uint32_t*>(keys.data_ptr<int>());
+  uint32_t* b = reinterpret_cast<uint32_t*>(alt.data_ptr<int>());
+  int where = de::radix_sort_keys32(temp.data_ptr(), a, b, n, static_cast<int>(end_bit),
+                                    cur_stream());
+  check_launch();
+  if (where == 1)
+    C10_CUDA_CHECK(cudaMemcpyAsync(a, b, static_cast<size_t>(n) * sizeof(uint32_t),
+                                   cudaMemcpyDeviceToDevice, cur_stream()));
+}
+
 std::tuple<Tensor, Tensor> head_segments(const Tensor& sorted_keys) {
   TORCH_CHECK(sorted_keys.is_cuda() && sorted_keys.scalar_type() == at::kLong &&
               sorted_keys.is_contiguous());
@@ -1111,6 +1134,52 @@ void head_eval(const Tensor& x, const Tensor& w, const Tensor& bias, const Tenso
   check_launch();
 }
 
+// Exact-AUC keys of rows below *n_valid appended at keys[state[0]:] (see de::launch_auc_append).
+void auc_append(const Tensor& probs, const Tensor& labels, const Tensor& n_valid, Tensor keys,
+                Tensor state) {
+  TORCH_CHECK(probs.is_cuda() && probs.scalar_type() == at::kFloat && probs.is_contiguous(),
+              "probs must be a contiguous fp32 CUDA tensor");
+  const auto dev = probs.device();
+  const int64_t batch = probs.numel();
+  TORCH_CHECK(labels.device() == dev && labels.scalar_type() == at::kFloat &&
+                  labels.is_contiguous() && labels.numel() == batch,
+              "labels must be a contiguous fp32 tensor with one value per row, on the device of "
+              "probs");
+  TORCH_CHECK(n_valid.device() == dev && n_valid.scalar_type() == at::kLong && n_valid.numel() == 1,
+              "n_valid must be one int64 word on the device of probs");
+  TORCH_CHECK(keys.device() == dev && keys.scalar_type() == at::kInt && keys.is_contiguous(),
+              "keys must be a contiguous int32 tensor on the device of probs");
+  TORCH_CHECK(state.device() == dev && state.scalar_type() == at::kLong &&
+                  state.is_contiguous() && state.numel() == 4,
+              "state must be 4 contiguous int64 words on the device of probs");
+  c10::cuda::CUDAGuard guard(dev);
+  de::launch_auc_append(probs.data_ptr<float>(), labels.data_ptr<float>(), batch,
+                        n_valid.data_ptr<int64_t>(),
+                        reinterpret_cast<uint32_t*>(keys.data_ptr<int>()), keys.numel(),
+                        state.data_ptr<int64_t>(), sm_count(), cur_stream());
+  check_launch();
+}
+
+// out = [P, N, U2] (int64) of the first n keys, sorted ascending (radix_sort_keys32)
+void auc_count(const Tensor& sorted_keys, int64_t n, Tensor out) {
+  TORCH_CHECK(sorted_keys.is_cuda() && sorted_keys.scalar_type() == at::kInt &&
+                  sorted_keys.is_contiguous(),
+              "sorted_keys must be a contiguous int32 CUDA tensor");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(sorted_keys.data_ptr()) % 16 == 0,
+              "sorted_keys must be 16-byte aligned");
+  TORCH_CHECK(n >= 0 && n <= sorted_keys.numel(), "n must be in [0, sorted_keys.numel()]");
+  TORCH_CHECK(n < (int64_t(1) << 31), "auc_count: too many keys");
+  TORCH_CHECK(out.device() == sorted_keys.device() && out.scalar_type() == at::kLong &&
+                  out.is_contiguous() && out.numel() == 3,
+              "out must be 3 contiguous int64 words on the device of sorted_keys");
+  c10::cuda::CUDAGuard guard(sorted_keys.device());
+  Tensor temp = at::empty({static_cast<int64_t>(std::max<size_t>(de::auc_count_temp_bytes(n), 1))},
+                          at::TensorOptions().device(sorted_keys.device()).dtype(at::kByte));
+  de::launch_auc_count(temp.data_ptr(), reinterpret_cast<const uint32_t*>(sorted_keys.data_ptr<int>()),
+                       n, out.data_ptr<int64_t>(), cur_stream());
+  check_launch();
+}
+
 // weight_decay_mode of the dense ops: 0 L2, 1 decoupled (see OptimizerArgs)
 void check_decay_mode(int64_t weight_decay_mode) {
   TORCH_CHECK(weight_decay_mode == de::kWeightDecayL2 ||
@@ -1488,6 +1557,7 @@ TORCH_LIBRARY(de_b200, m) {
         &radix_sort_pairs);
   m.def("radix_sort_pairs32(Tensor keys, Tensor items, int end_bit) -> (Tensor, Tensor)",
         &radix_sort_pairs32);
+  m.def("radix_sort_keys32(Tensor(a!) keys, int n, int end_bit) -> ()", &radix_sort_keys32);
   m.def("head_segments(Tensor sorted_keys) -> (Tensor, Tensor)", &head_segments);
   m.def(
       "segment_update(Tensor descs, Tensor tables, int n_tables, int batch, int grad_batch, "
@@ -1581,6 +1651,11 @@ TORCH_LIBRARY(de_b200, m) {
       "head_eval(Tensor x, Tensor w, Tensor bias, Tensor labels, Tensor n_valid, Tensor(a!) probs, "
       "Tensor(b!) hist, Tensor(c!) loss_sum, Tensor(d!) count) -> ()",
       &head_eval);
+  m.def(
+      "auc_append(Tensor probs, Tensor labels, Tensor n_valid, Tensor(a!) keys, Tensor(b!) state) "
+      "-> ()",
+      &auc_append);
+  m.def("auc_count(Tensor sorted_keys, int n, Tensor(a!) out) -> ()", &auc_count);
   m.def(
       "dense_sgd(Tensor(a!) p32, Tensor(b!) p16, Tensor(c!) g32, Tensor lr, float grad_scale, "
       "float weight_decay=0., int weight_decay_mode=0) -> ()",

@@ -173,6 +173,9 @@ int radix_sort_pairs(void* temp, int64_t* keys_a, uint32_t* items_a, int64_t* ke
 int radix_sort_pairs32(void* temp, uint32_t* keys_a, uint32_t* items_a, uint32_t* keys_b,
                        uint32_t* items_b, int64_t* keys_out64, int64_t n, int end_bit,
                        cudaStream_t stream);
+// keys only, sorted in place between keys_a and keys_b; returns 0 (sorted in a) or 1 (in b)
+int radix_sort_keys32(void* temp, uint32_t* keys_a, uint32_t* keys_b, int64_t n, int end_bit,
+                      cudaStream_t stream);
 size_t head_segments_temp_bytes(int64_t n);
 void head_segments(void* temp, const int64_t* sorted_keys, int64_t n, int64_t* seg_start,
                    int64_t* n_unique, cudaStream_t stream);
@@ -387,6 +390,17 @@ bool launch_head_loss(const void* x, int K, const void* w, const void* bias, con
 bool launch_head_eval(const void* x, int K, const void* w, const void* bias, const float* labels,
                       int64_t batch, const int64_t* n_valid, float* probs, int64_t* hist, int nb,
                       double* loss_sum, int64_t* count, int sm_count, cudaStream_t stream);
+// Exact ROC AUC of the evaluation (eval_auc.cu, utils/metrics.py ExactAUC).  auc_append: rows
+// below *n_valid become keys (bits(p) << 1 | label > 0.5) at keys[state[0] + i]; state (int64):
+// [0] keys stored, [1] rows dropped because they would pass `capacity`, [2] rows whose p is NaN
+// or outside [0, 1] (not stored), [3] block ticket, 0 between launches.
+void launch_auc_append(const float* probs, const float* labels, int64_t batch,
+                       const int64_t* n_valid, uint32_t* keys, int64_t capacity, int64_t* state,
+                       int sm_count, cudaStream_t stream);
+// auc_count: out = [P, N, U2] (int64) of n keys sorted ascending by radix_sort_keys32
+size_t auc_count_temp_bytes(int64_t n);
+void launch_auc_count(void* temp, const uint32_t* sorted_keys, int64_t n, int64_t* out,
+                      cudaStream_t stream);
 // weight_decay != 0: p32 -= lr * (grad_scale * g32 + weight_decay * p32) (both decay modes)
 void launch_sgd_update(float* p32, void* p16, float* g32, const float* lr_ptr, float grad_scale,
                        int64_t n, int sm_count, cudaStream_t stream, float weight_decay = 0.f);

@@ -105,8 +105,8 @@ __global__ void __launch_bounds__(kScanThreads)
 
 // KeyIn / KeyOut: int64 keys, or uint32 keys when every row key fits 32 bits (8 instead of 12
 // bytes per pair and pass); the last pass of a 32-bit sort widens to the int64 keys the update
-// kernels consume (KeyOut = int64_t).
-template <typename KeyIn, typename KeyOut>
+// kernels consume (KeyOut = int64_t).  kItems = false: keys only (items_in / items_out unused).
+template <typename KeyIn, typename KeyOut, bool kItems = true>
 __global__ void __launch_bounds__(kSortThreads)
     digit_scatter_kernel(const KeyIn* __restrict__ keys_in, const uint32_t* __restrict__ items_in,
                          KeyOut* __restrict__ keys_out, uint32_t* __restrict__ items_out,
@@ -133,7 +133,7 @@ __global__ void __launch_bounds__(kSortThreads)
     int64_t i = base + r * 32;
     bool valid = i < n;
     key[r] = valid ? keys_in[i] : 0;
-    item[r] = valid ? items_in[i] : 0u;
+    item[r] = kItems && valid ? items_in[i] : 0u;
   }
 #pragma unroll
   for (int r = 0; r < kRounds; ++r) {
@@ -168,7 +168,7 @@ __global__ void __launch_bounds__(kSortThreads)
       uint32_t d = static_cast<uint32_t>((key[r] >> shift) & (kBins - 1));
       uint32_t pos = warp_cnt[warp][d] + rank[r];
       keys_out[pos] = static_cast<KeyOut>(key[r]);
-      items_out[pos] = item[r];
+      if (kItems) items_out[pos] = item[r];
     }
   }
 }
@@ -323,6 +323,35 @@ int radix_sort_pairs32(void* temp, uint32_t* keys_a, uint32_t* items_a, uint32_t
     uint32_t* ti = iin;
     iin = iout;
     iout = ti;
+    where ^= 1;
+  }
+  return where;
+}
+
+// Keys only (every key < 2^32): the passes of radix_sort_pairs32 without items, ping-pong
+// between keys_a and keys_b (both clobbered).  Returns 0 when the sorted keys end in keys_a, 1
+// when they end in keys_b.
+int radix_sort_keys32(void* temp, uint32_t* keys_a, uint32_t* keys_b, int64_t n, int end_bit,
+                      cudaStream_t stream) {
+  if (n <= 0) return 0;
+  const int64_t n_tiles = tiles_of(n);
+  uint32_t* hist = static_cast<uint32_t*>(temp);
+  uint32_t* total = reinterpret_cast<uint32_t*>(
+      static_cast<char*>(temp) + align256(static_cast<size_t>(n_tiles) * kBins * sizeof(uint32_t)));
+  uint32_t *kin = keys_a, *kout = keys_b;
+  int where = 0;
+  if (end_bit < 1) end_bit = 1;
+  if (end_bit > 32) end_bit = 32;
+  for (int shift = 0; shift < end_bit; shift += 8) {
+    digit_hist_kernel<uint32_t><<<static_cast<unsigned>(n_tiles), kSortThreads, 0, stream>>>(
+        kin, n, shift, n_tiles, hist);
+    digit_scan_kernel<<<kBins, kScanThreads, 0, stream>>>(hist, n_tiles, total);
+    digit_scatter_kernel<uint32_t, uint32_t, false><<<static_cast<unsigned>(n_tiles),
+                                                      kSortThreads, 0, stream>>>(
+        kin, nullptr, kout, nullptr, n, shift, n_tiles, hist, total);
+    uint32_t* tk = kin;
+    kin = kout;
+    kout = tk;
     where ^= 1;
   }
   return where;

@@ -101,6 +101,153 @@ class BinnedAUC:
     return auc_from_histogram(self.hist)
 
 
+def auc_keys(probs, labels) -> np.ndarray:
+  """Exact-AUC keys ``(bits(p) << 1) | (y > 0.5)`` (uint32, below 2^31) of fp32 probabilities in
+  [0, 1]; -0.0 is keyed as 0.0.  Raises on a probability that is NaN or outside [0, 1]."""
+  p = np.ascontiguousarray(np.asarray(torch.as_tensor(probs).detach().cpu().float()).reshape(-1))
+  y = np.asarray(torch.as_tensor(labels).detach().cpu().float()).reshape(-1)
+  if p.size != y.size:
+    raise ValueError("probs and labels must have the same number of elements")
+  bad = int(np.count_nonzero(~((p >= 0) & (p <= 1))))
+  if bad:
+    raise ValueError(f"{bad} probabilities are NaN or outside [0, 1]")
+  bits = p.view(np.uint32) & np.uint32(0x7FFFFFFF)
+  return (bits << np.uint32(1)) | (y > 0.5).astype(np.uint32)
+
+
+def auc_counts_from_keys(keys) -> tuple:
+  """``(P, N, U2)`` of exact-AUC keys (any order), with numpy integers: ``U2`` is twice the
+  Mann-Whitney U of the positives' scores over the negatives' (ties count one half),
+  ``sum over positives j of 2 #{neg: p < p_j} + #{neg: p == p_j}``."""
+  k = np.sort(np.asarray(keys).astype(np.uint32).reshape(-1))
+  n = k.size
+  if n == 0:
+    return 0, 0, 0
+  neg = (1 - (k & 1)).astype(np.int64)
+  np_before = np.cumsum(neg) - neg  # negatives before each position: score <= its own
+  score = k >> 1
+  head = np.ones(n, dtype=bool)
+  head[1:] = score[1:] != score[:-1]
+  run_start = np.maximum.accumulate(np.where(head, np.arange(n), 0))
+  pos = neg == 0
+  # negatives before the score run: score strictly below
+  u2 = int(np_before[pos].sum()) + int(np_before[run_start[pos]].sum())
+  n_neg = int(neg.sum())
+  return n - n_neg, n_neg, u2
+
+
+def auc_from_counts(n_pos: int, n_neg: int, u2: int) -> float:
+  """``U2 / (2 P N)`` in float64; NaN when a class is empty."""
+  if n_pos == 0 or n_neg == 0:
+    return float("nan")
+  return u2 / (2 * n_pos * n_neg)
+
+
+class ExactAUC:
+  """Exact ROC AUC (Mann-Whitney, ties count one half) over every sample since the last reset,
+  accumulated without floating-point sums: each sample is kept as one 31-bit key (4 bytes, see
+  :func:`auc_keys`) in a ``capacity``-key buffer, and :meth:`counts` sorts the keys and counts
+  ``(P, N, U2)`` in 64-bit integers.  The value equals :func:`binary_auc`.
+
+  On CUDA, :meth:`update` is one ``auc_append`` kernel with the sample count and every offset on
+  the device (it replays inside a CUDA graph), and :meth:`counts` runs the first-party radix sort
+  and ``auc_count``; they need ``4 * n`` bytes of temporary space for ``n`` keys.  On CPU the same
+  integers come from a numpy sort (the reference the kernels are tested against).
+
+  ``state`` (int64): ``[keys stored, samples dropped because they would pass capacity, samples
+  whose probability is NaN or outside [0, 1], kernel ticket]``.  Overflow drops the whole update
+  (nothing is written past the buffer) and a bad probability is not stored; either makes
+  :meth:`counts` and :meth:`result` raise until :meth:`reset`."""
+
+  def __init__(self, capacity: int, device=None):
+    if int(capacity) < 1:
+      raise ValueError("capacity must be >= 1")
+    self.capacity = int(capacity)
+    self.keys = torch.zeros(self.capacity, dtype=torch.int32, device=device)
+    self.state = torch.zeros(4, dtype=torch.int64, device=device)
+
+  def update(self, probs: torch.Tensor, labels: torch.Tensor, n_valid=None):
+    """Append the first ``n_valid`` (default all) predictions in [0, 1] and their labels.  On
+    CUDA ``n_valid`` may be an int64 device word, read by the kernel."""
+    p = probs.reshape(-1)
+    y = labels.reshape(-1)
+    if p.numel() != y.numel():
+      raise ValueError("probs and labels must have the same number of elements")
+    if self.keys.is_cuda:
+      from ..ops import _native
+      if not isinstance(n_valid, torch.Tensor):
+        n = p.numel() if n_valid is None else int(n_valid)
+        n_valid = torch.full((1,), n, dtype=torch.int64, device=self.keys.device)
+      _native.require().auc_append(p.float().contiguous(), y.float().contiguous(), n_valid,
+                                   self.keys, self.state)
+      return
+    n = p.numel() if n_valid is None else int(n_valid)
+    n = max(0, min(n, p.numel()))
+    p, y = p[:n].float().numpy(), y[:n].float().numpy()
+    ok = (p >= 0) & (p <= 1)
+    self.state[2] += int(np.count_nonzero(~ok))
+    count = int(self.state[0])
+    if count + n > self.capacity:
+      self.state[1] += n
+      return
+    keys = auc_keys(np.where(ok, p, 0).astype(np.float32), y)
+    self.keys[count:count + n] = torch.from_numpy(keys.view(np.int32))
+    self.state[0] = count + n
+
+  def reset(self):
+    self.state.zero_()
+
+  def all_gather(self, group=None):
+    """Collective: afterwards every rank of ``group`` holds every rank's keys (counts may differ
+    between ranks) and the summed dropped / bad counts.  The buffers are replaced by new ones of
+    ``max(capacity, total keys)`` keys, so a CUDA graph that appends to the old ones no longer
+    reaches this object."""
+    import torch.distributed as dist
+    world = dist.get_world_size(group)
+    st = self.state[:3].clone()
+    states = [torch.empty_like(st) for _ in range(world)]
+    dist.all_gather(states, st, group=group)
+    states = torch.stack(states).cpu()
+    counts = [int(c) for c in states[:, 0]]
+    width = max(max(counts), 1)
+    send = torch.zeros(width, dtype=torch.int32, device=self.keys.device)
+    send[:counts[dist.get_rank(group)]] = self.keys[:counts[dist.get_rank(group)]]
+    recv = [torch.empty_like(send) for _ in range(world)]
+    dist.all_gather(recv, send, group=group)
+    total = sum(counts)
+    self.capacity = max(self.capacity, total)
+    keys = torch.zeros(self.capacity, dtype=torch.int32, device=self.keys.device)
+    keys[:total] = torch.cat([r[:c] for r, c in zip(recv, counts)])
+    state = torch.zeros(4, dtype=torch.int64, device=self.state.device)
+    state[:3] = states.sum(0).to(state.device)
+    self.keys, self.state = keys, state
+
+  def counts(self) -> tuple:
+    """``(P, N, U2)`` over the stored keys (host ints).  Raises when samples were dropped for
+    lack of capacity or a probability was NaN or outside [0, 1]."""
+    stored, dropped, bad = (int(v) for v in self.state[:3].tolist())
+    if dropped:
+      raise RuntimeError(
+          f"ExactAUC overflow: {stored + dropped} samples were evaluated but the key buffer holds "
+          f"{self.capacity}; {dropped} were not stored (raise the capacity)")
+    if bad:
+      raise RuntimeError(
+          f"ExactAUC: {bad} of {stored + dropped} probabilities were NaN or outside [0, 1] "
+          f"(capacity {self.capacity})")
+    if not self.keys.is_cuda:
+      return auc_counts_from_keys(self.keys[:stored].numpy())
+    from ..ops import _native
+    ops = _native.require()
+    out = torch.zeros(3, dtype=torch.int64, device=self.keys.device)
+    ops.radix_sort_keys32(self.keys, stored, 31)  # in place: the order of the keys is free
+    ops.auc_count(self.keys, stored, out)
+    return tuple(int(v) for v in out.tolist())
+
+  def result(self) -> float:
+    """Exact ROC AUC in float64 (NaN when a class is empty)."""
+    return auc_from_counts(*self.counts())
+
+
 class MetricsLogger:
   """Structured (JSON lines) metrics: one record per call, rank-0 only by default."""
 

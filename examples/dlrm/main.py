@@ -64,6 +64,10 @@ def parse():
                       "the eval split on the GPU (binned AUC, log loss); 0 = off")
   p.add_argument("--eval_batches", type=int, default=8,
                  help="eval batches per periodic evaluation (--eval_interval)")
+  p.add_argument("--eval_auc", choices=("binned", "exact"), default="binned",
+                 help="with --eval_interval: binned = 8000-threshold ROC AUC (the reference's "
+                      "metric); exact = exact ROC AUC from sorted keys on the GPU (4 bytes per "
+                      "eval sample), with the binned value beside it")
   p.add_argument("--amp", action="store_true", default=True)
   p.add_argument("--gpu_embedding_size", type=int, default=None,
                  help="per-rank HBM element budget of the tables; the largest beyond it live in "
@@ -182,7 +186,9 @@ def main():
                             embedding_optimizer=args.embedding_optimizer,
                             embedding_optimizer_kwargs=opt_kwargs,
                             dense_optimizer=args.dense_optimizer,
-                            dense_optimizer_kwargs=dense_kwargs)
+                            dense_optimizer_kwargs=dense_kwargs, eval_auc=args.eval_auc,
+                            eval_capacity=(args.eval_batches * args.batch_size
+                                           if args.eval_auc == "exact" else None))
     if args.interaction == "dcnv2":  # list of [b, h_f] ids
       step = lambda n, c, l: trainer.step(n, [x.to(torch.int32) for x in c], l)
     else:
@@ -200,7 +206,8 @@ def main():
       yield from train
 
   def periodic_eval(i):
-    """Binned AUC (8000 thresholds, as the reference reports) and log loss on the GPU."""
+    """Binned AUC (8000 thresholds, as the reference reports; --eval_auc exact: the exact AUC)
+    and log loss on the GPU."""
     for k, (num, cat, lab) in enumerate(evald):
       if k >= args.eval_batches:
         break
@@ -213,7 +220,8 @@ def main():
                        torch.stack([c.reshape(-1) for c in ids]), lab.to(device).float())
     m = trainer.eval_metrics()  # collective
     if rank == 0:
-      print(f"eval step: {i} AUC: {m['auc']:.6f} tie_bound: {m['tie_bound']:.2e} "
+      binned = f" binned_AUC: {m['binned_auc']:.6f}" if "binned_auc" in m else ""
+      print(f"eval step: {i} AUC: {m['auc']:.6f}{binned} tie_bound: {m['tie_bound']:.2e} "
             f"log_loss: {m['log_loss']:.6f}", flush=True)
 
   for i, (num, cat, lab) in enumerate(batches()):
